@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the two WaveNet hot paths on B200, with roofline and the CPU baseline beside it.
+"""bench.py -- throughput of the two WaveNet hot paths on H100, with roofline and the CPU baseline beside it.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload all|generate|train]
+                    [--dump-outputs DIR]
 
 Under torchrun (N>1) every rank runs; rank 0 prints ONE JSON line.
 
@@ -13,6 +14,8 @@ L=16000, output_length=10885), batch-sharded over the ranks (weak scaling; the f
 
 `value` is device-timed with inputs resident in HBM; `e2e` goes through the reference-facing Python API with host
 buffers.  `cpu_baseline` / `--impl reference` time the CPU port of the reference (oracle/) on the host cores.
+--dump-outputs DIR writes what the timed paths computed in their last timed step as DIR/<name>.npy (float32), from
+seeded inputs, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -50,19 +53,7 @@ def measured_peaks(what="hbm"):
         if what == "tensor":
             return float(d["bf16_tflops_sustained"]), "measured sustained cuBLAS bf16 (MEASURED_PEAKS.json)"
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return (1400.0 if what == "tensor" else 6650.0), "fallback (B200_PROFILING.md)"
-
-
-def captured_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed `ncu --set full` capture
-    (profiles/traffic.json, written by tools/ncu_summary.py traffic ...); None when there is no capture of it."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if not os.path.exists(path):
-        return None, None
-    with open(path) as f:
-        d = json.load(f)
-    e = d.get(kernel)
-    return (e["dram_bytes_per_launch"], e["source"]) if e else (None, None)
+    return (989.0 if what == "tensor" else 3350.0), "H100 SXM data sheet (dense bf16, HBM3), not a measured figure"
 
 
 class ClockSampler:
@@ -140,6 +131,14 @@ def max_over_ranks(x, world):
     return float(t.item())
 
 
+def grad_sample(model, n=1 << 20, seed=0):
+    """A fixed, seeded sample of n entries of all parameter gradients (parameters in definition order, flattened)."""
+    g = torch.cat([p.grad.reshape(-1) if p.grad is not None else torch.zeros(p.numel(), device=p.device)
+                   for p in model.parameters()])
+    idx = np.sort(np.random.default_rng(seed).choice(g.numel(), min(n, g.numel()), replace=False))
+    return g[torch.from_numpy(idx).to(g.device)].float().cpu().numpy()
+
+
 def build_model(kw, seed=0):
     import wavenet_model as wmod
     torch.manual_seed(seed)
@@ -187,6 +186,7 @@ def bench_generate(args, world, rank):
     barrier_sync(world)
     t_wall = time.perf_counter() - t_wall0
     clk = clocks.stop()
+    dump = {"generate_indices": out.cpu().numpy().astype(np.float32)}      # last timed step, (streams, samples)
     ms = sum(a.elapsed_time(b) for a, b in evs)
     ms = max_over_ranks(ms, world)
     value = world * NS * n * args.steps / (ms / 1e3)
@@ -195,7 +195,7 @@ def bench_generate(args, world, rank):
     model.generate_fast(256, temperature=TEMPERATURE)                     # warm
     barrier_sync(world)
     t0 = time.perf_counter()
-    e2e_steps = max(1, min(args.steps, 3))
+    e2e_steps = args.steps
     for _ in range(e2e_steps):
         audio = model.generate_fast(n, temperature=TEMPERATURE)
     torch.cuda.synchronize()
@@ -208,7 +208,7 @@ def bench_generate(args, world, rank):
     import ctypes, native
     # argmax path, for reference
     t_arg = []
-    for _ in range(2):
+    for _ in range(args.steps):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         rt.generate_resident(s, first, 1, n, 0.0, 0.0, out)
@@ -226,7 +226,7 @@ def bench_generate(args, world, rank):
         out_b = torch.zeros(NB, nb, dtype=torch.int32, device=dev)
         rt.generate_resident(sb, first_b, 1, 64, TEMPERATURE, 0.0, out_b[:, :64].contiguous(), d_uni=uni_b[:, :64].contiguous())
         tb = []
-        for _ in range(2):
+        for _ in range(args.steps):
             flush()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
@@ -246,7 +246,7 @@ def bench_generate(args, world, rank):
         out_b = torch.zeros(NB, nb, dtype=torch.int32, device=dev)
         rt.generate_resident(sb, first_b, 1, 64, TEMPERATURE, 0.0, out_b[:, :64].contiguous(), d_uni=uni_b[:, :64].contiguous())
         tb = []
-        for _ in range(2):
+        for _ in range(args.steps):
             flush()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
@@ -255,9 +255,10 @@ def bench_generate(args, world, rank):
             torch.cuda.synchronize()
             tb.append(e0.elapsed_time(e1))
         tbm = max_over_ranks(min(tb), world)
+        dump["generate_64_streams_indices"] = out_b.cpu().numpy().astype(np.float32)   # last timed launch, (64, 1000)
         gb_, bb_, _bars = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         native.lib().wn_gen_launch_info(sb["handle"], ctypes.byref(gb_), ctypes.byref(bb_), ctypes.byref(_bars))
-        # the same kernel where its 16-CTA clusters are all co-resident (7 x 8 streams) and at the 8-CTA variant's capacity
+        # the same kernel at two more stream counts (56 and 120 streams: 7 and 15 clusters of 8 streams)
         t56, g56, _ = run_streams(56, nb)
         t120, g120, _ = run_streams(120, nb)
         other = {"56_streams": {"value": world * 56 * nb / (t56 / 1e3), "us_per_step": t56 * 1e3 / nb, "grid": g56},
@@ -279,13 +280,12 @@ def bench_generate(args, world, rank):
     alg_bytes = n * (weight_bytes + 50 * 3 * 256 * 4)
     kid = native.lib().wn_gen_kernel_id(s["handle"])
     kname = {6: "gen_kernel_cl8", 3: "gen_kernel_fast", 4: "gen_kernel_cluster", 2: "gen_kernel_ll", 1: "gen_kernel", 5: "gen_kernel_x2"}[kid]
-    traffic, tsrc = captured_traffic(kname)
     sm_mhz = clk.get("sm_mhz") or 1965.0
     macs = sum(p.numel() for p in model.parameters()) - 256 * 256      # start conv is a gather
-    issue_peak = 148 * 128 * sm_mhz * 1e6                               # FMA lanes per second at the clock seen
+    issue_peak = torch.cuda.get_device_properties(0).multi_processor_count * 128 * sm_mhz * 1e6   # FMA lanes per second at the clock seen
     roof = {"kernel": kname, "bound": "hbm", "achieved": alg_bytes / (per_launch_ms / 1e3) / 1e9, "peak": peak,
             "unit": "GB/s", "frac": alg_bytes / (per_launch_ms / 1e3) / 1e9 / peak,
-            "traffic": None if traffic is None else traffic, "traffic_source": tsrc, "peak_source": peak_src,
+            "peak_source": peak_src,
             "us_per_sample": per_launch_ms * 1e3 / n, "exchange_stages_per_sample": bars.value,
             "us_per_exchange_stage": per_launch_ms * 1e3 / n / bars.value, "grid": g.value, "block": b.value,
             "issue": {"fma_per_sample": macs, "achieved_gfma_s": macs * n / (per_launch_ms / 1e3) / 1e9,
@@ -293,7 +293,7 @@ def bench_generate(args, world, rank):
     gen_dtype = ("bf16 hi/lo operand pairs, 3 MMAs per product, f32 accumulate (f32-class: logits within 2e-5 of the f32 "
                  "kernels, 1e-4 of the reference)") if kid == 6 else "f32"
     return dict(value=value, dtype=gen_dtype, ms_per_step=ms / args.steps, clocks=clk, e2e=e2e, roofline=roof,
-                argmax_samples_per_s=n / (min(t_arg) / 1e3), wall_s=t_wall, launches=args.steps, batched=batched)
+                argmax_samples_per_s=n / (min(t_arg) / 1e3), wall_s=t_wall, launches=args.steps, batched=batched, dump=dump)
 
 
 # ------------------------------------------------------------------------------------------------ training forward
@@ -343,6 +343,10 @@ def bench_train(args, world, rank):
         rt.block_events = None
         barrier_sync(world)
         clk = clocks.stop()
+        # a fixed, seeded sample of 4096 rows of the last timed forward's logits (the whole tensor is 89 MB)
+        rows = np.sort(np.random.default_rng(0).choice(y.shape[0], 4096, replace=False))
+        dump = {"train_forward_logits_sample": y[torch.from_numpy(rows).to(y.device)].float().cpu().numpy(),
+                "train_forward_sample_rows": rows.astype(np.float64)}
         fwd_mode = getattr(rt, "last_block_mode", "ffma")
         ms = max_over_ranks(sum(a.elapsed_time(b) for a, b in evs), world)
         block_ms = sum(a.elapsed_time(b) for a, b in bevs) / args.steps
@@ -354,7 +358,7 @@ def bench_train(args, world, rank):
         model(x_host.cuda(non_blocking=True))
         barrier_sync(world)
         t0 = time.perf_counter()
-        e2e_steps = max(1, min(args.steps, 3))
+        e2e_steps = args.steps
         for _ in range(e2e_steps):
             y = model(x_host.cuda(non_blocking=True))
             y_host.copy_(y, non_blocking=True)
@@ -382,7 +386,7 @@ def bench_train(args, world, rank):
             for _ in range(2):
                 y_fast = model.forward_indices(d_idx)
             fe = []
-            for _ in range(max(1, min(args.steps, 3))):
+            for _ in range(args.steps):
                 flush()
                 b0, b1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 rt.block_events = (b0, b1)
@@ -408,7 +412,7 @@ def bench_train(args, world, rank):
             for _ in range(2):
                 y_other = model.forward_indices(d_idx)
             oe = []
-            for _ in range(max(1, min(args.steps, 3))):
+            for _ in range(args.steps):
                 flush()
                 b0, b1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 rt.block_events = (b0, b1)
@@ -427,7 +431,7 @@ def bench_train(args, world, rank):
     red = dp.make_data_parallel(model)
     target = torch.randint(0, 256, (B * model.output_length,), generator=torch.Generator().manual_seed(99 + rank)).cuda()
     step_ms = []
-    for i in range(1 + max(1, min(args.steps, 3))):
+    for i in range(1 + args.steps):
         model.zero_grad(set_to_none=True)
         barrier_sync(world)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -444,6 +448,7 @@ def bench_train(args, world, rank):
                   "grad_buckets_per_step": red.buckets // max(1, 1 + len(step_ms)) if world > 1 else 0,
                   "forward_blocks": getattr(rt, "last_block_mode", "ffma"), "backward_data": getattr(rt, "last_bwd_mode", "ffma"),
                   "scaling": "weak (B=8 per GPU)"}
+    dump["train_step_grad_sample"] = grad_sample(model)                # gradients of the last timed step
     del loss
     model.zero_grad(set_to_none=True)
     if world > 1 and B % world == 0:
@@ -495,10 +500,9 @@ def bench_train(args, world, rank):
     mode = fwd_mode
     if mode == "tb":
         tpeak, tsrc = measured_peaks("tensor")
-        traffic, trsrc = captured_traffic("block_fused_kernel")
-        roof = {"kernel": "block_fused_kernel (tcgen05 cta_group::2, bf16 hi/lo pairs; all blocks in one persistent launch)",
+        roof = {"kernel": "block_fused_kernel (wgmma, bf16 hi/lo pairs; all blocks in one persistent launch)",
                 "bound": "tensor", "achieved": tflops, "peak": tpeak, "unit": "TFLOP/s", "frac": tflops / tpeak,
-                "traffic": traffic, "traffic_source": trsrc, "peak_source": tsrc,
+                "peak_source": tsrc,
                 "launches_per_step": getattr(rt, "last_block_launches", n_layers),
                 "avg_block_ms": block_ms / n_layers, "operand_split": "bf16x2",
                 "mma_per_product": 3, "tensor_pipe_equiv_frac": 3 * tflops / tpeak,
@@ -509,14 +513,11 @@ def bench_train(args, world, rank):
         tpeak, tsrc = measured_peaks("tensor")
         prec = getattr(rt, "tc_precision", "tf32x3")
         mma_per_flop = 3 if prec == "bf16x2" else 6          # bf16-rate MMA equivalents per algorithmic FLOP
-        roof = {"kernel": "frames_gemm_tc<GATE> + frames_gemm_tc<RES_SKIP> (tcgen05, " +
-                          ("kind::f16 on bf16 hi/lo pairs" if prec == "bf16x2" else "kind::tf32, 3xTF32") + ", one block = 2 launches)",
+        roof = {"kernel": "frames_gemm_tc<GATE> + frames_gemm_tc<RES_SKIP> (wgmma, " +
+                          ("bf16 hi/lo pairs" if prec == "bf16x2" else "tf32, 3xTF32") + ", one block = 2 launches)",
                 "bound": "tensor", "achieved": tflops, "peak": tpeak, "unit": "TFLOP/s", "frac": tflops / tpeak,
-                # dram__bytes_read+write of the two launches of one block from the ncu --set full capture
-                # profiles/prof_tc_block_r1_e.txt (layer of the cfg-3 forward, 3xTF32 variant: same activation traffic)
-                "traffic": 128.15e6 + 85.84e6 + 363.67e6 + 189.49e6,
-                "traffic_note": "per block (2 launches), ncu capture profiles/prof_tc_block_r1_e.txt; 1.67x the algorithmic "
-                                "bytes because z is written by the first launch and read back by the second",
+                "traffic": None,
+                "traffic_note": "z is written by the first launch of a block and read back by the second",
                 "peak_source": tsrc, "launches_per_step": 2 * n_layers,
                 "avg_block_ms": block_ms / n_layers, "operand_split": prec,
                 "note": "achieved counts the algorithmic fp32 FLOPs once; fp32-class accuracy costs three MMAs per product "
@@ -543,7 +544,7 @@ def bench_train(args, world, rank):
                                     "uint8 index input resident in HBM", "block_kernels": mode, "global_batch": world * B, "seq_len": L,
                         "l2": "256 MiB buffer written between timed iterations (L2 flush)",
                         "parallelism": f"dp{world} (batch shards, no collective in forward)"},
-                launches=args.steps * rt.launches_last_forward)
+                launches=args.steps * rt.launches_last_forward, dump=dump)
 
 
 # ------------------------------------------------------------------------------------------------ cfg 5: deep 512-channel stack, bf16
@@ -564,7 +565,7 @@ def bench_train_cfg5(args, world, rank):
     idx = torch.randint(0, 256, (1, L), generator=torch.Generator().manual_seed(4321 + rank)).to(torch.uint8).cuda()
     target = torch.randint(0, 256, (model.output_length,), generator=torch.Generator().manual_seed(55 + rank)).cuda()
     flush = L2Flush()
-    n = max(1, min(args.steps, 3))
+    n = args.steps
     with torch.no_grad():
         for _ in range(2):
             model.forward_indices(idx)
@@ -576,7 +577,7 @@ def bench_train_cfg5(args, world, rank):
             b0, b1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             rt.block_events = (b0, b1)
             e0.record()
-            model.forward_indices(idx)
+            y5 = model.forward_indices(idx)
             e1.record()
             evs.append((e0, e1)); bevs.append((b0, b1))
         rt.block_events = None
@@ -597,6 +598,9 @@ def bench_train_cfg5(args, world, rank):
         if i > 0:
             step_ms.append(e0.elapsed_time(e1))
     step_t = max_over_ranks(sum(step_ms) / len(step_ms), world)
+    rows = np.sort(np.random.default_rng(0).choice(y5.shape[0], 2048, replace=False))
+    dump = {"cfg5_forward_logits_sample": y5[torch.from_numpy(rows).to(y5.device)].float().cpu().numpy(),
+            "cfg5_forward_sample_rows": rows.astype(np.float64), "cfg5_step_grad_sample": grad_sample(model)}
     per_layer, start_b, head_b, flops = train_alg_bytes(model, 1, L, dense_input=False)
     tpeak, tsrc = measured_peaks("tensor")
     hpeak, _ = measured_peaks()
@@ -610,7 +614,7 @@ def bench_train_cfg5(args, world, rank):
            "roofline": {"kernel": "block_fused_kernel<512, single-pass bf16>", "bound": "tensor", "achieved": tflops, "peak": tpeak,
                         "unit": "TFLOP/s", "frac": tflops / tpeak, "peak_source": tsrc, "avg_block_ms": block_ms / len(per_layer),
                         "hbm_frac": (sum(per_layer) / (block_ms / 1e3) / 1e9) / hpeak, "traffic": None},
-           "parameters": model.parameter_count(), "scaling": "weak"}
+           "parameters": model.parameter_count(), "scaling": "weak", "dump": dump}
     del loss
     return out
 
@@ -710,11 +714,12 @@ def main():
     ap.add_argument("--no-batched", action="store_true", help="skip the 64-stream (cfg4) generation figure")
     ap.add_argument("--no-cfg5", action="store_true", help="skip the 512-channel bf16 deep-stack figures (cfg 5)")
     ap.add_argument("--variants", action="store_true", help="also time the other operand splits of the two-launch blocks")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback); use --impl reference for the CPU arm")
+        raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback); use --impl reference for the CPU arm")
     world, rank, _ = dist_setup(args.gpus)
     gen = bench_generate(args, world, rank) if args.workload in ("all", "generate") else None
     train = bench_train(args, world, rank) if args.workload in ("all", "train") else None
@@ -743,6 +748,13 @@ def main():
             train["cpu_baseline"] = {"value": res[best], "unit": "frames/s", "cores": best, "kind": "port",
                                      "sample": "one no_grad forward of B=1, L=16000 one-hot input per thread setting (best kept): "
                                                + ", ".join(f"{k} threads: {v:.0f} frames/s" for k, v in res.items())}
+    if rank == 0 and args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for part in (gen, train, cfg5):
+            for name, arr in (part or {}).pop("dump", {}).items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
+    for part in (gen, train, cfg5):
+        (part or {}).pop("dump", None)
     if rank == 0:
         primary = gen if gen is not None else train
         line = {

@@ -1,4 +1,4 @@
-/* wavenet_b200.h -- C ABI of libwavenet_b200.so (sm_100a).
+/* wavenet_b200.h -- C ABI of libwavenet_b200.so (sm_90a, H100).
  *
  * Drop-in boundary for the two hot paths of vincentherrmann/pytorch-wavenet:
  *   (T) the training-time dilated causal convolution stack  WaveNetModel.forward / .wavenet
@@ -38,7 +38,7 @@ extern "C" {
 
 #define WN_E_BADARG   (-1)   /* null pointer / non-positive size / inconsistent shapes        */
 #define WN_E_UNSUPP   (-2)   /* shape outside what the kernels cover (message says which)     */
-#define WN_E_NODEVICE (-3)   /* no sm_100 device visible                                      */
+#define WN_E_NODEVICE (-3)   /* no sm_90 device visible                                       */
 #define WN_E_STATE    (-4)   /* sampler handle used before wn_gen_bind / after destroy        */
 
 /* ---------------------------------------------------------------- library / device */
@@ -98,7 +98,7 @@ typedef struct wn_block_args {
 int wn_block_fwd(const wn_block_args* a, void* stream);
 
 /* ---------------------------------------------------------------- (T) the same block on the tensor cores
- * tcgen05.mma kind::tf32 with 3xTF32 operand splitting (hi*hi + lo*hi + hi*lo, fp32 accumulation in tensor memory):
+ * wgmma tf32 with 3xTF32 operand splitting (hi*hi + lo*hi + hi*lo, fp32 accumulation in registers):
  * fp32-class accuracy (~1e-6 relative) at tensor-core rate.  Two launches per block (conv+gate -> z, then the 1x1s);
  * d_z is a caller-provided (B,L,D) workspace.  Shapes: R % 256 == 0, S % 256 == 0, D % 128 == 0 (wn_tc_supported).
  * Weights are packed K-major and pre-split: d_wa [2][2D][k*R] (rows in 256-wide tiles: 128 filter channels then the
@@ -132,7 +132,7 @@ int wn_tc_read_trace(long long* host_out, int n);
 
 /* ---------------------------------------------------------------- (T) the block as ONE tensor-core launch (round 2 default)
  * Same mathematics as wn_block_fwd (reference wavenet_model.py:142-165) for R = D = S = 256, k = 2 (wn_tb_supported), with
- * fp32-class accuracy from bf16 (hi, lo) operand pairs on tcgen05.mma cta_group::2 (fp32 accumulation in tensor memory); the
+ * fp32-class accuracy from bf16 (hi, lo) operand pairs on wgmma (fp32 accumulation in registers); the
  * gated activation z never leaves the SM.  Activations use the CHUNKED PAIR LAYOUT: a (B, L, C) activation is stored as
  *     bf16 [b][plane: 0 = hi, 1 = lo][c / 8][t][c % 8]         x = hi + lo, hi = bf16(x), lo = bf16(x - hi)
  * (the same number of bytes as fp32 frames), and skip as fp32 [b][c / 4][t - skip_start][c % 4].  wn_pair_from_frames /
@@ -186,7 +186,7 @@ typedef struct wn_tb_stack_args {
 } wn_tb_stack_args;
 int       wn_tb_stack_fwd(const wn_tb_stack_args* a, void* stream);
 
-/* Backward of the same block on the same layout (tcgen05 cta_group::2, bf16 pairs), replacing autograd's backward through
+/* Backward of the same block on the same layout (wgmma, bf16 pairs), replacing autograd's backward through
  * wavenet_model.py:142-165.  Frame-range arguments are those of wn_block_bwd_args.  Buffers: d_dh_out (B,2,32,L,8) pair or
  * NULL (last layer), d_dskip (B,2,32,L-ds_start,8) pair on its own frame axis, d_fg the forward's d_fg_save, outputs d_dfg
  * (B,2,64,L,8) pair [dF chunks 0..31 | dG chunks 32..63], d_z (B,2,32,L,8) pair (recomputed tanh*sigmoid), d_dh_in pair.
@@ -206,7 +206,7 @@ typedef struct wn_tb_bwd_args {
 } wn_tb_bwd_args;
 int    wn_tb_block_bwd_data(const wn_tb_bwd_args* a, void* stream);
 /* All weight gradients of one block in one launch (+ a deterministic reduction): the contraction over frames reads the
- * chunked tiles as MN-major tcgen05 operands.  Outputs are the parameter-shaped tensors: d_gws (S,D,1), d_gwr (R,D,1),
+ * chunked tiles as MN-major wgmma operands.  Outputs are the parameter-shaped tensors: d_gws (S,D,1), d_gwr (R,D,1),
  * d_gwf / d_gwg (D,R,2).  id_start: first frame where dh_out flows straight into dh_in (= max(out_start, gs_out)).
  * d_work: wn_tb_wgrad_workspace_bytes() bytes. */
 size_t wn_tb_wgrad_workspace_bytes(void);
@@ -253,7 +253,7 @@ typedef struct wn_block_bwd_args {
 } wn_block_bwd_args;
 int wn_block_bwd_data(const wn_block_bwd_args* a, void* stream);
 
-/* The same two data-gradient GEMMs on the tensor cores (tcgen05, 3xTF32), for R % 256 == 0, S % 256 == 0, D % 256 == 0:
+/* The same two data-gradient GEMMs on the tensor cores (wgmma, 3xTF32), for R % 256 == 0, S % 256 == 0, D % 256 == 0:
  * weights packed K-major and pre-split by wn_tc_pack_block_bwd_weights into d_wdz [2][D][R+S] (row c: residual_conv
  * column c then skip_conv column c) and d_wdh [2][R][k*2D] (row r, column j*2D+n: [filter;gate].weight[n][r][j]).
  * d_wrs_rows / d_wfg_bwd of the args are ignored. */
@@ -290,7 +290,7 @@ typedef struct wn_wgrad_args {
 } wn_wgrad_args;
 size_t wn_wgrad_workspace_bytes(int N, int C);
 int wn_wgrad(const wn_wgrad_args* a, void* stream);
-/* The same contraction on the tensor cores (tcgen05 kind::f16 on bf16 hi/lo pairs, fp32 accumulation; the operand
+/* The same contraction on the tensor cores (wgmma on bf16 hi/lo pairs, fp32 accumulation; the operand
  * tiles are transposed to K-major while they are split): C == 256, N % 128 == 0, rows >= 1, ldg / ldx / sequence
  * strides multiples of 4 floats, d_g / d_x 16-byte aligned.  Same argument block and workspace as wn_wgrad. */
 int wn_tc_wgrad_supported(int N, int C);
@@ -374,8 +374,7 @@ typedef struct wn_gen_run_args {
 int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stream);
 int wn_gen_destroy(wn_gen_handle* h);
 /* Which sampler kernel runs (all implement the same schedule; call right after wn_gen_reset):
- *   0  auto: 256-wide k = 2 nets -> the tensor-core cluster kernel 6, for any number of streams (measured: one stream
- *            107.7 us/sample against 150.7 for kernel 3; 64 streams 382 k samples/s against 23 k for kernel 4);
+ *   0  auto: 256-wide k = 2 nets -> the tensor-core cluster kernel 6, for any number of streams;
  *            other nets: one stream -> the single-stream L2 kernel 3, several streams -> one cluster per stream
  *            (kernel 4) where it applies, otherwise the generic kernel
  *   1  atomic grid barrier between stages (the simple reference kernel)
@@ -384,15 +383,15 @@ int wn_gen_destroy(wn_gen_handle* h);
  *   4  cluster kernel: one 16-CTA thread-block cluster per stream, exchange through distributed shared memory
  *   5  single-stream two-level exchange: kernel 3's grid (64 CTAs x 4 rows) as 4 clusters of 16; values go to the 16 CTAs
  *      of the producer's cluster through distributed shared memory and reach the other clusters through ONE L2 poller per
- *      (cluster, producer) that forwards them by DSMEM (256-wide nets: R = D = S = E = classes = 256).  Measured 2x slower
+ *      (cluster, producer) that forwards them by DSMEM (256-wide nets: R = D = S = E = classes = 256).  Measured slower
  *      than kernel 3 (a 16-CTA DSMEM all-to-all costs as much as the L2 one it replaces): selectable, never the default
  *   6  tensor-core cluster kernel: up to 8 streams per thread-block cluster (256-wide nets: R = D = S = E = classes = 256,
  *      k = 2).  The weights of a stage enter shared memory once per 8 streams, as bf16 hi/lo pairs pre-split into MMA
  *      fragment order at wn_gen_reset (wn_gen_workspace_bytes includes the images; wn_gen_weights_changed after in-place
  *      weight updates); dot products are mma.sync m16n8k16 with three MMAs per product (fp32-class: ~1e-6 on the
  *      logits); the exchange is one 512-byte st.async.v4 block per destination CTA, credited to an mbarrier there.
- *      Clusters of 16 CTAs while all of them are co-resident (<= 7 clusters = 56 streams on a B200), else clusters of 8
- *      CTAs that own two 16-channel slices each (<= 15 clusters = 120 streams per wave)
+ *      Clusters of 16 CTAs while all of them are co-resident (as reported by the occupancy query), else clusters of 8
+ *      CTAs that own two 16-channel slices each (more clusters per wave)
  * Kernels 2, 3 and 5 sum in the same order (bit-identical results); kernel 4 splits rows differently (rounding-level
  * differences). */
 int wn_gen_set_mode(wn_gen_handle* h, int mode);

@@ -68,8 +68,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // Row ownership: CTA c owns the contiguous rows [c*per, min(N, (c+1)*per)), per = ceil(N/G).  Contiguous (not
 // interleaved) so that what a CTA publishes per stage is one run of {value,tag} pairs: with >= 4 rows per CTA the
-// stores of one warp instruction fill whole 32-byte sectors, which measured 2.6x faster to exchange than 16-byte
-// partial-sector writes from twice as many CTAs (tools/lat_probe.cu).
+// stores of one warp instruction fill whole 32-byte sectors rather than 16-byte partial-sector writes from twice as many
+// CTAs (tools/lat_probe.cu compares the two).
 __device__ __forceinline__ int own_per(int N, int G) { return (N + G - 1) / G; }
 __device__ __forceinline__ int own_cnt(int N, int G, int cta) {
     const int per = own_per(N, G), n = N - cta * per;
@@ -1329,8 +1329,8 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_fast(const GenParam
 // ================================================================================================ cluster kernel
 // One thread-block cluster (16 CTAs) per stream.  The stage-to-stage exchange no longer goes through the L2: a CTA
 // that has computed a value stores the {value, tag} pair straight into the shared memory of all 16 CTAs of its
-// cluster (distributed shared memory), and consumers spin on their OWN shared memory.  Measured on this part an L2
-// all-to-all costs ~1300-1650 cycles per stage (tools/lat_probe.cu); a DSMEM store lands in ~200-250.
+// cluster (distributed shared memory), and consumers spin on their OWN shared memory, which is closer than an L2
+// all-to-all (tools/lat_probe.cu measures both).
 //   stage 1 (conv rows)   warp-local: local poll of the layer input -> 4 rows per warp over the full K -> warp reduce ->
 //                         every lane recomputes z of the warp's 2 channels and stores it to one of the 16 CTAs
 //   stage 2 (1x1 rows)    warps 0-3 residual rows, warps 4-7 skip rows; one CTA barrier per layer before h' is
@@ -1697,19 +1697,18 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
 
 // ================================================================================================ two-level exchange kernel
 // Single stream, the grid of gen_kernel_fast (64 CTAs x 4 rows per stage vector) organised as 4 thread-block clusters of 16.
-// gen_kernel_fast pays ~1650 cycles per stage for an all-to-all in which 64 CTAs poll all 256 {value, tag} pairs through the
+// gen_kernel_fast pays, per stage, for an all-to-all in which 64 CTAs poll all 256 {value, tag} pairs through the
 // L2.  Here a value travels two hops instead:
-//   * inside a cluster the producer stores it straight into the shared memory of its 16 CTAs (distributed shared memory,
-//     ~250 cycles) -- and, once, to the L2 buffer the other kernels use (the ring history needs that anyway);
+//   * inside a cluster the producer stores it straight into the shared memory of its 16 CTAs (distributed shared memory)
+//     -- and, once, to the L2 buffer the other kernels use (the ring history needs that anyway);
 //   * between clusters ONE CTA per destination cluster polls it in the L2 -- rank r of cluster c fetches the 32-byte sector
 //     of the four values that rank r of each other cluster produced (3 sectors per stage instead of 64) -- and forwards it
 //     to its 16 cluster peers through DSMEM.
 // Every consumer then spins on its OWN shared memory (no polling storm on hot L2 lines, no staging pass and one CTA barrier
 // per stage instead of two).  Same row ownership, K split, summation order and activations as gen_kernel_fast /
 // gen_kernel_ll: logits and indices are bit-identical to theirs.
-// MEASURED (B200, cfg 2, 4000 samples): 299 us/sample against 150 us/sample for gen_kernel_fast.  The all-to-all inside a
-// 16-CTA cluster alone costs 910-940 cycles per round (tools/dsmem_probe.cu, variant A) -- no better than the L2 all-to-all
-// it replaces -- and the second hop is added on top.  Kept as mode 5 (selectable, tested bit-identical), never the default.
+// It measured slower than gen_kernel_fast: the all-to-all inside a 16-CTA cluster alone (tools/dsmem_probe.cu, variant A)
+// is no better than the L2 all-to-all it replaces, and the second hop is added on top.  Kept as mode 5 (selectable, tested bit-identical), never the default.
 __device__ __forceinline__ void wait_local2(const uint2* p, unsigned tag, float& a, float& b) {        // two pairs, 16-byte aligned
     const unsigned addr = smem_u32(p);
     unsigned x, y, z, w;
@@ -2120,8 +2119,8 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams 
 //     B operands are one LDS.128.  8 warps = 2 m-tiles x 4 K quarters; the partials meet in shared memory and 128-256
 //     finishing threads apply bias / tanh.sigmoid / the residual add and stage the CTA's block(s);
 //   * exchange: a pusher warp reads a staged 512-byte block back and issues ONE st.async.v4 per destination CTA, crediting
-//     the bytes to an mbarrier there; consumers sleep on their own mbarrier.  893-1 017 cycles per all-to-all round against
-//     1 125-1 254 with a bulk copy per destination and 2 624-4 144 with per-lane stores (tools/dsmem_probe.cu: H, F, E);
+//     the bytes to an mbarrier there; consumers sleep on their own mbarrier; tools/dsmem_probe.cu compares this (H) with a bulk
+//     copy per destination (F) and per-lane stores (E);
 //   * weights: producer warp(s) keep a 128 KB ring of images full (bulk copies; cp.async for the second block of an 8-CTA
 //     cluster's CTA);
 //   * history: the {value, tag} fp32 ring of the other kernels (same layout: sessions, queue export and kernel switches keep
@@ -2225,8 +2224,8 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
 }
 
 // CS = CTAs per cluster (16 or 8).  The exchanged vectors always consist of 16 blocks ("virtual ranks" of 16 channels);
-// a CTA of a CS-cluster owns VR = 16 / CS consecutive virtual ranks and walks them one after the other in every stage.  At
-// most 7 clusters of 16 CTAs are co-resident on a B200 (tools/cluster_occ.cu) but 15 clusters of 8: CS = 8 runs 64 streams
+// a CTA of a CS-cluster owns VR = 16 / CS consecutive virtual ranks and walks them one after the other in every stage.  Only
+// few clusters of 16 CTAs are co-resident (tools/cluster_occ.cu) but about twice as many clusters of 8: CS = 8 runs 64 streams
 // (8 clusters) in one wave on 64 SMs, at twice the per-CTA work -- the step is bound by the exchange latency, not by it.
 template <int CS>
 __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
@@ -2288,11 +2287,11 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
 
     // push the staged blocks `sb` into blocks v0 .. v0+VR-1 of vector `vec` of every CTA of the cluster: the pusher warp
     // (warp 9) reads each 512-byte block back (16 bytes per lane) and issues ONE st.async.v4 per destination -- a whole
-    // block per instruction, its bytes credited to the destination's mbarrier.  Measured per exchange round
-    // (tools/dsmem_probe.cu, 8 clusters of 16): 1 017 cycles this way (H), 1 254 with one cp.async.bulk per destination (F,
-    // which also occupies the SM's bulk-copy engine and needs a proxy fence after staging), 4 144 with per-lane 8-byte
-    // stores from the worker warps (E), and ~1 200 more for a multicast copy from a global staging slot (the fence after the
-    // global stores).  The workers only signal "staged" (bar.arrive on barrier 2) and move on to the next stage.
+    // block per instruction, its bytes credited to the destination's mbarrier.  The alternatives tools/dsmem_probe.cu
+    // compares are one cp.async.bulk per destination (which also occupies the SM's bulk-copy engine and needs a proxy
+    // fence after staging), per-lane 8-byte stores from the worker warps, and a multicast copy from a global staging slot
+    // (which needs a fence after the global stores).  The workers only signal "staged" (bar.arrive on barrier 2) and
+    // move on to the next stage.
     const unsigned sm_base = smem_u32(smb);
     unsigned rdelta[CS];                                 // shared::cluster address of CTA d minus the local address (pusher warp)
 #pragma unroll
@@ -2336,10 +2335,9 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         return;
     }
     // ---- producer warp: the weight images of this CTA for every stage, in order: ONE bulk copy per stage kind (the images
-    // of the CTA's VR virtual ranks are adjacent).  One lane issues; the issuing thread is held ~100 cycles + bytes/84 per
-    // instruction, so whole images it is: 8 KB pieces cap an SM at 45 B/cycle, 32 KB images reach 42 and 64 KB images 84
-    // with two in flight (tools/bulk_bw_probe.cu).  The exchange no longer uses the bulk-copy engine (st.async), which had
-    // throttled these copies to ~22 B/cycle.
+    // of the CTA's VR virtual ranks are adjacent).  One lane issues; the issuing thread is held per
+    // instruction, so whole images it is: fewer, larger copies with two in flight give an SM the most bytes per cycle
+    // (tools/bulk_bw_probe.cu).  The exchange does not use the bulk-copy engine (st.async), which would throttle these copies.
     if (warp == GEN_WARPS) {
         if (lane == 0) {
             unsigned q = 0;
@@ -3264,7 +3262,7 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
             p.n_wslots = h->n_wslots_cluster;
             p.wslot_floats = h->wslot_cluster;
             rc = launch_gen_cluster(h, p, st);
-        } else if (h->mode == 5 && h->x2_ok) {                // never picked automatically: measured 2x slower than kernel 3
+        } else if (h->mode == 5 && h->x2_ok) {                // never picked automatically: measured slower than kernel 3
             p.n_wslots = h->n_wslots_x2;
             rc = launch_gen_x2(h, p, st);
         } else if ((h->mode == 0 || h->mode == 3) && h->fast_ok) {

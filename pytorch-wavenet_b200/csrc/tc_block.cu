@@ -5,29 +5,27 @@
 //   skip[t]  (+)= Ws z[t] + bs                                                                 t in [skip_start, L)
 //
 // Numerics: fp32-class through bf16 PAIRS -- every operand x is carried as hi = bf16(x), lo = bf16(x - hi) and a product is
-// hi*hi + lo*hi + hi*lo on tcgen05 kind::f16 with fp32 accumulation in tensor memory (16 mantissa bits per operand; measured
-// 6.5e-6 on the logits of the 50-layer cfg-2/3 net, tools/split_sim.py; the parity bar is 1e-4).
+// hi*hi + lo*hi + hi*lo on wgmma (bf16 operands, fp32 accumulation in registers; 16 mantissa bits per operand, see
+// tools/split_sim.py; the parity bar is 1e-4).
 //
 // Data layout ("chunked pair layout", DESIGN.md section 2): an activation tensor of C channels over L frames is stored as
 //   [sequence b][plane: hi, lo][channel chunk c/8][frame t][8 channels] bf16            (same bytes as fp32 (B,L,C))
 // so that  (1) a TMA box {128 frames, 4 chunks, 2 planes} lands in shared memory exactly as the SWIZZLE_NONE K-major
-// core-matrix image tcgen05 consumes ([k-chunk][row][16 B], LBO = 2048, SBO = 128): no splitter, no swizzle, no conflicts;
-//          (2) an epilogue thread (= one frame, tcgen05.ld 32x32b) reads/writes 16-byte pieces that are CONTIGUOUS across the
-// lanes of its warp (consecutive frames): fully coalesced global accesses with no shared-memory transpose;
+// core-matrix image wgmma consumes ([k-chunk][row][16 B], LBO = 2048, SBO = 128): no splitter, no swizzle, no conflicts;
+//          (2) the four lanes of a quad hold the 8 channels of one frame of an accumulator fragment, so an epilogue store
+// instruction of a warp writes 8 consecutive frames of one chunk = 128 contiguous bytes, with no shared-memory transpose;
 //          (3) the same image is the MN-major operand of the weight-gradient GEMM (contraction over frames).
 // skip is [b][channel chunk c/4][frame][4 channels] fp32 for the same reason.  Weights are pre-split and pre-tiled into the
-// shared-memory image of every (n-tile, k-slab, CTA half), so a weight slab is one contiguous 16 KB TMA box.
+// shared-memory image of every (n-tile, k-slab, 128-row half), so a weight slab half is one contiguous 16 KB TMA box.
 //
-// Kernel: clusters of 2 CTAs (one per SM of a TPC), cta_group::2 MMAs M256 N256 K16: CTA r owns frames t0+128r..+127 of a
-// 256-frame item (its A rows, its 128 accumulator lanes) and stages half of every weight slab (its 128 of the 256 B rows).
-//   warp 0      TMA producer (both CTAs): ring of six 16 KB slots; a k-slab of pass A = one activation slot (32 channels of
-//               one tap, hi+lo) + one weight slot; pass B = weight slots only (its A operand z is resident)
-//   warp 1      tensor memory (512 columns = two 256-column accumulators) and, in the leader CTA, the MMA issue loop
-//   warps 2-9   epilogue: two groups x four TMEM lane quadrants
-// Per item the MMA warp runs  A0 -> acc0, A1 -> acc1  (filter|gate of channels 0..127 / 128..255, K = 2 taps x 256),
-// B0 -> acc0 (residual), B1 -> acc1 (skip; skipped for items left of skip_start).  The gate epilogue writes z as a bf16 pair
-// image into shared memory (128 KB: the A operand of pass B never leaves the SM) and signals it per 32-channel slab, so pass
-// B starts on the first slabs while the rest of the gate is still being computed.
+// Kernel: an item is 256 frames; CTA r = blockIdx.x & 1 of a pair owns frames t0+128r..+127 (the two CTAs do not talk).
+//   warp 8      TMA producer: ring of 48 KB stages = one activation slot (32 channels of one tap, hi+lo) + the two 16 KB
+//               halves of a weight slab; pass B stages carry weights only (its A operand z is resident)
+//   warps 0-7   two consumer warpgroups; warpgroup g owns frames 64g..64g+63 of the CTA: wgmma m64n128k16 into two
+//               128-column register accumulators, then the epilogue straight from the fragments
+// Per item a warpgroup runs pass A, n-tile j: acc0 = filter, acc1 = gate pre-activations of channels 128j..128j+127 (K = 2 taps
+// x CH), and writes z as a bf16 pair image into shared memory (the A operand of pass B never leaves the SM; each warpgroup
+// reads back only its own rows); pass B: residual tiles, then skip tiles (skipped for items left of skip_start).
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <cstdlib>
@@ -40,11 +38,13 @@ using namespace px;
 
 constexpr int BM = 128;                   // frames per CTA
 constexpr int PM = 256;                   // frames per item (CTA pair)
-constexpr int SLOT = 16384;               // one ring slot
-constexpr int NSLOT = 6;
-constexpr int NTHREADS = 320;
-constexpr int EPI_WARPS = 8;
+constexpr int SLOT = 16384;               // one activation slot / one weight half
+constexpr int STAGE = 3 * SLOT;           // activation slot + both weight halves
+constexpr int NTHREADS = 288;
+constexpr int EPI_WARPS = 8;              // consumer warps (two warpgroups)
+constexpr int CONSUMERS = 32 * EPI_WARPS;
 constexpr unsigned LBO = BM * 16, SBO = 128;
+constexpr int SMEM_MAX = 227 * 1024;
 
 // Shapes and operand precision.  PAIR: every MMA operand is a bf16 (hi, lo) pair and a product costs three MMAs
 // (fp32-class: the parity path).  !PAIR: single-pass bf16 operands (the hi planes only) with fp32 accumulation -- the
@@ -64,13 +64,12 @@ struct Cfg {
     static constexpr int NT_B = 2 * CH / 256;
     static constexpr int ZPLANE = (CH / 8) * BM * 16;        // one plane of the resident z image
     static constexpr int ZBYTES = PLANES * ZPLANE;
-    static constexpr int NZ = CH / KS;                       // z slabs = z_ready barriers
     static constexpr int WROWS_A = NT_A * SLABS_A * 2 * 8;   // 2 KB rows of one layer's packed pass-A weights
     static constexpr int WROWS_LAYER = WROWS_A + NT_B * SLABS_B * 2 * 8;
     static constexpr size_t W_LAYER_BYTES = (size_t)WROWS_LAYER * 2048;
-    static constexpr size_t SMEM_BYTES = 128 + ZBYTES + NSLOT * SLOT + 256;
-    static_assert(ZBYTES <= 131072, "the z image must fit beside the ring");
-    static_assert(NZ <= 8, "z_ready barriers");
+    static constexpr int NST = (SMEM_MAX - 384 - ZBYTES) / STAGE;     // ring depth that fits beside z
+    static constexpr size_t SMEM_BYTES = 128 + ZBYTES + (size_t)NST * STAGE + 256;
+    static_assert(NST >= 2, "the ring needs two stages beside the z image");
 };
 
 // One layer of a launch.  A single-layer launch carries it as a kernel parameter; the whole-stack launch reads an array of
@@ -93,7 +92,7 @@ struct BlockParams {
     int n_layers, total_items;
     float4* skip;                  // chunked (B, CH/4, L - skip_start, 4) fp32
     const LayerDesc* layers;       // whole-stack launch: [n_layers] in global memory
-    unsigned* item_done;           // whole-stack launch: [total_items] arrival counters (2 CTAs x 8 epilogue warps = 16 when complete)
+    unsigned* item_done;           // whole-stack launch: [total_items] arrival counters (2 CTAs x 8 consumer warps = 16 when complete)
     unsigned* layer_done;          //                     [n_layers] completed items per layer
 };
 
@@ -110,65 +109,77 @@ __device__ __forceinline__ void wait_counter(const unsigned* p, unsigned target)
     }
 }
 
+// One k-slab of a warpgroup: acc[h] (+)= A[64 rows x KS] * W_h[KS x 128] for the two weight halves h.  a: this warpgroup's
+// rows of the activation image (hi plane), a_lo: bytes to its lo plane, w: the first weight half (the second follows at
+// +SLOT, each half's lo plane at +SLOT/2).  first: the slab starts the accumulation.
+template <typename C>
+__device__ __forceinline__ void slab_mma(float (&acc)[2][64], unsigned a, unsigned a_lo, unsigned w, bool first) {
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < C::KS / 16; ++ks)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const unsigned long long ah = wg_desc(a + ks * 2 * LBO, LBO, SBO), bh = wg_desc(w + h * SLOT + ks * 2 * LBO, LBO, SBO);
+            wgmma_bf16_t00(acc[h], ah, bh, (first && ks == 0) ? 0u : 1u);
+            if constexpr (C::PAIR) {
+                wgmma_bf16_t00(acc[h], wg_desc(a + a_lo + ks * 2 * LBO, LBO, SBO), bh, 1u);
+                wgmma_bf16_t00(acc[h], ah, wg_desc(w + h * SLOT + SLOT / 2 + ks * 2 * LBO, LBO, SBO), 1u);
+            }
+        }
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_keep(acc[0]);
+    wgmma_keep(acc[1]);
+}
+
 // MULTI = false: one layer (`single`), items are independent.  MULTI = true: ALL layers of a forward in one persistent launch:
-// the global item list is layer-major and dealt round-robin to the clusters, an item waits (in its producer) for the items of the
-// previous layer that wrote the frames it reads, and announces itself when its epilogues have stored -- no launch gaps and no
-// idle tail between layers (a layer of cfg 3 is 456 items for 74 clusters: 6.16 rounds that cost 7 as separate launches).
+// the global item list is layer-major and dealt round-robin to the CTA pairs, an item waits (in its producer) for the items of
+// the previous layer that wrote the frames it reads, and announces itself when its epilogues have stored -- no launch gaps and
+// no idle tail between layers.
 template <typename C, bool MULTI>
 __global__ void __launch_bounds__(NTHREADS, 1)
 block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_constant__ CUtensorMap mapW, const BlockParams p) {
-    constexpr int CH = C::CH;
+    constexpr int CH = C::CH, NST = C::NST;
     auto LD = [&](int l) -> const LayerDesc& { return MULTI ? p.layers[l] : single; };
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
     unsigned char* zbuf = base;
     unsigned char* ring = base + C::ZBYTES;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + NSLOT * SLOT);
-    unsigned long long* full = bars;                   // [NSLOT]  leader: both CTAs' bytes of the slot have landed
-    unsigned long long* empty = bars + NSLOT;          // [NSLOT]  per CTA: the MMAs reading the slot have retired
-    unsigned long long* acc_full = bars + 2 * NSLOT;   // [2]      per CTA: accumulator complete
-    unsigned long long* acc_empty = acc_full + 2;      // [2]      leader: both CTAs' epilogues are done with the accumulator
-    unsigned long long* z_ready = acc_empty + 2;       // [8]      leader: both CTAs wrote z slab s of the current item
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(z_ready + 8);
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + NST * STAGE);
+    unsigned long long* full = bars;                   // [NST]  the stage's bytes have landed
+    unsigned long long* empty = bars + NST;            // [NST]  every consumer thread is done with the stage
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const unsigned rank = cluster_rank();
-    const int n_clusters = gridDim.x >> 1, cluster_id = blockIdx.x >> 1;
+    const int rank = (int)(blockIdx.x & 1);
+    const int n_pairs = gridDim.x >> 1, pair_id = blockIdx.x >> 1;
 
     if (tid == 0) {
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, 2 * EPI_WARPS); }
-        for (int i = 0; i < 8; ++i) mbar_init(z_ready + i, 2 * EPI_WARPS);
+        for (int i = 0; i < NST; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, CONSUMERS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
     }
-    if (warp == 1) tmem2_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===================================================================== TMA producer (one lane, both CTAs)
-        if (elect_one()) {
+    if (warp == EPI_WARPS) {
+        // ===================================================================== TMA producer (one lane)
+        if (lane == 0) {
             unsigned it = 0;
-            auto acquire = [&](unsigned& bar_addr) -> unsigned char* {
-                const unsigned s = it % NSLOT, ph = (it / NSLOT) & 1;
+            auto acquire = [&](unsigned long long*& bar, unsigned bytes) -> unsigned char* {
+                const unsigned s = it % NST, ph = (it / NST) & 1;
                 mbar_wait(empty + s, ph ^ 1);
-                if (rank == 0) mbar_expect_tx(full + s, 2 * SLOT);
-                bar_addr = mapa(s32(full + s), 0);
+                bar = full + s;
+                mbar_expect_tx(bar, bytes);
                 ++it;
-                return ring + s * SLOT;
+                return ring + s * STAGE;
             };
             int l = 0;
-            for (int n = cluster_id; n < p.total_items; n += n_clusters) {
+            for (int n = pair_id; n < p.total_items; n += n_pairs) {
                 while (n >= LD(l).item_base + LD(l).n_items) ++l;
                 const LayerDesc& Ld = LD(l);
                 const int item = n - Ld.item_base, dil = Ld.dil, w_row0 = Ld.w_row0;
                 const int b = item / Ld.tiles_per_seq, t0 = Ld.t_begin + (item % Ld.tiles_per_seq) * PM;
                 const bool need_skip = t0 + PM > p.skip_start;
-                const int tc = t0 + (int)rank * BM - Ld.in_start;          // this CTA's first frame, relative to the map origin
+                const int tc = t0 + rank * BM - Ld.in_start;               // this CTA's first frame, relative to the map origin
                 const CUtensorMap* mapH = &Ld.mapH;
                 if (MULTI && l > 0) {
                     // the previous layer's items that produced frames [t0 - d, t0 - d + 255] and [t0, t0 + 255] of this sequence
@@ -188,251 +199,130 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
                 }
                 for (int j = 0; j < C::NT_A; ++j)
                     for (int sl = 0; sl < C::SLABS_A; ++sl) {
-                        unsigned bar;
-                        unsigned char* dst = acquire(bar);
+                        unsigned long long* bar;
+                        unsigned char* dst = acquire(bar, 3 * SLOT);
                         const int tap = sl / (C::SLABS_A / 2);              // tap 0 reads h[t - d], tap 1 reads h[t]
-                        tma2_load_4d(dst, mapH, 2 * (tc - (1 - tap) * dil), (sl % (C::SLABS_A / 2)) * C::KC, 0, b, bar);
-                        dst = acquire(bar);
-                        tma2_load_2d(dst, &mapW, 0, w_row0 + ((j * C::SLABS_A + sl) * 2 + (int)rank) * 8, bar);
+                        tma_load_4d(dst, mapH, 2 * (tc - (1 - tap) * dil), (sl % (C::SLABS_A / 2)) * C::KC, 0, b, bar);
+                        for (int h = 0; h < 2; ++h)
+                            tma_load_2d(dst + (1 + h) * SLOT, &mapW, 0, w_row0 + ((j * C::SLABS_A + sl) * 2 + h) * 8, bar);
                     }
                 for (int j = 0; j < (need_skip ? C::NT_B : C::NT_R); ++j)
                     for (int s8 = 0; s8 < C::SLABS_B; ++s8) {
-                        unsigned bar;
-                        unsigned char* dst = acquire(bar);
-                        tma2_load_2d(dst, &mapW, 0, w_row0 + C::WROWS_A + ((j * C::SLABS_B + s8) * 2 + (int)rank) * 8, bar);
+                        unsigned long long* bar;
+                        unsigned char* dst = acquire(bar, 2 * SLOT);
+                        for (int h = 0; h < 2; ++h)
+                            tma_load_2d(dst + (1 + h) * SLOT, &mapW, 0, w_row0 + C::WROWS_A + ((j * C::SLABS_B + s8) * 2 + h) * 8, bar);
                     }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================================================== MMA issuer (leader CTA)
-        if (rank == 0) {
-            constexpr unsigned idesc = make_idesc_bf16(PM, 256);
-            unsigned it = 0, q = 0, n_item = 0;                  // slot counter, n-tile counter (accumulator = q & 1), item counter
-            // the products of one k-step (16 channels = 2 chunks): a / bw = byte addresses of the hi planes; the lo planes sit
-            // a_lo / SLOT/2 bytes further (pairs only)
-            auto mma_step = [&](unsigned d, unsigned a, unsigned a_lo, unsigned bw, unsigned accumulate) {
-                const unsigned long long ah = smem_desc(a, LBO, SBO), bh = smem_desc(bw, LBO, SBO);
-                umma2_f16(d, ah, bh, idesc, accumulate);
-                if constexpr (C::PAIR) {
-                    umma2_f16(d, smem_desc(a + a_lo, LBO, SBO), bh, idesc, 1);
-                    umma2_f16(d, ah, smem_desc(bw + SLOT / 2, LBO, SBO), idesc, 1);
-                }
-            };
-            auto next_acc = [&]() -> unsigned {                  // claim the next accumulator buffer (waits for its epilogue)
-                const unsigned ab = q & 1, u = q >> 1;
-                ++q;
-                if (u > 0) mbar_wait_cluster(acc_empty + ab, (u - 1) & 1);
-                tc_fence_after();
-                return ab;
-            };
-            int l = 0;
-            for (int n = cluster_id; n < p.total_items; n += n_clusters, ++n_item) {
-                while (n >= LD(l).item_base + LD(l).n_items) ++l;
-                const int item = n - LD(l).item_base;
-                const int t0 = LD(l).t_begin + (item % LD(l).tiles_per_seq) * PM;
-                const bool need_skip = t0 + PM > p.skip_start;
-                // ---------------- pass A: n-tiles of [tanh | sigmoid] pre-activations, K = 2 taps x CH
-                for (int j = 0; j < C::NT_A; ++j) {
-                    const unsigned ab = next_acc(), d = tmem_base + ab * 256;
-                    for (int sl = 0; sl < C::SLABS_A; ++sl) {
-                        const unsigned sa = it % NSLOT, pa = (it / NSLOT) & 1; ++it;
-                        const unsigned sw = it % NSLOT, pw = (it / NSLOT) & 1; ++it;
-                        mbar_wait_cluster(full + sa, pa);
-                        mbar_wait_cluster(full + sw, pw);
-                        tc_fence_after();
-                        if (elect_one()) {
-                            const unsigned a = s32(ring + sa * SLOT), w = s32(ring + sw * SLOT);
-#pragma unroll
-                            for (int ks = 0; ks < C::KS / 16; ++ks)
-                                mma_step(d, a + ks * 2 * LBO, SLOT / 2, w + ks * 2 * LBO, (sl | ks) != 0);
-                            umma2_commit(empty + sa);
-                            umma2_commit(empty + sw);
-                            if (sl == C::SLABS_A - 1) umma2_commit(acc_full + ab);
-                        }
-                        __syncwarp();
-                    }
-                }
-                // ---------------- pass B: residual tiles, then skip tiles, from the resident z image
-                for (int j = 0; j < (need_skip ? C::NT_B : C::NT_R); ++j) {
-                    const unsigned ab = next_acc(), d = tmem_base + ab * 256;
-                    for (int s8 = 0; s8 < C::SLABS_B; ++s8) {
-                        const unsigned sw = it % NSLOT, pw = (it / NSLOT) & 1; ++it;
-                        mbar_wait_cluster(z_ready + s8, n_item & 1);
-                        mbar_wait_cluster(full + sw, pw);
-                        tc_fence_after();
-                        if (elect_one()) {
-                            const unsigned a = s32(zbuf) + (unsigned)s8 * C::KC * LBO, w = s32(ring + sw * SLOT);
-#pragma unroll
-                            for (int ks = 0; ks < C::KS / 16; ++ks)
-                                mma_step(d, a + ks * 2 * LBO, C::ZPLANE, w + ks * 2 * LBO, (s8 | ks) != 0);
-                            umma2_commit(empty + sw);
-                            if (s8 == C::SLABS_B - 1) umma2_commit(acc_full + ab);
-                        }
-                        __syncwarp();
-                    }
-                }
             }
         }
     } else {
-        // ===================================================================== epilogue: warps 2..9
-        const int qd = warp & 3, grp = (warp - 2) >> 2;               // TMEM lane quadrant (= warp id mod 4), column group
-        const int row = qd * 32 + lane;
-        const unsigned lane_addr = tmem_base + ((unsigned)(qd * 32) << 16);
-        const unsigned acc_empty_addr[2] = {mapa(s32(acc_empty), 0), mapa(s32(acc_empty + 1), 0)};
-        const unsigned z_ready_addr = mapa(s32(z_ready), 0);
+        // ===================================================================== consumers: warpgroup g = warps 4g..4g+3
+        const int g = warp >> 2;
+        const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);        // this thread's fragment rows: r0 and r0 + 8
+        const int q2 = 2 * (lane & 3);                                 // its columns in every 8-column group: q2, q2 + 1
+        const unsigned a_off = (unsigned)(64 * g * 16);               // the warpgroup's rows inside an operand image
         const size_t plane_stride = (size_t)(CH / 8) * p.L;            // 16-byte pieces per plane of a pair tensor
         const int Tsk = p.L - p.skip_start;
-        unsigned q = 0;
+        unsigned it = 0;
+        float acc[2][64];
+        auto wait_stage = [&]() -> unsigned {
+            const unsigned s = it % NST, ph = (it / NST) & 1;
+            ++it;
+            mbar_wait(full + s, ph);
+            return s;
+        };
         int l = 0;
-        for (int n = cluster_id; n < p.total_items; n += n_clusters) {
+        for (int n = pair_id; n < p.total_items; n += n_pairs) {
             while (n >= LD(l).item_base + LD(l).n_items) ++l;
             const LayerDesc& Ld = LD(l);
             const int item = n - Ld.item_base;
             const int b = item / Ld.tiles_per_seq, t0 = Ld.t_begin + (item % Ld.tiles_per_seq) * PM;
             const bool need_skip = t0 + PM > p.skip_start;
-            const int t = t0 + (int)rank * BM + row;                   // this thread's frame
-            const bool live = t < p.L;
+            const int tf = t0 + rank * BM;                             // first frame of this CTA
             const float* bias = Ld.bias;
-            float4* fg_save = Ld.fg_save;
+            float* fg_save = reinterpret_cast<float*>(Ld.fg_save);
             const int skip_init = Ld.skip_init;
-            // ---------------- gate: z = tanh(F + bf) * sigmoid(G + bg) -> shared-memory operand image (+ optional saves)
+            // ---------------- pass A + gate: z = tanh(F + bf) * sigmoid(G + bg) -> shared-memory operand image (+ optional saves)
             for (int j = 0; j < C::NT_A; ++j) {
-                const unsigned ab = q & 1, u = q >> 1;
-                ++q;
-                mbar_wait(acc_full + ab, u & 1);
-                tc_fence_after();
-                const unsigned ta = lane_addr + ab * 256;
-#pragma unroll 1
-                for (int sb = 0; sb < 128 / C::KS; ++sb) {
-                    // slab sb of this n-tile = KS dilation channels; the two column groups take half each, so the slabs become
-                    // ready in the order pass B consumes them
-#pragma unroll 1
-                    for (int c = sb * C::KS + grp * (C::KS / 2); c < sb * C::KS + (grp + 1) * (C::KS / 2); c += 16) {
-                        float f[16], g[16];
-                        tmem_ld16(ta + c, f);
-                        tmem_ld16(ta + 128 + c, g);
-                        tmem_ld_wait();
-                        const int ch = j * 128 + c;                    // first of the 16 dilation channels
-                        const float4* bf4 = reinterpret_cast<const float4*>(bias + ch);
-                        const float4* bg4 = reinterpret_cast<const float4*>(bias + CH + ch);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float4 x = __ldg(bf4 + i), y = __ldg(bg4 + i);
-                            f[4 * i] = tanh_fast(f[4 * i] + x.x); f[4 * i + 1] = tanh_fast(f[4 * i + 1] + x.y);
-                            f[4 * i + 2] = tanh_fast(f[4 * i + 2] + x.z); f[4 * i + 3] = tanh_fast(f[4 * i + 3] + x.w);
-                            g[4 * i] = sigmoid_fast(g[4 * i] + y.x); g[4 * i + 1] = sigmoid_fast(g[4 * i + 1] + y.y);
-                            g[4 * i + 2] = sigmoid_fast(g[4 * i + 2] + y.z); g[4 * i + 3] = sigmoid_fast(g[4 * i + 3] + y.w);
-                        }
-                        if (fg_save != nullptr && live) {
-                            float4* fs = fg_save + ((size_t)b * (2 * CH / 4) + ch / 4) * p.L + t;
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                fs[(size_t)i * p.L] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-                                fs[(size_t)(CH / 4 + i) * p.L] = make_float4(g[4 * i], g[4 * i + 1], g[4 * i + 2], g[4 * i + 3]);
-                            }
-                        }
-                        unsigned hi[8], lo[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) split2(f[2 * i] * g[2 * i], f[2 * i + 1] * g[2 * i + 1], hi[i], lo[i]);
-                        unsigned char* zr = zbuf + (ch / 8) * (BM * 16) + row * 16;
-                        *reinterpret_cast<uint4*>(zr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                        *reinterpret_cast<uint4*>(zr + BM * 16) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                        if constexpr (C::PAIR) {
-                            *reinterpret_cast<uint4*>(zr + C::ZPLANE) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                            *reinterpret_cast<uint4*>(zr + C::ZPLANE + BM * 16) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                        }
-                    }
-                    // this warp's 32 rows of its half of z slab (128j / KS + sb) are in shared memory
-                    fence_async_smem();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(z_ready_addr + 8u * (unsigned)(j * (128 / C::KS) + sb));
+                for (int sl = 0; sl < C::SLABS_A; ++sl) {
+                    const unsigned s = wait_stage();
+                    const unsigned st = s32(ring + s * STAGE);
+                    slab_mma<C>(acc, st + a_off, SLOT / 2, st + SLOT, sl == 0);
+                    mbar_arrive(empty + s);
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(acc_empty_addr[ab]);
+#pragma unroll
+                for (int nb = 0; nb < 16; ++nb) {
+                    const int ch = j * 128 + 8 * nb + q2;                      // first of this thread's two dilation channels
+                    const float2 bf = __ldg(reinterpret_cast<const float2*>(bias + ch));
+                    const float2 bg = __ldg(reinterpret_cast<const float2*>(bias + CH + ch));
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const int row = r0 + 8 * r, t = tf + row;
+                        const float f0 = tanh_fast(acc[0][4 * nb + 2 * r] + bf.x), f1 = tanh_fast(acc[0][4 * nb + 2 * r + 1] + bf.y);
+                        const float g0 = sigmoid_fast(acc[1][4 * nb + 2 * r] + bg.x), g1 = sigmoid_fast(acc[1][4 * nb + 2 * r + 1] + bg.y);
+                        if (fg_save != nullptr && t < p.L) {
+                            float* fs = fg_save + (((size_t)b * (2 * CH / 4) + ch / 4) * p.L + t) * 4 + (ch & 3);
+                            *reinterpret_cast<float2*>(fs) = make_float2(f0, f1);
+                            *reinterpret_cast<float2*>(fs + (size_t)(CH / 4) * p.L * 4) = make_float2(g0, g1);
+                        }
+                        unsigned hi, lo;
+                        split2(f0 * g0, f1 * g1, hi, lo);
+                        unsigned char* zr = zbuf + (ch / 8) * (BM * 16) + row * 16 + q2 * 2;
+                        *reinterpret_cast<unsigned*>(zr) = hi;
+                        if constexpr (C::PAIR) *reinterpret_cast<unsigned*>(zr + C::ZPLANE) = lo;
+                    }
+                }
             }
+            // the warpgroup's rows of z are complete: make the generic-proxy stores visible to its wgmma reads
+            fence_async_smem();
+            wg_bar(1 + g, 128);
             // ---------------- pass B tiles: residual h_out = acc + br + h_in -> pair; then skip (+)= acc + bs
             for (int j = 0; j < (need_skip ? C::NT_B : C::NT_R); ++j) {
-                const unsigned ab = q & 1, u = q >> 1;
-                ++q;
-                mbar_wait(acc_full + ab, u & 1);
-                tc_fence_after();
-                const unsigned ta = lane_addr + ab * 256;
+                for (int s8 = 0; s8 < C::SLABS_B; ++s8) {
+                    const unsigned s = wait_stage();
+                    slab_mma<C>(acc, s32(zbuf) + a_off + (unsigned)s8 * C::KC * LBO, C::ZPLANE, s32(ring + s * STAGE) + SLOT, s8 == 0);
+                    mbar_arrive(empty + s);
+                }
                 if (j < C::NT_R) {
-                    const int n0 = j * 256;                                // first residual channel of this tile
-                    const uint4* hin = Ld.h_in + (size_t)b * 2 * plane_stride + t;
-                    uint4* hout = Ld.h_out + (size_t)b * 2 * plane_stride + t;
-                    uint4 nx[4];
-                    auto load_res = [&](int c) {
-                        nx[0] = nx[1] = nx[2] = nx[3] = make_uint4(0, 0, 0, 0);
-                        if (live) {
-                            const uint4* s = hin + (size_t)((n0 + c) / 8) * p.L;
-                            nx[0] = __ldg(s); nx[1] = __ldg(s + p.L); nx[2] = __ldg(s + plane_stride); nx[3] = __ldg(s + plane_stride + p.L);
-                        }
-                    };
-                    load_res(grp * 128);
-#pragma unroll 1
-                    for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                        float v[16];
-                        tmem_ld16(ta + c, v);
-                        const uint4 xh0 = nx[0], xh1 = nx[1], xl0 = nx[2], xl1 = nx[3];
-                        if (c + 16 < grp * 128 + 128) load_res(c + 16);        // next chunk's loads fly under this chunk's math
-                        tmem_ld_wait();
-                        const float4* b4 = reinterpret_cast<const float4*>(bias + 2 * CH + n0 + c);
-                        const unsigned xh[8] = {xh0.x, xh0.y, xh0.z, xh0.w, xh1.x, xh1.y, xh1.z, xh1.w};
-                        const unsigned xl[8] = {xl0.x, xl0.y, xl0.z, xl0.w, xl1.x, xl1.y, xl1.z, xl1.w};
-                        unsigned hi[8], lo[8];
+                    const unsigned* hin = reinterpret_cast<const unsigned*>(Ld.h_in + (size_t)b * 2 * plane_stride);
+                    unsigned* hout = reinterpret_cast<unsigned*>(Ld.h_out + (size_t)b * 2 * plane_stride);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float4 bb = __ldg(b4 + i);
-                            const float2 h0 = unpack_bf16x2(xh[2 * i]), l0 = unpack_bf16x2(xl[2 * i]);
-                            const float2 h1 = unpack_bf16x2(xh[2 * i + 1]), l1 = unpack_bf16x2(xl[2 * i + 1]);
-                            split2(v[4 * i] + bb.x + (h0.x + l0.x), v[4 * i + 1] + bb.y + (h0.y + l0.y), hi[2 * i], lo[2 * i]);
-                            split2(v[4 * i + 2] + bb.z + (h1.x + l1.x), v[4 * i + 3] + bb.w + (h1.y + l1.y), hi[2 * i + 1], lo[2 * i + 1]);
-                        }
-                        if (live) {
-                            uint4* o = hout + (size_t)((n0 + c) / 8) * p.L;
-                            o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                            o[p.L] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                            o[plane_stride] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                            o[plane_stride + p.L] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                        }
-                    }
-                } else {
-                    const int n0 = (j - C::NT_R) * 256;                    // first skip channel of this tile
-                    const bool on = live && t >= p.skip_start;
-                    float4* sk = p.skip + (size_t)b * (CH / 4) * Tsk + (t - p.skip_start);
-                    float4 nx[4];
-                    const bool rmw = on && !skip_init;
-                    auto load_skip = [&](int c) {
+                    for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            nx[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (rmw) nx[i] = sk[(size_t)((n0 + c) / 4 + i) * Tsk];
-                        }
-                    };
-                    load_skip(grp * 128);
-#pragma unroll 1
-                    for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                        float v[16];
-                        tmem_ld16(ta + c, v);
-                        const float4 x[4] = {nx[0], nx[1], nx[2], nx[3]};
-                        if (c + 16 < grp * 128 + 128) load_skip(c + 16);
-                        tmem_ld_wait();
-                        const float4* b4 = reinterpret_cast<const float4*>(bias + 3 * CH + n0 + c);
-                        if (on) {
+                        for (int nb = 0; nb < 16; ++nb) {
+                            const int ch = j * 256 + 128 * h + 8 * nb + q2;        // first of this thread's two residual channels
+                            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 2 * CH + ch));
 #pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float4 bb = __ldg(b4 + i);
-                                sk[(size_t)((n0 + c) / 4 + i) * Tsk] = make_float4(v[4 * i] + bb.x + x[i].x, v[4 * i + 1] + bb.y + x[i].y,
-                                                                                   v[4 * i + 2] + bb.z + x[i].z, v[4 * i + 3] + bb.w + x[i].w);
+                            for (int r = 0; r < 2; ++r) {
+                                const int t = tf + r0 + 8 * r;
+                                if (t >= p.L) continue;
+                                const size_t w = ((size_t)(ch / 8) * p.L + t) * 4 + (q2 >> 1);    // 32-bit word of the hi plane
+                                // plain (coherent) loads: in the whole-stack launch h_in was written by other CTAs of this kernel
+                                const float2 xh = unpack_bf16x2(hin[w]), xl = unpack_bf16x2(hin[w + plane_stride * 4]);
+                                unsigned hi, lo;
+                                split2(acc[h][4 * nb + 2 * r] + bb.x + (xh.x + xl.x), acc[h][4 * nb + 2 * r + 1] + bb.y + (xh.y + xl.y), hi, lo);
+                                hout[w] = hi;
+                                hout[w + plane_stride * 4] = lo;
                             }
                         }
-                    }
+                } else {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int nb = 0; nb < 16; ++nb) {
+                            const int ch = (j - C::NT_R) * 256 + 128 * h + 8 * nb + q2;   // first of this thread's two skip channels
+                            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 3 * CH + ch));
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) {
+                                const int t = tf + r0 + 8 * r;
+                                if (t >= p.L || t < p.skip_start) continue;
+                                float* sk = reinterpret_cast<float*>(p.skip) + (((size_t)b * (CH / 4) + ch / 4) * Tsk + (t - p.skip_start)) * 4 + (ch & 3);
+                                float2 x = make_float2(0.f, 0.f);
+                                if (!skip_init) x = *reinterpret_cast<const float2*>(sk);
+                                *reinterpret_cast<float2*>(sk) = make_float2(acc[h][4 * nb + 2 * r] + bb.x + x.x, acc[h][4 * nb + 2 * r + 1] + bb.y + x.y);
+                            }
+                        }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(acc_empty_addr[ab]);
             }
             if (MULTI) {
                 // this warp's stores of h_out / skip are done: publish (release at gpu scope); the 16th arrival completes the item
@@ -445,10 +335,6 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync();                               // the peer may still multicast commits at this CTA's barriers until here
-    if (warp == 1) tmem2_dealloc(tmem_base, 512);
 }
 
 // ---------------------------------------------------------------------------------------------- weight packing
@@ -678,18 +564,12 @@ extern "C" int wn_tb_start_index_i64(const int64_t* d_idx, const float* d_w_t, c
     return start_pair(d_idx, false, d_w_t, d_b_p, d_h_pair, B, classes, L, R, d_err, stream);
 }
 
-static int launch_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, int grid, size_t smem, cudaStream_t st) {
+static int launch_cfg(cudaLaunchConfig_t& cfg, int grid, size_t smem, cudaStream_t st) {
     cfg = cudaLaunchConfig_t{};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(tb::NTHREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     return 0;
 }
 
@@ -727,8 +607,7 @@ static int launch_block(const wn_tb_block_args* a, cudaStream_t st) {
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, grid, C::SMEM_BYTES, st);
+    launch_cfg(cfg, grid, C::SMEM_BYTES, st);
     WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, false>, d, mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;
@@ -792,13 +671,12 @@ static int launch_stack(const wn_tb_stack_args* a, cudaStream_t st) {
     p.layers = (const tb::LayerDesc*)a->d_desc;
     p.item_done = a->d_flags; p.layer_done = a->d_flags + base;
     WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
-    // every cluster must be resident (items wait for items of other clusters): one CTA per SM, at most sms/2 clusters
+    // every CTA must be resident (items wait for items of other CTAs): one CTA per SM, at most sms/2 pairs
     int grid = 2 * base;
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, grid, C::SMEM_BYTES, st);
+    launch_cfg(cfg, grid, C::SMEM_BYTES, st);
     WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, true>, desc[0], mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;

@@ -1,20 +1,20 @@
 // tc_bwd2.cu -- backward of the residual block (what autograd computes through reference wavenet_model.py:142-165 after
-// loss.backward(), wavenet_training.py:71) on the chunked bf16-pair layout of tc_block.cu, tcgen05 cta_group::2 throughout.
+// loss.backward(), wavenet_training.py:71) on the chunked bf16-pair layout of tc_block.cu, wgmma throughout.
 //
 // Data gradients, two launches per block (the second needs dF|dG of OTHER frames, t and t + d, so it cannot be fused):
 //   pair_gemm<EPI_DZ>  dz[t] = Wr^T dh_out[t] + Ws^T dskip[t]           (K = 512, N = 256 dilation channels)
 //                      epilogue: dF = dz g (1 - f^2), dG = dz f g (1 - g), z = f g  ->  dFG pair (512 ch), z pair
 //   pair_gemm<EPI_DH>  dh_in[t] = dh_out[t] + sum_tap [Wf;Wg]_tap^T dFG[t + (1-tap) d]      (K = 1024, N = 256 residual ch.)
-// Same machinery as the forward's pass A: 256-frame items over a CTA pair, ring of 16 KB slots (activation slot + weight
-// slot per 32-channel k-slab), two 256-column accumulators alternating between items so the epilogue of one item runs
-// under the MMAs of the next.  Frames outside a tensor's valid range come back as zeros from the TMA bounds check, which
+// Same machinery as the forward's pass A: 256-frame items over a CTA pair (128 frames per CTA), a ring of 48 KB stages
+// (activation slot + both weight halves per 32-channel k-slab), two consumer warpgroups with register accumulators of
+// 64 frames x 256 columns each, the TMA producer running ahead while they compute the epilogue.  Frames outside a tensor's valid range come back as zeros from the TMA bounds check, which
 // is exactly the structure of the gradients (zero left of gs_out / ds_start / gz, nothing right of L).
 //
 // Weight gradients: dW[n][c] = sum_b sum_t g[b][t][n] x[b][t][c] contracts over FRAMES.  In the chunked layout a tile
 // [8-channel chunk][frame][8] is the SWIZZLE_NONE *MN-major* operand image (LBO = 128 between 8-frame groups, SBO =
-// frames*16 between chunks), so the TMA boxes feed tcgen05 directly -- no transposing splitter as in round 1.  One launch
-// per block covers all six 256x256 jobs (skip, residual, filter/gate x 2 taps); a job is split over frame ranges across
-// clusters, partial sums go to a workspace and a second kernel adds them in fixed order (deterministic).
+// frames*16 between chunks), so the TMA boxes feed wgmma directly as transposed operands -- no transposing splitter.  One
+// launch per block covers all six 256x256 jobs (skip, residual, filter/gate x 2 taps); a job is split over frame ranges
+// across CTA pairs (each CTA of a pair takes 128 of the 256 rows), partial sums go to a workspace and a second kernel adds them in fixed order (deterministic).
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <cstdlib>
@@ -29,8 +29,9 @@ namespace tb2 {
 using namespace px;
 
 constexpr int BM = 128, PM = 256;
-constexpr int SLOT = 16384, NSLOT = 8;
-constexpr int NTHREADS = 320, EPI_WARPS = 8;
+constexpr int SLOT = 16384, STAGE = 3 * SLOT;
+constexpr int NTHREADS = 288, EPI_WARPS = 8, CONSUMERS = 256;     // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int NST = (227 * 1024 - 384) / STAGE;
 constexpr unsigned LBO = BM * 16, SBO = 128;
 enum { EPI_DZ = 0, EPI_DH = 1 };
 
@@ -50,13 +51,13 @@ struct Cfg {
     static constexpr int WROWS_BWD_LAYER = WROWS_DZ + NT * SLABS_DH * 2 * 8;
     static constexpr size_t WB_LAYER_BYTES = (size_t)WROWS_BWD_LAYER * 2048;
 };
-constexpr size_t SMEM_PG = 128 + NSLOT * SLOT + 256;
+constexpr size_t SMEM_PG = 128 + (size_t)NST * STAGE + 256;
 
 struct KSeg { int shift, origin, slabs, pad; };    // A rows of frame t: the segment's tensor at frame t + shift - origin
 struct PgParams {
     int B, L, t_begin, tiles_per_seq, n_items;
     int n_seg; KSeg seg[2];
-    int w_row0, w_slabs_per_tile, w_slab_off;      // weight slot of (n-tile j, k-slab s): row w_row0 + ((j*w_slabs_per_tile + w_slab_off + s)*2 + rank)*8
+    int w_row0, w_slabs_per_tile, w_slab_off;      // weight half h of (n-tile j, k-slab s): rows w_row0 + ((j*w_slabs_per_tile + w_slab_off + s)*2 + h)*8
     const float4* fg;        // DZ: chunked (B, 2CH/4, L, 4) tanh | sigmoid outputs
     uint4* out0;             // DZ: dFG pair (B, 2, 2CH/8, L, 8)      DH: dh_in pair (B, 2, CH/8, L, 8)
     uint4* out1;             // DZ: z pair (B, 2, CH/8, L, 8)
@@ -71,191 +72,139 @@ pair_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
     constexpr int CH = C::CH;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + NSLOT * SLOT);
-    unsigned long long* full = bars;                   // [NSLOT] leader
-    unsigned long long* empty = bars + NSLOT;          // [NSLOT] per CTA
-    unsigned long long* acc_full = bars + 2 * NSLOT;   // [2] per CTA
-    unsigned long long* acc_empty = acc_full + 2;      // [2] leader
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(acc_empty + 2);
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + NST * STAGE);
+    unsigned long long* full = bars;                   // [NST]
+    unsigned long long* empty = bars + NST;            // [NST]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const unsigned rank = cluster_rank();
-    const int n_clusters = gridDim.x >> 1, cluster_id = blockIdx.x >> 1;
+    const int rank = (int)(blockIdx.x & 1);
+    const int n_pairs = gridDim.x >> 1, pair_id = blockIdx.x >> 1;
     if (tid == 0) {
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, 2 * EPI_WARPS); }
+        for (int i = 0; i < NST; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, CONSUMERS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA0) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA1) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
     }
-    if (warp == 1) tmem2_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
     const int slabs = p.seg[0].slabs + (p.n_seg > 1 ? p.seg[1].slabs : 0);
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (warp == EPI_WARPS) {
+        if (lane == 0) {
             unsigned it = 0;
-            auto acquire = [&](unsigned& bar_addr) -> unsigned char* {
-                const unsigned s = it % NSLOT, ph = (it / NSLOT) & 1;
-                mbar_wait(empty + s, ph ^ 1);
-                if (rank == 0) mbar_expect_tx(full + s, 2 * SLOT);
-                bar_addr = mapa(s32(full + s), 0);
-                ++it;
-                return ring + s * SLOT;
-            };
-            for (int item = cluster_id; item < p.n_items; item += n_clusters) {
-                const int b = item / p.tiles_per_seq, t0 = p.t_begin + (item % p.tiles_per_seq) * PM + (int)rank * BM;
+            for (int item = pair_id; item < p.n_items; item += n_pairs) {
+                const int b = item / p.tiles_per_seq, t0 = p.t_begin + (item % p.tiles_per_seq) * PM + rank * BM;
                 for (int j = 0; j < C::NT; ++j) {
                     int gsl = 0;
                     for (int sg = 0; sg < p.n_seg; ++sg) {
                         const KSeg s = p.seg[sg];
                         const CUtensorMap* map = sg == 0 ? &mapA0 : &mapA1;
-                        for (int sl = 0; sl < s.slabs; ++sl, ++gsl) {
-                            unsigned bar;
-                            unsigned char* dst = acquire(bar);
-                            tma2_load_4d(dst, map, 2 * (t0 + s.shift - s.origin), sl * C::KC, 0, b, bar);
-                            dst = acquire(bar);
-                            tma2_load_2d(dst, &mapW, 0, p.w_row0 + ((j * p.w_slabs_per_tile + p.w_slab_off + gsl) * 2 + (int)rank) * 8, bar);
+                        for (int sl = 0; sl < s.slabs; ++sl, ++gsl, ++it) {
+                            const unsigned st = it % NST, ph = (it / NST) & 1;
+                            mbar_wait(empty + st, ph ^ 1);
+                            mbar_expect_tx(full + st, STAGE);
+                            unsigned char* dst = ring + st * STAGE;
+                            tma_load_4d(dst, map, 2 * (t0 + s.shift - s.origin), sl * C::KC, 0, b, full + st);
+                            for (int h = 0; h < 2; ++h)
+                                tma_load_2d(dst + (1 + h) * SLOT, &mapW, 0,
+                                            p.w_row0 + ((j * p.w_slabs_per_tile + p.w_slab_off + gsl) * 2 + h) * 8, full + st);
                         }
                     }
                 }
             }
-        }
-    } else if (warp == 1) {
-        if (rank == 0) {
-            constexpr unsigned idesc = make_idesc_bf16(PM, 256);
-            unsigned it = 0, q = 0;
-            for (int item = cluster_id; item < p.n_items; item += n_clusters)
-                for (int j = 0; j < C::NT; ++j, ++q) {
-                    const unsigned ab = q & 1, u = q >> 1;
-                    if (u > 0) mbar_wait_cluster(acc_empty + ab, (u - 1) & 1);
-                    tc_fence_after();
-                    const unsigned d = tmem_base + ab * 256;
-                    for (int sl = 0; sl < slabs; ++sl) {
-                        const unsigned sa = it % NSLOT, pa = (it / NSLOT) & 1; ++it;
-                        const unsigned sw = it % NSLOT, pw = (it / NSLOT) & 1; ++it;
-                        mbar_wait_cluster(full + sa, pa);
-                        mbar_wait_cluster(full + sw, pw);
-                        tc_fence_after();
-                        if (elect_one()) {
-                            const unsigned a = s32(ring + sa * SLOT), w = s32(ring + sw * SLOT);
-#pragma unroll
-                            for (int ks = 0; ks < C::KS / 16; ++ks) {
-                                const unsigned long long ah = smem_desc(a + ks * 2 * LBO, LBO, SBO), bh = smem_desc(w + ks * 2 * LBO, LBO, SBO);
-                                umma2_f16(d, ah, bh, idesc, (sl | ks) != 0);
-                                if constexpr (C::PAIR) {
-                                    umma2_f16(d, smem_desc(a + SLOT / 2 + ks * 2 * LBO, LBO, SBO), bh, idesc, 1);
-                                    umma2_f16(d, ah, smem_desc(w + SLOT / 2 + ks * 2 * LBO, LBO, SBO), idesc, 1);
-                                }
-                            }
-                            umma2_commit(empty + sa);
-                            umma2_commit(empty + sw);
-                            if (sl == slabs - 1) umma2_commit(acc_full + ab);
-                        }
-                        __syncwarp();
-                    }
-                }
         }
     } else {
-        const int qd = warp & 3, grp = (warp - 2) >> 2;
-        const int row = qd * 32 + lane;
-        const unsigned lane_addr = tmem_base + ((unsigned)(qd * 32) << 16);
-        const unsigned acc_empty_addr[2] = {mapa(s32(acc_empty), 0), mapa(s32(acc_empty + 1), 0)};
+        const int g = warp >> 2;
+        const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);        // fragment rows r0, r0 + 8
+        const int q2 = 2 * (lane & 3);                                 // fragment columns q2, q2 + 1 of every 8-column group
+        const unsigned a_off = (unsigned)(64 * g * 16);
         const size_t L = (size_t)p.L;
-        unsigned q = 0;
-        for (int item = cluster_id; item < p.n_items; item += n_clusters)
-          for (int j = 0; j < C::NT; ++j, ++q) {
-            const unsigned ab = q & 1, u = q >> 1;
+        unsigned it = 0;
+        float acc[2][64];
+        for (int item = pair_id; item < p.n_items; item += n_pairs)
+          for (int j = 0; j < C::NT; ++j) {
             const int b = item / p.tiles_per_seq;
-            const int t = p.t_begin + (item % p.tiles_per_seq) * PM + (int)rank * BM + row;
-            const bool live = t < p.L;
+            const int tf = p.t_begin + (item % p.tiles_per_seq) * PM + rank * BM;
             const int n0 = j * 256;                                     // first output channel of this n-tile
-            mbar_wait(acc_full + ab, u & 1);
-            tc_fence_after();
-            const unsigned ta = lane_addr + ab * 256;
-            if (EPI == EPI_DZ) {
-                const float4* fg = p.fg + ((size_t)b * (2 * CH / 4) + n0 / 4) * L + t;
-                uint4* dfg = p.out0 + ((size_t)b * 2 * (2 * CH / 8) + n0 / 8) * L + t;     // planes of 2CH/8 chunks
-                uint4* zo = p.out1 + ((size_t)b * 2 * (CH / 8) + n0 / 8) * L + t;          // planes of CH/8 chunks
-                const size_t pl_fg = (size_t)(2 * CH / 8) * L, pl_z = (size_t)(CH / 8) * L;
-#pragma unroll 1
-                for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                    float v[16];
-                    tmem_ld16(ta + c, v);
-                    float4 fq[4], gq[4];
+            for (int sl = 0; sl < slabs; ++sl, ++it) {
+                const unsigned s = it % NST, ph = (it / NST) & 1;
+                mbar_wait(full + s, ph);
+                const unsigned st = s32(ring + s * STAGE);
+                wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        fq[i] = gq[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (live) { fq[i] = __ldg(fg + (size_t)(c / 4 + i) * L); gq[i] = __ldg(fg + (size_t)(CH / 4 + c / 4 + i) * L); }
-                    }
-                    tmem_ld_wait();
-                    if (live) {
-                        const float* f = reinterpret_cast<const float*>(fq);
-                        const float* g = reinterpret_cast<const float*>(gq);
-                        unsigned fh[8], fl[8], gh[8], gl[8], zh[8], zl[8];
+                for (int ks = 0; ks < C::KS / 16; ++ks)
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const float f0 = f[2 * i], f1 = f[2 * i + 1], g0 = g[2 * i], g1 = g[2 * i + 1];
-                            split2(v[2 * i] * g0 * (1.f - f0 * f0), v[2 * i + 1] * g1 * (1.f - f1 * f1), fh[i], fl[i]);
-                            split2(v[2 * i] * f0 * g0 * (1.f - g0), v[2 * i + 1] * f1 * g1 * (1.f - g1), gh[i], gl[i]);
-                            split2(f0 * g0, f1 * g1, zh[i], zl[i]);
+                    for (int h = 0; h < 2; ++h) {
+                        const unsigned a = st + a_off + ks * 2 * LBO, w = st + (1 + h) * SLOT + ks * 2 * LBO;
+                        const unsigned long long ah = wg_desc(a, LBO, SBO), bh = wg_desc(w, LBO, SBO);
+                        wgmma_bf16_t00(acc[h], ah, bh, (sl == 0 && ks == 0) ? 0u : 1u);
+                        if constexpr (C::PAIR) {
+                            wgmma_bf16_t00(acc[h], wg_desc(a + SLOT / 2, LBO, SBO), bh, 1u);
+                            wgmma_bf16_t00(acc[h], ah, wg_desc(w + SLOT / 2, LBO, SBO), 1u);
                         }
-                        uint4* o = dfg + (size_t)(c / 8) * L;
-                        o[0] = make_uint4(fh[0], fh[1], fh[2], fh[3]); o[L] = make_uint4(fh[4], fh[5], fh[6], fh[7]);
-                        o[pl_fg] = make_uint4(fl[0], fl[1], fl[2], fl[3]); o[pl_fg + L] = make_uint4(fl[4], fl[5], fl[6], fl[7]);
-                        o += (size_t)(CH / 8) * L;
-                        o[0] = make_uint4(gh[0], gh[1], gh[2], gh[3]); o[L] = make_uint4(gh[4], gh[5], gh[6], gh[7]);
-                        o[pl_fg] = make_uint4(gl[0], gl[1], gl[2], gl[3]); o[pl_fg + L] = make_uint4(gl[4], gl[5], gl[6], gl[7]);
-                        uint4* zz = zo + (size_t)(c / 8) * L;
-                        zz[0] = make_uint4(zh[0], zh[1], zh[2], zh[3]); zz[L] = make_uint4(zh[4], zh[5], zh[6], zh[7]);
-                        zz[pl_z] = make_uint4(zl[0], zl[1], zl[2], zl[3]); zz[pl_z + L] = make_uint4(zl[4], zl[5], zl[6], zl[7]);
                     }
-                }
-            } else {
-                const size_t pl = (size_t)(CH / 8) * L;
-                const uint4* rs = p.res ? p.res + ((size_t)b * 2 * (CH / 8) + n0 / 8) * L + t : nullptr;
-                uint4* o0 = p.out0 + ((size_t)b * 2 * (CH / 8) + n0 / 8) * L + t;
-                const bool add = live && rs != nullptr && t >= p.id_start;
-#pragma unroll 1
-                for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                    float v[16];
-                    tmem_ld16(ta + c, v);
-                    uint4 xh0, xh1, xl0, xl1;
-                    xh0 = xh1 = xl0 = xl1 = make_uint4(0, 0, 0, 0);
-                    if (add) {
-                        const uint4* s = rs + (size_t)(c / 8) * L;
-                        xh0 = __ldg(s); xh1 = __ldg(s + L); xl0 = __ldg(s + pl); xl1 = __ldg(s + pl + L);
-                    }
-                    tmem_ld_wait();
-                    if (live) {
-                        const unsigned xh[8] = {xh0.x, xh0.y, xh0.z, xh0.w, xh1.x, xh1.y, xh1.z, xh1.w};
-                        const unsigned xl[8] = {xl0.x, xl0.y, xl0.z, xl0.w, xl1.x, xl1.y, xl1.z, xl1.w};
-                        unsigned hi[8], lo[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const float2 h = unpack_bf16x2(xh[i]), l = unpack_bf16x2(xl[i]);
-                            split2(v[2 * i] + (h.x + l.x), v[2 * i + 1] + (h.y + l.y), hi[i], lo[i]);
-                        }
-                        uint4* o = o0 + (size_t)(c / 8) * L;
-                        o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]); o[L] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                        o[pl] = make_uint4(lo[0], lo[1], lo[2], lo[3]); o[pl + L] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                    }
-                }
+                wgmma_commit();
+                wgmma_wait0();
+                wgmma_keep(acc[0]);
+                wgmma_keep(acc[1]);
+                mbar_arrive(empty + s);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(acc_empty_addr[ab]);
+            if (EPI == EPI_DZ) {
+                const float* fg = reinterpret_cast<const float*>(p.fg) + (size_t)b * (2 * CH / 4) * L * 4;
+                unsigned* dfg = reinterpret_cast<unsigned*>(p.out0 + (size_t)b * 2 * (2 * CH / 8) * L);   // planes of 2CH/8 chunks
+                unsigned* zo = reinterpret_cast<unsigned*>(p.out1 + (size_t)b * 2 * (CH / 8) * L);          // planes of CH/8 chunks
+                const size_t pl_fg = (size_t)(2 * CH / 8) * L * 4, pl_z = (size_t)(CH / 8) * L * 4;       // 32-bit words per plane
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int nb = 0; nb < 16; ++nb) {
+                        const int n = n0 + 128 * h + 8 * nb + q2;          // first of this thread's two dilation channels
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const int t = tf + r0 + 8 * r;
+                            if (t >= p.L) continue;
+                            const float2 f = __ldg(reinterpret_cast<const float2*>(fg + ((size_t)(n / 4) * L + t) * 4 + (n & 3)));
+                            const float2 gg = __ldg(reinterpret_cast<const float2*>(fg + ((size_t)(CH / 4 + n / 4) * L + t) * 4 + (n & 3)));
+                            const float v0 = acc[h][4 * nb + 2 * r], v1 = acc[h][4 * nb + 2 * r + 1];
+                            unsigned fh, fl, gh, gl, zh, zl;
+                            split2(v0 * gg.x * (1.f - f.x * f.x), v1 * gg.y * (1.f - f.y * f.y), fh, fl);
+                            split2(v0 * f.x * gg.x * (1.f - gg.x), v1 * f.y * gg.y * (1.f - gg.y), gh, gl);
+                            split2(f.x * gg.x, f.y * gg.y, zh, zl);
+                            const size_t wf = ((size_t)(n / 8) * L + t) * 4 + (q2 >> 1);
+                            const size_t wg = wf + (size_t)(CH / 8) * L * 4;
+                            dfg[wf] = fh; dfg[wf + pl_fg] = fl;
+                            dfg[wg] = gh; dfg[wg + pl_fg] = gl;
+                            zo[wf] = zh; zo[wf + pl_z] = zl;
+                        }
+                    }
+            } else {
+                const size_t pl = (size_t)(CH / 8) * L * 4;                // 32-bit words per plane
+                const unsigned* rs = p.res ? reinterpret_cast<const unsigned*>(p.res + (size_t)b * 2 * (CH / 8) * L) : nullptr;
+                unsigned* o0 = reinterpret_cast<unsigned*>(p.out0 + (size_t)b * 2 * (CH / 8) * L);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int nb = 0; nb < 16; ++nb) {
+                        const int n = n0 + 128 * h + 8 * nb + q2;          // first of this thread's two residual channels
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const int t = tf + r0 + 8 * r;
+                            if (t >= p.L) continue;
+                            const size_t w = ((size_t)(n / 8) * L + t) * 4 + (q2 >> 1);
+                            float2 x = make_float2(0.f, 0.f);
+                            if (rs != nullptr && t >= p.id_start) {
+                                const float2 xh = unpack_bf16x2(__ldg(rs + w)), xl = unpack_bf16x2(__ldg(rs + w + pl));
+                                x = make_float2(xh.x + xl.x, xh.y + xl.y);
+                            }
+                            unsigned hi, lo;
+                            split2(acc[h][4 * nb + 2 * r] + x.x, acc[h][4 * nb + 2 * r + 1] + x.y, hi, lo);
+                            o0[w] = hi;
+                            o0[w + pl] = lo;
+                        }
+                    }
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync();
-    if (warp == 1) tmem2_dealloc(tmem_base, 512);
 }
 
 // ---------------------------------------------------------------------------------------------- weight packing (backward)
@@ -295,16 +244,17 @@ __global__ void pack_bwd_all_kernel(const float* const* __restrict__ ptrs, __nv_
 
 // ============================================================================================== weight gradients
 constexpr int WG_KF = 32;                         // frames per k-slab: slot image [plane][chunk 16][frame 32][16 B]
-constexpr int WG_NSLOT = 8;
-constexpr int WG_THREADS = 192;                   // warp 0 TMA, warp 1 MMA + TMEM, warps 2-5 epilogue
-constexpr size_t SMEM_WG = 128 + WG_NSLOT * SLOT + 256;
+constexpr int WG_STAGE = 3 * SLOT;                // g box (this CTA's 128 channels) + two x boxes (all 256 channels)
+constexpr int WG_NST = (227 * 1024 - 384) / WG_STAGE;
+constexpr int WG_THREADS = 288;                   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr size_t SMEM_WG = 128 + (size_t)WG_NST * WG_STAGE + 256;
 constexpr int WG_MAX_JOBS = 24;
 
 struct WgJob {
     int g_map, g_chunk0, g_origin;                // g operand: tensor map index, first chunk of the 256-channel M tile, map origin frame
     int x_map, x_origin, x_shift, x_chunk0;       // x operand: frames t + x_shift, first chunk of the 256-channel N tile
     int t_lo, slabs_per_seq, total_slabs;         // frames [t_lo, L) of every sequence, in slabs of 32
-    int split0, n_splits, slabs_per_split;        // clusters [split0, split0 + n_splits) work on this job
+    int split0, n_splits, slabs_per_split;        // CTA pairs [split0, split0 + n_splits) work on this job
     int work_slot0;                               // partial (256 x 256 fp32) index of split 0 in the workspace
 };
 struct WgParams {
@@ -313,112 +263,93 @@ struct WgParams {
     float* work;
 };
 
+// CTA r of a pair computes rows 128r..128r+127 (g channels) x all 256 columns (x channels) of its split's partial
 template <bool PAIR>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad2_kernel(const __grid_constant__ CUtensorMap m0, const __grid_constant__ CUtensorMap m1, const __grid_constant__ CUtensorMap m2,
               const __grid_constant__ CUtensorMap m3, const __grid_constant__ CUtensorMap m4, const WgParams p) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + WG_NSLOT * SLOT);
-    unsigned long long* full = bars;                   // [WG_NSLOT] leader
-    unsigned long long* empty = bars + WG_NSLOT;       // [WG_NSLOT] per CTA
-    unsigned long long* acc_full = bars + 2 * WG_NSLOT;
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(acc_full + 1);
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(ring + WG_NST * WG_STAGE);
+    unsigned long long* full = bars;                   // [WG_NST]
+    unsigned long long* empty = bars + WG_NST;         // [WG_NST]
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const unsigned rank = cluster_rank();
-    const int cluster_id = blockIdx.x >> 1;
-    // which job / split is this cluster's
+    const int rank = (int)(blockIdx.x & 1);
+    const int pair_id = blockIdx.x >> 1;
+    // which job / split is this pair's
     int ji = -1;
     for (int j = 0; j < p.n_jobs; ++j)
-        if (cluster_id >= p.job[j].split0 && cluster_id < p.job[j].split0 + p.job[j].n_splits) ji = j;
+        if (pair_id >= p.job[j].split0 && pair_id < p.job[j].split0 + p.job[j].n_splits) ji = j;
     const WgJob jb = p.job[ji < 0 ? 0 : ji];
-    const int sp = cluster_id - jb.split0;
+    const int sp = pair_id - jb.split0;
     const int s_beg = ji < 0 ? 0 : sp * jb.slabs_per_split;
     const int s_end = ji < 0 ? 0 : (s_beg + jb.slabs_per_split < jb.total_slabs ? s_beg + jb.slabs_per_split : jb.total_slabs);
     const int n_slabs = s_end > s_beg ? s_end - s_beg : 0;
     if (tid == 0) {
-        for (int i = 0; i < WG_NSLOT; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
-        mbar_init(acc_full, 1);
+        for (int i = 0; i < WG_NST; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, CONSUMERS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem2_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
     auto map_of = [&](int i) -> const CUtensorMap* { return i == 0 ? &m0 : (i == 1 ? &m1 : (i == 2 ? &m2 : (i == 3 ? &m3 : &m4))); };
+    constexpr int BOX = PAIR ? SLOT : SLOT / 2;        // bytes of one {32 frames, 16 chunks, planes} box
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (warp == EPI_WARPS) {
+        if (lane == 0) {
             const CUtensorMap* gm = map_of(jb.g_map);
             const CUtensorMap* xm = map_of(jb.x_map);
-            unsigned it = 0;
             for (int i = 0; i < n_slabs; ++i) {
                 const int s = s_beg + i, b = s / jb.slabs_per_seq, t0 = jb.t_lo + (s % jb.slabs_per_seq) * WG_KF;
-                for (int which = 0; which < 2; ++which, ++it) {
-                    const unsigned sl = it % WG_NSLOT, ph = (it / WG_NSLOT) & 1;
-                    mbar_wait(empty + sl, ph ^ 1);
-                    if (rank == 0) mbar_expect_tx(full + sl, PAIR ? 2 * SLOT : SLOT);          // single pass: the hi plane only
-                    const unsigned bar = mapa(s32(full + sl), 0);
-                    if (which == 0) tma2_load_4d(ring + sl * SLOT, gm, 2 * (t0 - jb.g_origin), jb.g_chunk0 + 16 * (int)rank, 0, b, bar);
-                    else tma2_load_4d(ring + sl * SLOT, xm, 2 * (t0 + jb.x_shift - jb.x_origin), jb.x_chunk0 + 16 * (int)rank, 0, b, bar);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0 && n_slabs > 0) {
-            constexpr unsigned idesc = make_idesc_bf16(PM, 256, 1, 1);            // both operands MN-major
-            constexpr unsigned KLBO = 128, KSBO = WG_KF * 16;                      // 8-frame groups / 8-channel chunks
-            unsigned it = 0;
-            for (int i = 0; i < n_slabs; ++i) {
-                const unsigned sg = it % WG_NSLOT, pg = (it / WG_NSLOT) & 1; ++it;
-                const unsigned sx = it % WG_NSLOT, pxx = (it / WG_NSLOT) & 1; ++it;
-                mbar_wait_cluster(full + sg, pg);
-                mbar_wait_cluster(full + sx, pxx);
-                tc_fence_after();
-                if (elect_one()) {
-                    const unsigned g = s32(ring + sg * SLOT), x = s32(ring + sx * SLOT);
-#pragma unroll
-                    for (int ks = 0; ks < WG_KF / 16; ++ks) {
-                        const unsigned long long gh = smem_desc(g + ks * 2 * KLBO, KLBO, KSBO), xh = smem_desc(x + ks * 2 * KLBO, KLBO, KSBO);
-                        umma2_f16(tmem_base, gh, xh, idesc, (i | ks) != 0);
-                        if constexpr (PAIR) {
-                            umma2_f16(tmem_base, smem_desc(g + SLOT / 2 + ks * 2 * KLBO, KLBO, KSBO), xh, idesc, 1);
-                            umma2_f16(tmem_base, gh, smem_desc(x + SLOT / 2 + ks * 2 * KLBO, KLBO, KSBO), idesc, 1);
-                        }
-                    }
-                    umma2_commit(empty + sg);
-                    umma2_commit(empty + sx);
-                    if (i == n_slabs - 1) umma2_commit(acc_full);
-                }
-                __syncwarp();
+                const unsigned st = i % WG_NST, ph = (i / WG_NST) & 1;
+                mbar_wait(empty + st, ph ^ 1);
+                mbar_expect_tx(full + st, 3 * BOX);
+                unsigned char* dst = ring + st * WG_STAGE;
+                tma_load_4d(dst, gm, 2 * (t0 - jb.g_origin), jb.g_chunk0 + 16 * rank, 0, b, full + st);
+                for (int h = 0; h < 2; ++h)
+                    tma_load_4d(dst + (1 + h) * SLOT, xm, 2 * (t0 + jb.x_shift - jb.x_origin), jb.x_chunk0 + 16 * h, 0, b, full + st);
             }
         }
     } else if (ji >= 0) {
-        // epilogue: partial[row n = rank*128 + q*32 + lane][256 columns] -> workspace
-        const int q = warp & 3;
-        float* out = p.work + ((size_t)(jb.work_slot0 + sp) * 256 + rank * 128 + q * 32 + lane) * 256;
-        if (n_slabs > 0) {
-            mbar_wait(acc_full, 0);
-            tc_fence_after();
-            const unsigned ta = tmem_base + ((unsigned)(q * 32) << 16);
-#pragma unroll 1
-            for (int c = 0; c < 256; c += 16) {
-                float v[16];
-                tmem_ld16(ta + c, v);
-                tmem_ld_wait();
+        // consumer warpgroup g: rows 64g..64g+63 of this CTA's 128 (= chunks 8g..8g+7 of the g box), both operands MN-major
+        constexpr unsigned KLBO = 128, KSBO = WG_KF * 16;               // 8-frame groups / 8-channel chunks
+        const int g = warp >> 2;
+        float acc[2][64];
+        for (int i = 0; i < n_slabs; ++i) {
+            const unsigned s = i % WG_NST, ph = (i / WG_NST) & 1;
+            mbar_wait(full + s, ph);
+            const unsigned st = s32(ring + s * WG_STAGE);
+            const unsigned ga = st + (unsigned)g * 8 * KSBO;
+            wgmma_fence();
 #pragma unroll
-                for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(out + c + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-            }
-        } else {
-            for (int c = 0; c < 256; c += 4) *reinterpret_cast<float4*>(out + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int ks = 0; ks < WG_KF / 16; ++ks)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const unsigned xa = st + (1 + h) * SLOT;
+                    const unsigned long long gh = wg_desc(ga + ks * 2 * KLBO, KLBO, KSBO), xh = wg_desc(xa + ks * 2 * KLBO, KLBO, KSBO);
+                    wgmma_bf16_t11(acc[h], gh, xh, (i == 0 && ks == 0) ? 0u : 1u);
+                    if constexpr (PAIR) {
+                        wgmma_bf16_t11(acc[h], wg_desc(ga + BOX / 2 + ks * 2 * KLBO, KLBO, KSBO), xh, 1u);
+                        wgmma_bf16_t11(acc[h], gh, wg_desc(xa + BOX / 2 + ks * 2 * KLBO, KLBO, KSBO), 1u);
+                    }
+                }
+            wgmma_commit();
+            wgmma_wait0();
+            wgmma_keep(acc[0]);
+            wgmma_keep(acc[1]);
+            mbar_arrive(empty + s);
         }
+        // partial[row n = rank*128 + r][256 columns] -> workspace
+        const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2), q2 = 2 * (lane & 3);
+        float* out = p.work + ((size_t)(jb.work_slot0 + sp) * 256 + rank * 128) * 256;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float2 v = n_slabs > 0 ? make_float2(acc[h][4 * nb + 2 * r], acc[h][4 * nb + 2 * r + 1]) : make_float2(0.f, 0.f);
+                    *reinterpret_cast<float2*>(out + (size_t)(r0 + 8 * r) * 256 + 128 * h + 8 * nb + q2) = v;
+                }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync();
-    if (warp == 1) tmem2_dealloc(tmem_base, 256);
 }
 
 struct WgOut { float* dst; long long n_stride, c_stride; int work_slot0, n_splits; };
@@ -482,10 +413,6 @@ static int launch_pg(const CUtensorMap& a0, const CUtensorMap& a1, const CUtenso
     cfg.blockDim = dim3(tb2::NTHREADS);
     cfg.dynamicSmemBytes = tb2::SMEM_PG;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
     WN_CUDA(cudaLaunchKernelEx(&cfg, tb2::pair_gemm_kernel<C, EPI>, a0, a1, w, p));
     WN_CUDA(cudaGetLastError());
     return 0;
@@ -605,7 +532,7 @@ extern "C" int wn_tb_wgrad(const wn_tb_wgrad_args* a, void* stream) {
         add(2, CH / 8, a->gz, 4, a->in_start, -sh, lo, a->d_gwg + tap, 2 * CC, 2);     // gate.weight
     }
     p.n_jobs = rp.n_jobs = nj;
-    // clusters per job proportional to its slabs (at least 1), one wave of sms/2 clusters
+    // CTA pairs per job proportional to its slabs (at least 1), one wave of sms/2 pairs
     const int n_clusters = sms / 2;
     long long total = 0;
     for (int j = 0; j < nj; ++j) total += p.job[j].total_slabs > 0 ? p.job[j].total_slabs : 1;
@@ -628,10 +555,6 @@ extern "C" int wn_tb_wgrad(const wn_tb_wgrad_args* a, void* stream) {
     cfg.blockDim = dim3(tb2::WG_THREADS);
     cfg.dynamicSmemBytes = tb2::SMEM_WG;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
     if (pair) {
         WN_CUDA(cudaFuncSetAttribute(tb2::wgrad2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb2::SMEM_WG));
         WN_CUDA(cudaLaunchKernelEx(&cfg, tb2::wgrad2_kernel<true>, m[0], m[1], m[2], m[3], m[4], p));

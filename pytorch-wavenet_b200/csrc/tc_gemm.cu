@@ -1,5 +1,5 @@
-// tc_gemm.cu -- tensor-core (tcgen05 / TMEM / TMA) form of the training block: exact-fp32-class numerics through
-// 3xTF32 (hi/lo split of both operands, fp32 accumulation in tensor memory).
+// tc_gemm.cu -- tensor-core (wgmma / TMA) form of the training block: exact-fp32-class numerics through
+// 3xTF32 (hi/lo split of both operands, fp32 accumulation in registers).
 //
 // Same mathematics and frames layout as train_fwd.cu (reference wavenet_model.py:142-165), split in two launches
 // per block because the gated activation cannot stay on chip in split form (128 frames x 256 ch x {hi,lo} = 256 KB):
@@ -7,14 +7,14 @@
 //            the dilation; frames left of in_start come back as zeros from the TMA out-of-bounds fill)
 //            epilogue: z = tanh(F+bf) * sigmoid(G+bg)  -> z (B,L,D)  [+ optional f,g for the backward]
 //   pass B   [O|S][128 x 256] per tile = z[128 x D] * Wb^T ;  h_out = O + br + h_in,  skip (+)= S + bs
-// Kernel anatomy (one CTA per SM, persistent over (sequence, 128-frame tile) items, 448 threads):
-//   warp 0        TMA producer: per K slab (16 fp32 = one 64-byte swizzle row) loads A raw, W_hi, W_lo (4-stage ring)
-//   warp 1        allocates TMEM, issues tcgen05.mma kind::tf32 (M128 N256 K8): hi*hi + lo*hi + hi*lo per k-step
-//   warps 2,3,8,9 splitter: rewrite the landed A slab as hi = rna_tf32(x) in place and lo = x - hi in a second buffer
-//   warps 4-7,10-13 epilogue (2 groups x 4 TMEM lane quadrants): tcgen05.ld the finished accumulator (2 x 256 TMEM
-//                 columns, double buffered), apply gate / residual / skip, store whole sectors
-// mbarriers: full (TMA landed), split (lo ready), empty (MMAs of the stage retired), acc_full / acc_empty.
+// Kernel anatomy (one CTA per SM, persistent over (sequence, 128-frame tile) items, 288 threads):
+//   warp 8        TMA producer: per K slab (16 fp32 = one 64-byte swizzle row) loads A raw, W_hi, W_lo (4-stage ring)
+//   warps 0-7     two consumer warpgroups, each owning 64 of the 128 frames: split the warpgroup's rows of the landed A
+//                 slab into hi = rna_tf32(x) (in place) and lo = x - hi, issue wgmma m64n128k8 tf32 (hi*hi + lo*hi + hi*lo
+//                 per k-step) into two 128-column register accumulators, then apply gate / residual / skip from the fragments
+// mbarriers: full (TMA landed), empty (every consumer thread is done with the stage).
 #include "common.cuh"
+#include "tc_ptx.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -22,13 +22,11 @@
 
 namespace wn {
 namespace tc {
+using namespace px;
 
 constexpr int BM = 128;            // frames per tile (UMMA M)
 constexpr int BN = 256;            // output columns per tile (UMMA N)
-constexpr int BK = 16;             // fp32 per K slab = 64 bytes = one 64B-swizzle row (two k-steps of 8).  Measured on B200:
-                                   // 128B rows x 2 stages 36.4 ms, 64B x 4 stages 27.7 ms, 32B x 8 stages 33.5 ms per cfg-3
-                                   // forward -- a stage slot needs ~3500 cycles to come round (TMA ~1900, split ~700), so
-                                   // depth matters, but TMA latency grows again when the boxes get too small
+constexpr int BK = 16;             // fp32 per K slab = 64 bytes = one 64B-swizzle row (two k-steps of 8)
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 4;          // 8 KB
 constexpr int W_BYTES = BN * BK * 4;          // 16 KB
@@ -40,115 +38,12 @@ constexpr int ABF_BYTES = BM * BK * 2;        // 4 KB
 constexpr int WBF_BYTES = BN * BK * 2;        // 8 KB
 constexpr int STAGE_BYTES_BF = A_BYTES + 2 * ABF_BYTES + 2 * WBF_BYTES;     // 32 KB
 enum { PREC_TF32X3 = 0, PREC_TF32X1 = 1, PREC_BF16X2 = 2 };
-constexpr int NTHREADS = 448;             // 14 warps: TMA, MMA, 4 split (2,3,8,9), 2 x 4 epilogue (4-7 and 10-13)
-constexpr int EPI_THREADS = 256;
-constexpr int SPLIT_THREADS = 128;
-constexpr int CS = 2;                       // CTAs per cluster sharing every weight slab through TMA multicast
-constexpr int TP = 20;                      // pitch of the 32x16 epilogue transpose tile (16-byte aligned rows)
-constexpr unsigned SPIN_LIMIT = 1u << 28;     // a barrier that never completes traps instead of hanging the GPU
+constexpr int NTHREADS = 288;             // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int CONSUMERS = 256;
 
-// ---------------------------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned n) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(b)), "r"(n) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* b) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* b, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity) {
-    unsigned done, spins = 0;
-    do {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(done) : "r"(s32(b)), "r"(parity) : "memory");
-        if (!done && ++spins > SPIN_LIMIT) asm volatile("trap;");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2,
-                                            unsigned long long* bar) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(s32(bar)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(s32(bar)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, int c0, int c1, unsigned long long* bar,
-                                               unsigned short mask) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
-                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(s32(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(unsigned long long* bar, unsigned short mask) {   // arrive on `bar` of every CTA in mask
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(s32(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ unsigned cluster_rank_() {
-    unsigned r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc(unsigned* slot_in_smem, unsigned cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(slot_in_smem)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(unsigned addr, unsigned cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_tf32(unsigned d_tmem, unsigned long long a_desc, unsigned long long b_desc, unsigned idesc,
-                                          unsigned accumulate) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p; }"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_f16(unsigned d_tmem, unsigned long long a_desc, unsigned long long b_desc, unsigned idesc,
-                                         unsigned accumulate) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p; }"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {       // arrives when all prior MMAs of this thread retire
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, float (&v)[16]) {
-    unsigned r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                   "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-    unsigned pred;
-    asm volatile("{ .reg .pred p; elect.sync _|p, 0xffffffff; selp.u32 %0, 1, 0, p; }" : "=r"(pred));
-    return pred != 0;
-}
-
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): K-major rows of BK*4 bytes with the matching swizzle
-// (64B rows -> SWIZZLE_64B, 128B rows -> SWIZZLE_128B); 8-row atoms are 8*row_bytes apart
-template <unsigned row_bytes = BK * 4>
-__device__ __forceinline__ unsigned long long smem_desc(unsigned saddr) {
-    constexpr unsigned long long layout = (row_bytes == 128) ? 2ull : (row_bytes == 64 ? 4ull : 6ull);   // SWIZZLE_128B/64B/32B
-    unsigned long long d = 0;
-    d |= (unsigned long long)((saddr >> 4) & 0x3fff);            // start address, 16-byte units
-    d |= (unsigned long long)1 << 16;                            // leading byte offset (unused for swizzled K-major)
-    d |= (unsigned long long)((8 * row_bytes) >> 4) << 32;       // stride byte offset between 8-row atoms
-    d |= (unsigned long long)1 << 46;                            // descriptor version (Blackwell)
-    d |= layout << 61;
-    return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D f32, A/B tf32 (format 2, kind::tf32) or bf16 (format 1,
-// kind::f16), both K-major, M=128, N=256
-__host__ __device__ constexpr unsigned make_idesc(bool bf16 = false) {
-    return (1u << 4) | ((bf16 ? 1u : 2u) << 7) | ((bf16 ? 1u : 2u) << 10) | ((unsigned)(BN >> 3) << 17) | ((unsigned)(BM >> 4) << 24);
-}
+// swizzled K-major descriptors (layout 2 = 64B, 3 = 32B swizzle): sbo = bytes between 8-row atoms
+__device__ __forceinline__ unsigned long long desc64(unsigned saddr) { return wg_desc(saddr, 16, 8 * 64, 2); }
+__device__ __forceinline__ unsigned long long desc32(unsigned saddr) { return wg_desc(saddr, 16, 8 * 32, 3); }
 
 // ---------------------------------------------------------------------------------------------- kernel
 enum { EPI_GATE = 0, EPI_RES_SKIP = 1, EPI_GATE_BWD = 2, EPI_ADD = 3 };
@@ -175,7 +70,7 @@ struct TcParams {
 __device__ __forceinline__ float sigmoid_tc(float x) { return 1.f / (1.f + expf(-x)); }
 
 // PREC_TF32X3: 3xTF32 (hi*hi + lo*hi + hi*lo, hi = rna_tf32(x)): ~6e-7 on the logits after 50 layers.
-// PREC_BF16X2: both operands as bf16 pairs (hi = bf16(x), lo = bf16(x - hi)), the same three products on kind::f16 at
+// PREC_BF16X2: both operands as bf16 pairs (hi = bf16(x), lo = bf16(x - hi)), the same three products on bf16 MMAs at
 //              twice the tf32 rate: 16 mantissa bits per operand, ~3e-6 on the logits after 50 layers (inside the 1e-4 bar).
 // PREC_TF32X1: one TF32 MMA per k-step on the raw fp32 operands (the tensor core drops the low mantissa bits):
 //              ~1e-3 relative on the logits after 50 layers, i.e. outside the parity bar; opt-in, reported separately.
@@ -187,62 +82,42 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     constexpr bool BF = PREC == PREC_BF16X2;
     constexpr int ST = BF ? STAGES_BF : STAGES;                // ring depth
     constexpr int SB = BF ? STAGE_BYTES_BF : STAGE_BYTES;      // bytes per stage
-    // mapW's box is BN/CS rows: every CTA of the cluster fetches its share of a weight slab and multicasts it to all
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* stage_mem = base;                                           // ST * SB
     unsigned long long* bars = reinterpret_cast<unsigned long long*>(base + ST * SB);
     unsigned long long* full = bars;                 // [ST]
-    unsigned long long* split = bars + ST;           // [ST]
-    unsigned long long* empty = bars + 2 * ST;       // [ST]
-    unsigned long long* acc_full = bars + 3 * ST;          // [2]
-    unsigned long long* acc_empty = bars + 3 * ST + 2;     // [2]
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(bars + 3 * ST + 4);
+    unsigned long long* empty = bars + ST;           // [ST]
     float* bias_s = reinterpret_cast<float*>(base + ST * SB + 512);                                // [n_total]
-    float* stage_t = bias_s + ((p.n_total + 3) & ~3);                          // [4 warps][32][TP] epilogue transpose tiles
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m_tiles = (p.L - p.t_begin + BM - 1) / BM;
-    const int items = p.B * m_tiles;
-    // Work: item (sequence b, 128-frame tile) number (cluster + round * n_clusters) * CS + rank.  The CTAs of a cluster walk
-    // the same (output tile, K slab) sequence in lockstep because they share the weight slabs; a CTA whose item does not
-    // exist runs a ghost tile (frames beyond L: TMA zero fill, no stores) so that it keeps feeding its peers.
-    const int crank = (int)cluster_rank_(), n_clusters = gridDim.x / CS, cluster_id = blockIdx.x / CS;
-    const int rounds = (items + n_clusters * CS - 1) / (n_clusters * CS);
-    const unsigned short mc_mask = (unsigned short)((1u << CS) - 1u);
+    const int items = p.B * m_tiles;                            // item = (sequence b, 128-frame tile), dealt round-robin to the CTAs
     const int slabs_per_tap = p.C / BK;
     const int slabs1 = p.taps * slabs_per_tap;                  // K slabs of the first A source
     const int slabs = slabs1 + p.C2 / BK;
 
-    if (warp == 0 && lane == 0) {
-        for (int i = 0; i < ST; ++i) { mbar_init(full + i, 1); mbar_init(split + i, SPLIT_THREADS); mbar_init(empty + i, CS); }
-        for (int i = 0; i < 2; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, EPI_THREADS); }
+    if (tid == 0) {
+        for (int i = 0; i < ST; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, CONSUMERS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
     for (int i = tid; i < p.n_total; i += NTHREADS) bias_s[i] = p.bias ? p.bias[i] : 0.f;
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_();                              // peers' barriers are initialised before anything is multicast at them
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================================================================= TMA producer
-        if (elect_one()) {
+        if (lane == 0) {
             unsigned it = 0;
-            for (int rd = 0; rd < rounds; ++rd) {
-                const int item = (cluster_id + rd * n_clusters) * CS + crank;
-                const bool ghost = item >= items;
-                const int b = ghost ? 0 : item / m_tiles, t0 = ghost ? p.L : p.t_begin + (item % m_tiles) * BM;
+            for (int item = blockIdx.x; item < items; item += gridDim.x) {
+                const int b = item / m_tiles, t0 = p.t_begin + (item % m_tiles) * BM;
                 for (int nt = 0; nt < p.n_tiles; ++nt)
                     for (int sl = 0; sl < slabs; ++sl, ++it) {
                         const int st = it % ST;
                         const unsigned ph = (it / ST) & 1;
                         if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it * 8 + 0] = clock64();
-                        mbar_wait(empty + st, ph ^ 1);           // every CTA of the cluster is done with this stage
+                        mbar_wait(empty + st, ph ^ 1);
                         if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it * 8 + 1] = clock64();
                         unsigned char* sm = stage_mem + st * SB;
                         mbar_expect_tx(full + st, BF ? A_BYTES + 2 * WBF_BYTES : A_BYTES + (EXACT ? 2 : 1) * W_BYTES);
@@ -252,84 +127,43 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         } else {
                             tma_load_3d(sm, &mapA2, (sl - slabs1) * BK, t0 - p.a2_origin, b, full + st);
                         }
-                        constexpr int WR = BN / CS;                          // this CTA's rows of the slab
                         constexpr int WT = BF ? WBF_BYTES : W_BYTES;        // bytes of one weight tile (hi or lo)
                         constexpr int W0 = BF ? A_BYTES + 2 * ABF_BYTES : 2 * A_BYTES;      // offset of W_hi in the stage
-                        tma_load_2d_mc(sm + W0 + crank * (WT / CS), &mapW, sl * BK, nt * BN + crank * WR, full + st, mc_mask);
-                        if (EXACT || BF)
-                            tma_load_2d_mc(sm + W0 + WT + crank * (WT / CS), &mapW, sl * BK, p.n_total + nt * BN + crank * WR,
-                                           full + st, mc_mask);
+                        for (int h = 0; h < 2; ++h) {                       // the map's box is 128 rows: two per tile
+                            tma_load_2d(sm + W0 + h * (WT / 2), &mapW, sl * BK, nt * BN + h * 128, full + st);
+                            if (EXACT || BF)
+                                tma_load_2d(sm + W0 + WT + h * (WT / 2), &mapW, sl * BK, p.n_total + nt * BN + h * 128, full + st);
+                        }
                     }
             }
         }
-    } else if (warp == 1) {
-        // ================================================================= MMA issuer
-        constexpr unsigned idesc = make_idesc(BF);
-        unsigned it = 0, tile = 0;
-        for (int rd = 0; rd < rounds; ++rd)
-            for (int nt = 0; nt < p.n_tiles; ++nt, ++tile) {
-                const unsigned ab = tile & 1, aph = (tile >> 1) & 1;
-                mbar_wait(acc_empty + ab, aph ^ 1);
-                tc_fence_after();
-                const unsigned d_tmem = tmem_base + ab * BN;
-                for (int sl = 0; sl < slabs; ++sl, ++it) {
-                    const int st = it % ST;
-                    const unsigned ph = (it / ST) & 1;
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && lane == 0) p.dbg[it * 8 + 2] = clock64();
-                    mbar_wait(split + st, ph);                   // TMA landed and the splitter produced hi/lo
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && lane == 0) p.dbg[it * 8 + 3] = clock64();
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const unsigned sa = s32(stage_mem + st * SB);
-                        if constexpr (BF) {
-                            // one k-step per slab: 16 bf16 = one 32-byte swizzle row
-                            const unsigned long long a_hi = smem_desc<32>(sa + A_BYTES), a_lo = smem_desc<32>(sa + A_BYTES + ABF_BYTES);
-                            const unsigned long long w_hi = smem_desc<32>(sa + A_BYTES + 2 * ABF_BYTES);
-                            const unsigned long long w_lo = smem_desc<32>(sa + A_BYTES + 2 * ABF_BYTES + WBF_BYTES);
-                            umma_f16(d_tmem, a_hi, w_hi, idesc, sl != 0);
-                            umma_f16(d_tmem, a_lo, w_hi, idesc, 1);
-                            umma_f16(d_tmem, a_hi, w_lo, idesc, 1);
-                        } else {
-                            const unsigned long long a_hi = smem_desc(sa), a_lo = smem_desc(sa + A_BYTES);
-                            const unsigned long long w_hi = smem_desc(sa + 2 * A_BYTES), w_lo = smem_desc(sa + 2 * A_BYTES + W_BYTES);
-#pragma unroll
-                            for (int kk = 0; kk < BK / 8; ++kk) {    // 8 tf32 = 32 bytes = 2 descriptor units per k-step
-                                const unsigned long long o = (unsigned long long)(kk * 2);
-                                umma_tf32(d_tmem, a_hi + o, w_hi + o, idesc, (sl | kk) != 0);
-                                if (EXACT) {
-                                    umma_tf32(d_tmem, a_lo + o, w_hi + o, idesc, 1);
-                                    umma_tf32(d_tmem, a_hi + o, w_lo + o, idesc, 1);
-                                }
-                            }
-                        }
-                        umma_commit_mc(empty + st, mc_mask);     // stage reusable (in every CTA) once these MMAs retire
-                        if (sl == slabs - 1) umma_commit(acc_full + ab);
-                    }
-                    __syncwarp();
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && lane == 0) p.dbg[it * 8 + 4] = clock64();
-                }
-            }
-    } else if (warp == 2 || warp == 3 || warp == 8 || warp == 9) {
-        // ================================================================= splitter (warps 2,3,8,9 = 128 threads)
-        const int st_tid = warp < 4 ? tid - 64 : tid - 192;
+    } else {
+        // ================================================================= consumers: warpgroup g = warps 4g..4g+3, frames 64g..64g+63
+        const int g = warp >> 2, gtid = tid & 127;
+        const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);        // fragment rows r0, r0 + 8
+        const int q2 = 2 * (lane & 3);                                 // fragment columns q2, q2 + 1 of every 8-column group
+        float acc[2][64];
         unsigned it = 0;
-        for (int rd = 0; rd < rounds; ++rd)
-            for (int nt = 0; nt < p.n_tiles; ++nt)
+        for (int item = blockIdx.x; item < items; item += gridDim.x) {
+            const int b = item / m_tiles, t0 = p.t_begin + (item % m_tiles) * BM;
+            for (int nt = 0; nt < p.n_tiles; ++nt) {
                 for (int sl = 0; sl < slabs; ++sl, ++it) {
                     const int st = it % ST;
                     const unsigned ph = (it / ST) & 1;
+                    if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 2] = clock64();
                     mbar_wait(full + st, ph);
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && st_tid == 0) p.dbg[it * 8 + 5] = clock64();
-                    float4* hi = reinterpret_cast<float4*>(stage_mem + st * SB);
-                    float4* lo = reinterpret_cast<float4*>(stage_mem + st * SB + A_BYTES);
+                    if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 3] = clock64();
+                    unsigned char* sm = stage_mem + st * SB;
+                    // ---- split this warpgroup's 64 rows of the raw A slab (rows are 64 bytes = 4 float4)
                     if constexpr (BF) {
                         // raw slab: 128 rows x 64 bytes, 64B-swizzled by the TMA (16-byte chunk c of row r sits at c ^ ((r>>1)&3));
                         // operand tiles: 128 rows x 32 bytes of bf16, 32B swizzle (chunk c of row r sits at c ^ ((r>>2)&1))
-                        unsigned char* ahi = stage_mem + st * SB + A_BYTES;
+                        const float4* raw = reinterpret_cast<const float4*>(sm);
+                        unsigned char* ahi = sm + A_BYTES;
                         unsigned char* alo = ahi + ABF_BYTES;
 #pragma unroll
-                        for (int i = st_tid; i < A_BYTES / 16; i += SPLIT_THREADS) {
-                            const float4 x = hi[i];
+                        for (int i = g * 256 + gtid; i < g * 256 + 256; i += 128) {
+                            const float4 x = raw[i];
                             const int row = i >> 2, lch = (i & 3) ^ ((row >> 1) & 3);      // logical chunk: fp32 k = 4*lch .. 4*lch+3
                             const __nv_bfloat162 h01 = __floats2bfloat162_rn(x.x, x.y), h23 = __floats2bfloat162_rn(x.z, x.w);
                             const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
@@ -343,203 +177,122 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                             *reinterpret_cast<uint2*>(alo + off) = lv;
                         }
                     }
+                    if constexpr (EXACT) {
+                        float4* hi = reinterpret_cast<float4*>(sm);
+                        float4* lo = reinterpret_cast<float4*>(sm + A_BYTES);
 #pragma unroll
-                    for (int i = st_tid; EXACT && i < A_BYTES / 16; i += SPLIT_THREADS) {
-                        const float4 x = hi[i];
-                        float4 h, l;
-                        unsigned u;
-                        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.x)); h.x = __uint_as_float(u); l.x = x.x - h.x;
-                        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.y)); h.y = __uint_as_float(u); l.y = x.y - h.y;
-                        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.z)); h.z = __uint_as_float(u); l.z = x.z - h.z;
-                        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.w)); h.w = __uint_as_float(u); l.w = x.w - h.w;
-                        hi[i] = h;
-                        lo[i] = l;
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> visible to the MMA
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && st_tid == 0) p.dbg[it * 8 + 6] = clock64();
-                    if (p.dbg && blockIdx.x == 0 && it < 512 && warp == 9 && lane == 0) p.dbg[it * 8 + 7] = clock64();   // last splitter warp
-                    mbar_arrive(split + st);
-                }
-    } else if ((warp >= 4 && warp < 8) || warp >= 10) {
-        // ================================================================= epilogue: two groups of 4 warps (4-7 and 10-13); warp w may
-        // touch TMEM lanes 32*(w%4)..+31, so each group covers all 128 accumulator rows and takes half of the tile's columns.
-        // A 16-column chunk is read row-per-thread, turned through a 32x16 shared-memory tile and leaves as 64-byte row pieces
-        // (instruction i: lane -> frame 8i + lane/4, 16-byte piece lane%4): whole sectors, 8 rows per warp instruction.
-        const int grp = warp >= 10 ? 1 : 0, q = warp & 3;
-        float* tt = stage_t + (grp * 4 + q) * 32 * TP;
-        const int sub_r = lane >> 2, sub_c = (lane & 3) * 4;
-        unsigned tile = 0;
-        for (int rd = 0; rd < rounds; ++rd) {
-            const int item = (cluster_id + rd * n_clusters) * CS + crank;
-            const bool ghost = item >= items;
-            const int b = ghost ? 0 : item / m_tiles, t0 = ghost ? p.L : p.t_begin + (item % m_tiles) * BM;
-            const int tbase = t0 + q * 32;                                   // first frame of this warp's rows
-            for (int nt = 0; nt < p.n_tiles; ++nt, ++tile) {
-                const unsigned ab = tile & 1, aph = (tile >> 1) & 1;
-                mbar_wait(acc_full + ab, aph);
-                tc_fence_after();
-                const unsigned taddr = tmem_base + ab * BN + ((unsigned)(q * 32) << 16);
-                if (EPI == EPI_GATE) {
-                    // tile columns: [0,128) = F of channels 128*nt.., [128,256) = G of the same channels; group g takes 64 channels
-                    const float* bt = bias_s + nt * BN;
-#pragma unroll 1
-                    for (int c = grp * 64; c < grp * 64 + 64; c += 16) {
-                        float f[16], g[16];
-                        tmem_ld16(taddr + c, f);
-                        tmem_ld16(taddr + 128 + c, g);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            f[i] = tanhf(f[i] + bt[c + i]);
-                            g[i] = sigmoid_tc(g[i] + bt[128 + c + i]);
+                        for (int i = g * 256 + gtid; i < g * 256 + 256; i += 128) {
+                            const float4 x = hi[i];
+                            float4 h, l;
+                            unsigned u;
+                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.x)); h.x = __uint_as_float(u); l.x = x.x - h.x;
+                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.y)); h.y = __uint_as_float(u); l.y = x.y - h.y;
+                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.z)); h.z = __uint_as_float(u); l.z = x.z - h.z;
+                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.w)); h.w = __uint_as_float(u); l.w = x.w - h.w;
+                            hi[i] = h;
+                            lo[i] = l;
                         }
-                        const int n_pass = p.out1 ? 3 : 1;                   // z, then (optionally) f and g for the backward
-                        for (int ps = 0; ps < n_pass; ++ps) {
-                            __syncwarp();
+                    }
+                    if constexpr (EXACT || BF) {
+                        fence_async_smem();                       // generic writes -> visible to the MMA
+                        wg_bar(1 + g, 128);
+                    }
+                    if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 4] = clock64();
+                    // ---- MMAs of this warpgroup's 64 rows against both 128-row halves of the weight tile
+                    const unsigned sa = s32(sm);
+                    wgmma_fence();
+                    if constexpr (BF) {
+                        const unsigned a_hi = sa + A_BYTES + g * 64 * 32, a_lo = a_hi + ABF_BYTES;
 #pragma unroll
-                            for (int i = 0; i < 16; i += 4) {
-                                float4 v;
-                                if (ps == 0) v = make_float4(f[i] * g[i], f[i + 1] * g[i + 1], f[i + 2] * g[i + 2], f[i + 3] * g[i + 3]);
-                                else if (ps == 1) v = make_float4(f[i], f[i + 1], f[i + 2], f[i + 3]);
-                                else v = make_float4(g[i], g[i + 1], g[i + 2], g[i + 3]);
-                                *reinterpret_cast<float4*>(tt + lane * TP + i) = v;
+                        for (int h = 0; h < 2; ++h) {
+                            const unsigned w_hi = sa + A_BYTES + 2 * ABF_BYTES + h * (WBF_BYTES / 2), w_lo = w_hi + WBF_BYTES;
+                            wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_hi), sl != 0);
+                            wgmma_bf16_t00(acc[h], desc32(a_lo), desc32(w_hi), 1u);
+                            wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_lo), 1u);
+                        }
+                    } else {
+                        const unsigned a_hi = sa + g * 64 * 64, a_lo = a_hi + A_BYTES;
+#pragma unroll
+                        for (int kk = 0; kk < BK / 8; ++kk)          // 8 tf32 = 32 bytes per k-step
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const unsigned w_hi = sa + 2 * A_BYTES + h * (W_BYTES / 2) + kk * 32, w_lo = w_hi + W_BYTES;
+                                wgmma_tf32(acc[h], desc64(a_hi + kk * 32), desc64(w_hi), (sl | kk) != 0);
+                                if (EXACT) {
+                                    wgmma_tf32(acc[h], desc64(a_lo + kk * 32), desc64(w_hi), 1u);
+                                    wgmma_tf32(acc[h], desc64(a_hi + kk * 32), desc64(w_lo), 1u);
+                                }
                             }
-                            __syncwarp();
+                    }
+                    wgmma_commit();
+                    wgmma_wait0();
+                    wgmma_keep(acc[0]);
+                    wgmma_keep(acc[1]);
+                    mbar_arrive(empty + st);                     // stage reusable once every consumer thread got here
+                    if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 5] = clock64();
+                }
+                // ================================================================= epilogue from the fragments
+                const int n0 = nt * BN;
+                const int Tsk = p.L - p.skip_start;
 #pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int fr = tbase + 8 * i + sub_r;
-                                if (fr < p.L) {
-                                    const float4 v = *reinterpret_cast<const float4*>(tt + (8 * i + sub_r) * TP + sub_c);
-                                    float* dst = (ps == 0) ? p.out0 + ((size_t)b * p.L + fr) * p.D + nt * 128 + c + sub_c
-                                                           : p.out1 + ((size_t)b * p.L + fr) * (2 * p.D) + (ps == 2 ? p.D : 0) + nt * 128 + c + sub_c;
-                                    *reinterpret_cast<float4*>(dst) = v;
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const int fr = t0 + r0 + 8 * r;
+                            if (fr >= p.L) continue;
+                            const float v0 = acc[h][4 * nb + 2 * r], v1 = acc[h][4 * nb + 2 * r + 1];
+                            const int c = 8 * nb + q2;                       // column inside the 128-column half
+                            if (EPI == EPI_GATE) {
+                                // tile columns: half 0 = F of channels 128*nt.., half 1 = G of the same channels
+                                if (h == 1) continue;
+                                const float* bt = bias_s + n0;
+                                const float gv0 = acc[1][4 * nb + 2 * r], gv1 = acc[1][4 * nb + 2 * r + 1];
+                                const float f0 = tanhf(v0 + bt[c]), f1 = tanhf(v1 + bt[c + 1]);
+                                const float g0 = sigmoid_tc(gv0 + bt[128 + c]), g1 = sigmoid_tc(gv1 + bt[128 + c + 1]);
+                                const int ch = nt * 128 + c;
+                                *reinterpret_cast<float2*>(p.out0 + ((size_t)b * p.L + fr) * p.D + ch) = make_float2(f0 * g0, f1 * g1);
+                                if (p.out1) {
+                                    float* fs = p.out1 + ((size_t)b * p.L + fr) * (2 * p.D) + ch;
+                                    *reinterpret_cast<float2*>(fs) = make_float2(f0, f1);
+                                    *reinterpret_cast<float2*>(fs + p.D) = make_float2(g0, g1);
+                                }
+                            } else if (EPI == EPI_GATE_BWD) {
+                                // dz (columns = dilation channels n): dF = dz*g*(1-f^2), dG = dz*f*g*(1-g), z = f*g
+                                const int n = n0 + 128 * h + c;
+                                const float* fgp = p.res + ((size_t)b * p.L + fr) * (2 * p.D) + n;
+                                const float2 f = __ldg(reinterpret_cast<const float2*>(fgp));
+                                const float2 gg = __ldg(reinterpret_cast<const float2*>(fgp + p.D));
+                                float* dfg = p.out0 + ((size_t)b * p.L + fr) * (2 * p.D) + n;
+                                *reinterpret_cast<float2*>(dfg) = make_float2(v0 * gg.x * (1.f - f.x * f.x), v1 * gg.y * (1.f - f.y * f.y));
+                                *reinterpret_cast<float2*>(dfg + p.D) = make_float2(v0 * f.x * gg.x * (1.f - gg.x), v1 * f.y * gg.y * (1.f - gg.y));
+                                *reinterpret_cast<float2*>(p.out2 + ((size_t)b * p.L + fr) * p.D + n) = make_float2(f.x * gg.x, f.y * gg.y);
+                            } else if (EPI == EPI_ADD) {
+                                // dh_in (columns = residual channels n) = acc + dh_out(t) for t >= id_start
+                                const int n = n0 + 128 * h + c;
+                                float2 x = make_float2(0.f, 0.f);
+                                if (p.res != nullptr && fr >= p.id_start) x = __ldg(reinterpret_cast<const float2*>(p.res + ((size_t)b * p.L + fr) * p.R + n));
+                                *reinterpret_cast<float2*>(p.out0 + ((size_t)b * p.L + fr) * p.R + n) = make_float2(v0 + x.x, v1 + x.y);
+                            } else {
+                                // global output column n: n < R residual, else skip channel n - R
+                                const int n = n0 + 128 * h + c;
+                                const float o0 = v0 + bias_s[n], o1 = v1 + bias_s[n + 1];
+                                if (n0 < p.R) {
+                                    float2 x = make_float2(0.f, 0.f);
+                                    if (fr >= p.in_start) x = __ldg(reinterpret_cast<const float2*>(p.res + ((size_t)b * p.L + fr) * p.R + n));
+                                    *reinterpret_cast<float2*>(p.out0 + ((size_t)b * p.L + fr) * p.R + n) = make_float2(o0 + x.x, o1 + x.y);
+                                } else if (fr >= p.skip_start) {
+                                    float* sk = p.out1 + ((size_t)b * Tsk + (fr - p.skip_start)) * p.S + (n - p.R);
+                                    float2 x = make_float2(0.f, 0.f);
+                                    if (!p.skip_init) x = *reinterpret_cast<const float2*>(sk);
+                                    *reinterpret_cast<float2*>(sk) = make_float2(o0 + x.x, o1 + x.y);
                                 }
                             }
                         }
-                    }
-                } else if (EPI == EPI_GATE_BWD) {
-                    // dz tile (columns = dilation channels nt*256 + c): dF = dz*g*(1-f^2), dG = dz*f*g*(1-g), z = f*g
-                    const int n0 = nt * BN;
-#pragma unroll 1
-                    for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                        float v[16];
-                        tmem_ld16(taddr + c, v);
-                        float4 fq[4], gq[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            fq[i] = gq[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (fr < p.L) {
-                                const float* fg = p.res + ((size_t)b * p.L + fr) * (2 * p.D) + n0 + c + sub_c;
-                                fq[i] = __ldg(reinterpret_cast<const float4*>(fg));
-                                gq[i] = __ldg(reinterpret_cast<const float4*>(fg + p.D));
-                            }
-                        }
-                        tmem_ld_wait();
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4)
-                            *reinterpret_cast<float4*>(tt + lane * TP + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            if (fr >= p.L) continue;
-                            const float4 dz = *reinterpret_cast<const float4*>(tt + (8 * i + sub_r) * TP + sub_c);
-                            const float4 f = fq[i], g = gq[i];
-                            float* dfg = p.out0 + ((size_t)b * p.L + fr) * (2 * p.D) + n0 + c + sub_c;
-                            *reinterpret_cast<float4*>(dfg) = make_float4(dz.x * g.x * (1.f - f.x * f.x), dz.y * g.y * (1.f - f.y * f.y),
-                                                                          dz.z * g.z * (1.f - f.z * f.z), dz.w * g.w * (1.f - f.w * f.w));
-                            *reinterpret_cast<float4*>(dfg + p.D) = make_float4(dz.x * f.x * g.x * (1.f - g.x), dz.y * f.y * g.y * (1.f - g.y),
-                                                                                dz.z * f.z * g.z * (1.f - g.z), dz.w * f.w * g.w * (1.f - g.w));
-                            *reinterpret_cast<float4*>(p.out2 + ((size_t)b * p.L + fr) * p.D + n0 + c + sub_c) =
-                                make_float4(f.x * g.x, f.y * g.y, f.z * g.z, f.w * g.w);
-                        }
-                    }
-                } else if (EPI == EPI_ADD) {
-                    // dh_in tile (columns = residual channels nt*256 + c) = acc + dh_out(t) for t >= id_start
-                    const int n0 = nt * BN;
-#pragma unroll 1
-                    for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                        float v[16];
-                        tmem_ld16(taddr + c, v);
-                        float4 x[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (fr < p.L && p.res != nullptr && fr >= p.id_start)
-                                x[i] = __ldg(reinterpret_cast<const float4*>(p.res + ((size_t)b * p.L + fr) * p.R + n0 + c + sub_c));
-                        }
-                        tmem_ld_wait();
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4)
-                            *reinterpret_cast<float4*>(tt + lane * TP + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            if (fr >= p.L) continue;
-                            float4 o = *reinterpret_cast<const float4*>(tt + (8 * i + sub_r) * TP + sub_c);
-                            o.x += x[i].x; o.y += x[i].y; o.z += x[i].z; o.w += x[i].w;
-                            *reinterpret_cast<float4*>(p.out0 + ((size_t)b * p.L + fr) * p.R + n0 + c + sub_c) = o;
-                        }
-                    }
-                } else {
-                    // tile columns: global output column n = nt*256 + c; n < R residual, else skip channel n - R; group g takes 128
-                    const int n0 = nt * BN;
-                    const bool is_res = n0 < p.R;
-                    const float* bt = bias_s + n0;
-                    const int Tsk = p.L - p.skip_start;
-#pragma unroll 1
-                    for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                        float v[16];
-                        tmem_ld16(taddr + c, v);
-                        // the values this lane will add in the coalesced domain (residual h_in(t) or the running skip)
-                        float4 x[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (fr < p.L) {
-                                if (is_res) {
-                                    if (fr >= p.in_start)
-                                        x[i] = __ldg(reinterpret_cast<const float4*>(p.res + ((size_t)b * p.L + fr) * p.R + n0 + c + sub_c));
-                                } else if (!p.skip_init && fr >= p.skip_start) {
-                                    x[i] = *reinterpret_cast<const float4*>(p.out1 + ((size_t)b * Tsk + (fr - p.skip_start)) * p.S + (n0 - p.R) + c + sub_c);
-                                }
-                            }
-                        }
-                        tmem_ld_wait();
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4)
-                            *reinterpret_cast<float4*>(tt + lane * TP + i) =
-                                make_float4(v[i] + bt[c + i], v[i + 1] + bt[c + i + 1], v[i + 2] + bt[c + i + 2], v[i + 3] + bt[c + i + 3]);
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int fr = tbase + 8 * i + sub_r;
-                            if (fr >= p.L) continue;
-                            float4 o = *reinterpret_cast<const float4*>(tt + (8 * i + sub_r) * TP + sub_c);
-                            o.x += x[i].x; o.y += x[i].y; o.z += x[i].z; o.w += x[i].w;
-                            if (is_res)
-                                *reinterpret_cast<float4*>(p.out0 + ((size_t)b * p.L + fr) * p.R + n0 + c + sub_c) = o;
-                            else if (fr >= p.skip_start)
-                                *reinterpret_cast<float4*>(p.out1 + ((size_t)b * Tsk + (fr - p.skip_start)) * p.S + (n0 - p.R) + c + sub_c) = o;
-                        }
-                    }
-                }
-                tc_fence_before();
-                mbar_arrive(acc_empty + ab);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_();                              // no peer may still signal this CTA's barriers after it is gone
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ---------------------------------------------------------------------------------------------- weight packing
@@ -654,7 +407,7 @@ static int make_act_map(CUtensorMap* m, const float* base, int B, int L, int C, 
     WN_REQUIRE(r == CUDA_SUCCESS, WN_E_UNSUPP, "cuTensorMapEncodeTiled(activations) failed with %d", (int)r);
     return 0;
 }
-// weights (rows, K) fp32 K-major: dims {K, rows}, box {32, 256}
+// weights (rows, K) fp32 K-major: dims {K, rows}, box {BK, 128}
 // `col0`: first K column (element offset into every row); bf16 = true: the array holds bf16 pairs (32-byte slab rows)
 static int make_w_map(CUtensorMap* m, const void* base, int rows, int K, int col0 = 0, bool bf16 = false) {
     EncodeTiledFn fn = encode_fn();
@@ -662,7 +415,7 @@ static int make_w_map(CUtensorMap* m, const void* base, int rows, int K, int col
     const int es = bf16 ? 2 : 4;
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)K * es};
-    cuuint32_t box[2] = {BK, BN / CS};          // one CTA's share of a slab; the multicast assembles the rest
+    cuuint32_t box[2] = {BK, BN / 2};           // half a tile: 128 rows
     cuuint32_t estr[2] = {1, 1};
     const int row_bytes = BK * es;
     CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
@@ -676,7 +429,7 @@ static int make_w_map(CUtensorMap* m, const void* base, int rows, int K, int col
 
 static size_t tc_smem_bytes(int n_total, int prec) {
     const size_t ring = prec == PREC_BF16X2 ? (size_t)STAGES_BF * STAGE_BYTES_BF : (size_t)STAGES * STAGE_BYTES;
-    return 1024 + ring + 512 + sizeof(float) * ((n_total + 3) & ~3) + sizeof(float) * 8 * 32 * TP;
+    return 1024 + ring + 512 + sizeof(float) * ((n_total + 3) & ~3);
 }
 
 template <int EPI, int PREC>
@@ -687,21 +440,12 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtens
     const size_t smem = tc_smem_bytes(p.n_total, PREC);
     WN_CUDA(cudaFuncSetAttribute(frames_gemm_tc<EPI, PREC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int items = p.B * ((p.L - p.t_begin + BM - 1) / BM);
-    int grid = ((items + CS - 1) / CS) * CS;
-    const int max_grid = (sms / CS) * CS;
-    if (grid > max_grid) grid = max_grid;
+    const int grid = items < sms ? items : sms;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(NTHREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     WN_CUDA(cudaLaunchKernelEx(&cfg, frames_gemm_tc<EPI, PREC>, mA, mA2, mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;
@@ -718,16 +462,15 @@ static int launch_tc_prec(int prec, const CUtensorMap& mA, const CUtensorMap& mA
 // ============================================================================================== weight gradients
 // dW[n][c] = sum over sequences b and frames t of g[b][t][n] * x[b][t][c]  (what wn_wgrad computes on the FMA pipe,
 // wgrad.cu) on the tensor cores.  The contraction runs over frames, the SLOW axis of both row-major operands, so the
-// tiles arrive "MN-major"; instead of MN-major descriptors the splitter -- which has to rewrite every element as a
-// bf16 (hi, lo) pair anyway -- writes the operand tiles TRANSPOSED, i.e. in the same K-major, 32-byte-swizzled form the
-// block kernels use.  One CTA = one 128-row tile of n (UMMA M) x all C = 256 columns (UMMA N) x one range of K slabs
-// (16 frames each); its fp32 partial goes to the split-frames workspace and wgrad_tc_reduce_kernel adds the partials.
-//   warp 0      TMA producer: raw fp32 tiles g[16 frames][128 ch] and x[16 frames][256 ch] (no swizzle), 4-stage ring
-//   warp 1      TMEM (256 columns), tcgen05.mma kind::f16: hi*hi + lo*hi + hi*lo per slab
-//   warps 2-9   splitter: thread = (channel, 8 frames): 8 conflict-free LDS.32 down a column, bf16 hi/lo split,
-//               one 16-byte store per operand tile row chunk
-//   warps 2-9   after the last slab: TMEM -> registers -> workspace
-constexpr int WG_THREADS = 320;
+// tiles arrive "MN-major"; the consumers -- which have to rewrite every element as a bf16 (hi, lo) pair anyway -- write
+// the operand tiles TRANSPOSED, i.e. in the same K-major, 32-byte-swizzled form the block kernels use.  One CTA = one
+// 128-row tile of n (M) x all C = 256 columns (N) x one range of K slabs (16 frames each); its fp32 partial goes to the
+// split-frames workspace and wgrad_tc_reduce_kernel adds the partials.
+//   warp 8      TMA producer: raw fp32 tiles g[16 frames][128 ch] and x[16 frames][256 ch] (no swizzle), 4-stage ring
+//   warps 0-7   split (thread = (channel, 8 frames): 8 conflict-free LDS.32 down a column, bf16 hi/lo split, one 16-byte
+//               store per operand tile row chunk), then warpgroup g issues wgmma for rows 64g..64g+63: hi*hi + lo*hi + hi*lo;
+//               after the last slab: registers -> workspace
+constexpr int WG_THREADS = 288;
 constexpr int WG_SPLIT_THREADS = 256;
 constexpr int WG_STAGES = 4;
 constexpr int WG_RAW_A = BK * BM * 4;            // 8 KB   [16 frames][128 ch] fp32
@@ -746,10 +489,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned long long* bars = reinterpret_cast<unsigned long long*>(base + WG_STAGES * WG_STAGE_BYTES);
     unsigned long long* full = bars;                       // [WG_STAGES] TMA landed
-    unsigned long long* split = bars + WG_STAGES;          // [WG_STAGES] operand tiles written
-    unsigned long long* empty = bars + 2 * WG_STAGES;      // [WG_STAGES] MMAs of the stage retired
-    unsigned long long* acc_full = bars + 3 * WG_STAGES;   // [1]
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(bars + 3 * WG_STAGES + 1);
+    unsigned long long* empty = bars + WG_STAGES;          // [WG_STAGES] every consumer thread is done with the stage
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m_tile = blockIdx.x % p.m_tiles, sp = blockIdx.x / p.m_tiles;
@@ -757,21 +497,16 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
     const int s_end = (s_beg + p.slabs_per_split < p.total_slabs) ? s_beg + p.slabs_per_split : p.total_slabs;
     const int n_slabs = s_end > s_beg ? s_end - s_beg : 0;
 
-    if (warp == 0 && lane == 0) {
-        for (int i = 0; i < WG_STAGES; ++i) { mbar_init(full + i, 1); mbar_init(split + i, WG_SPLIT_THREADS); mbar_init(empty + i, 1); }
-        mbar_init(acc_full, 1);
+    if (tid == 0) {
+        for (int i = 0; i < WG_STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, WG_SPLIT_THREADS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapG) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&mapX) : "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (warp == 8) {
+        if (lane == 0) {
             for (int i = 0; i < n_slabs; ++i) {
                 const int st = i % WG_STAGES;
                 const unsigned ph = (i / WG_STAGES) & 1;
@@ -783,28 +518,10 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
                 tma_load_3d(sm + WG_RAW_A, &mapX, 0, t0, b, full + st);
             }
         }
-    } else if (warp == 1) {
-        constexpr unsigned idesc = make_idesc(true);
-        for (int i = 0; i < n_slabs; ++i) {
-            const int st = i % WG_STAGES;
-            const unsigned ph = (i / WG_STAGES) & 1;
-            mbar_wait(split + st, ph);
-            tc_fence_after();
-            if (elect_one()) {
-                const unsigned sa = s32(base + st * WG_STAGE_BYTES) + WG_RAW_A + WG_RAW_B;
-                const unsigned long long a_hi = smem_desc<32>(sa), a_lo = smem_desc<32>(sa + ABF_BYTES);
-                const unsigned long long b_hi = smem_desc<32>(sa + 2 * ABF_BYTES), b_lo = smem_desc<32>(sa + 2 * ABF_BYTES + WBF_BYTES);
-                umma_f16(tmem_base, a_hi, b_hi, idesc, i != 0);
-                umma_f16(tmem_base, a_lo, b_hi, idesc, 1);
-                umma_f16(tmem_base, a_hi, b_lo, idesc, 1);
-                umma_commit(empty + st);
-                if (i == n_slabs - 1) umma_commit(acc_full);
-            }
-            __syncwarp();
-        }
     } else {
-        // ---------------------------------------------------------------- splitter (256 threads), then epilogue
-        const int stid = tid - 64;
+        // ---------------------------------------------------------------- split (256 threads), MMA, then epilogue
+        const int g = warp >> 2;
+        float acc[2][64];
         for (int i = 0; i < n_slabs; ++i) {
             const int st = i % WG_STAGES;
             const unsigned ph = (i / WG_STAGES) & 1;
@@ -816,9 +533,9 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
 #pragma unroll
             for (int j = 0; j < 3; ++j) {
                 // groups 0..255: A (128 channels x 2 halves of 8 frames); groups 256..767: B (256 channels x 2 halves)
-                const int g = stid + WG_SPLIT_THREADS * j;
-                const bool isA = g < 2 * BM;
-                const int gg = isA ? g : g - 2 * BM;
+                const int gr = tid + WG_SPLIT_THREADS * j;
+                const bool isA = gr < 2 * BM;
+                const int gg = isA ? gr : gr - 2 * BM;
                 const int nch = isA ? BM : BN;
                 const int ch = gg % nch, half = gg / nch;
                 const float* src = (isA ? rawA : rawB) + (half * 8) * nch + ch;
@@ -827,13 +544,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
                 for (int k = 0; k < 8; ++k) x[k] = src[k * nch];
                 unsigned hv[4], lv[4];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const __nv_bfloat162 h = __floats2bfloat162_rn(x[2 * k], x[2 * k + 1]);
-                    const float2 hf = __bfloat1622float2(h);
-                    const __nv_bfloat162 l = __floats2bfloat162_rn(x[2 * k] - hf.x, x[2 * k + 1] - hf.y);
-                    hv[k] = *reinterpret_cast<const unsigned*>(&h);
-                    lv[k] = *reinterpret_cast<const unsigned*>(&l);
-                }
+                for (int k = 0; k < 4; ++k) split2(x[2 * k], x[2 * k + 1], hv[k], lv[k]);
                 // K-major tile, 32-byte rows (16 bf16), 32B swizzle: 16-byte chunk `half` of row `ch` sits at half ^ ((ch>>2)&1)
                 const unsigned off = (unsigned)ch * 32u + ((unsigned)(half ^ ((ch >> 2) & 1)) << 4);
                 unsigned char* hi_t = tiles + (isA ? 0 : 2 * ABF_BYTES);
@@ -841,33 +552,37 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant_
                 *reinterpret_cast<uint4*>(hi_t + off) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
                 *reinterpret_cast<uint4*>(lo_t + off) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_arrive(split + st);
-        }
-        // epilogue: warp w reads TMEM lanes 32*(w%4)..+31 (= rows of the n tile); warps 2-5 take columns [0,128), 6-9 [128,256)
-        const int q = warp & 3, grp = (warp - 2) >> 2;
-        const int n = m_tile * BM + q * 32 + lane;
-        float* out = p.work + ((size_t)sp * p.N + n) * p.C;
-        if (n_slabs > 0) {
-            mbar_wait(acc_full, 0);
-            tc_fence_after();
-            const unsigned taddr = tmem_base + ((unsigned)(q * 32) << 16);
-#pragma unroll 1
-            for (int c = grp * 128; c < grp * 128 + 128; c += 16) {
-                float v[16];
-                tmem_ld16(taddr + c, v);
-                tmem_ld_wait();
+            fence_async_smem();
+            wg_bar(1, WG_SPLIT_THREADS);                  // both warpgroups read the whole B tile
+            const unsigned sa = s32(tiles);
+            const unsigned a_hi = sa + g * 64 * 32, a_lo = a_hi + ABF_BYTES;
+            wgmma_fence();
 #pragma unroll
-                for (int i = 0; i < 16; i += 4)
-                    *reinterpret_cast<float4*>(out + c + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+            for (int h = 0; h < 2; ++h) {
+                const unsigned b_hi = sa + 2 * ABF_BYTES + h * (WBF_BYTES / 2), b_lo = b_hi + WBF_BYTES;
+                wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(b_hi), i != 0);
+                wgmma_bf16_t00(acc[h], desc32(a_lo), desc32(b_hi), 1u);
+                wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(b_lo), 1u);
             }
-        } else {
-            for (int c = grp * 128; c < grp * 128 + 128; c += 4) *reinterpret_cast<float4*>(out + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+            wgmma_commit();
+            wgmma_wait0();
+            wgmma_keep(acc[0]);
+            wgmma_keep(acc[1]);
+            mbar_arrive(empty + st);
         }
+        // epilogue: fragment rows of the n tile, all 256 columns
+        const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2), q2 = 2 * (lane & 3);
+        float* out = p.work + ((size_t)sp * p.N + m_tile * BM) * p.C;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float2 v = n_slabs > 0 ? make_float2(acc[h][4 * nb + 2 * r], acc[h][4 * nb + 2 * r + 1]) : make_float2(0.f, 0.f);
+                    *reinterpret_cast<float2*>(out + (size_t)(r0 + 8 * r) * p.C + 128 * h + 8 * nb + q2) = v;
+                }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 256);
 }
 
 __global__ void wgrad_tc_reduce_kernel(const float* __restrict__ work, float* __restrict__ dw, int N, int C, int splits,

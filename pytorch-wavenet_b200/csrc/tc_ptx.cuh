@@ -1,6 +1,5 @@
-// tc_ptx.cuh -- inline-PTX wrappers for the cta_group::2 tensor-core kernels (tc_block.cu, tc_bwd2.cu): mbarrier, TMA with
-// the barrier in the pair's leader CTA, tcgen05 alloc / mma / commit / ld, SWIZZLE_NONE shared-memory descriptors.
-// Every form used here was verified on a B200 by tools/umma_probe.cu (profiles/umma_probe_r2_a.txt).
+// tc_ptx.cuh -- inline-PTX wrappers for the Hopper (sm_90a) tensor-core kernels (tc_gemm.cu, tc_block.cu, tc_bwd2.cu):
+// mbarrier, TMA, warpgroup MMA (wgmma) with shared-memory descriptors, gate activations and bf16 pair splitting.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -12,15 +11,6 @@ namespace px {
 constexpr unsigned SPIN_LIMIT = 1u << 28;     // a barrier that never completes traps instead of hanging the GPU
 
 __device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned cluster_rank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ unsigned mapa(unsigned addr, unsigned rank) {
-    unsigned r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
-}
 __device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned n) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(b)), "r"(n) : "memory");
 }
@@ -29,10 +19,6 @@ __device__ __forceinline__ void mbar_expect_tx(unsigned long long* b, unsigned b
 }
 __device__ __forceinline__ void mbar_arrive(unsigned long long* b) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(b)) : "memory");
-}
-// arrive (release at cluster scope) on a barrier given by its shared::cluster address (any CTA of the cluster)
-__device__ __forceinline__ void mbar_arrive_cluster(unsigned cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ bool mbar_try(unsigned long long* b, unsigned parity) {
     unsigned done;
@@ -44,81 +30,66 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity
     unsigned spins = 0;
     while (!mbar_try(b, parity)) if (++spins > SPIN_LIMIT) asm volatile("trap;");
 }
-// the same with acquire at cluster scope: the arrivals came from the peer CTA (mbar_arrive_cluster)
-__device__ __forceinline__ void mbar_wait_cluster(unsigned long long* b, unsigned parity) {
-    unsigned done, spins = 0;
-    do {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(done) : "r"(s32(b)), "r"(parity) : "memory");
-        if (!done && ++spins > SPIN_LIMIT) asm volatile("trap;");
-    } while (!done);
+// ---- TMA loads into this CTA's shared memory, completing on this CTA's barrier
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(s32(bar)) : "memory");
 }
-__device__ __forceinline__ bool elect_one() {
-    unsigned pred;
-    asm volatile("{ .reg .pred p; elect.sync _|p, 0xffffffff; selp.u32 %0, 1, 0, p; }" : "=r"(pred));
-    return pred != 0;
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(s32(bar)) : "memory");
 }
-
-// ---- TMA loads executed by both CTAs of a pair; `bar` is the shared::cluster address of the LEADER's barrier
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, unsigned bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
+__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(s32(bar)) : "memory");
 }
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, unsigned bar) {
-    asm volatile("cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-                 ::"r"(s32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-
-// ---- tensor memory, cta_group::2 (the same warp of BOTH CTAs executes alloc / dealloc)
-__device__ __forceinline__ void tmem2_alloc(unsigned* slot_in_smem, unsigned cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(slot_in_smem)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem2_dealloc(unsigned addr, unsigned cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier of one warpgroup (ids 1.. ; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (bf16 operands, fp32 accumulate), M = 256 over the CTA pair; leader thread only
-__device__ __forceinline__ void umma2_f16(unsigned d_tmem, unsigned long long a_desc, unsigned long long b_desc, unsigned idesc,
-                                          unsigned accumulate) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p; }"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on `bar` (same shared-memory offset) in BOTH CTAs once all MMAs issued so far by this thread have retired
-__device__ __forceinline__ void umma2_commit(unsigned long long* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(s32(bar)), "h"((unsigned short)3) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, float (&v)[16]) {
-    unsigned r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                   "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
+// ---- wgmma (sm_90a): a warpgroup (4 consecutive warps) computes D[64 x 128] (+)= A[64 x K] * B[K x 128] from shared memory,
+// fp32 accumulators in registers.  Fragment of thread i of the warpgroup (warp w = i / 32, lane l): d[4n + 2r + c] is row
+// 16w + l/4 + 8r, column 8n + 2(l%4) + c.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_keep(float (&d)[N]) {       // the accumulators stay in place across the async MMAs
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// bf16 x bf16 -> fp32, K = 16; t<A><B>: 0 = K-major operand, 1 = MN-major (transposed) operand.  acc = 0 overwrites D.
+__device__ __forceinline__ void wgmma_bf16_t00(float (&d)[64], unsigned long long a, unsigned long long b, unsigned acc) {
+    asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0; }"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_bf16_t11(float (&d)[64], unsigned long long a, unsigned long long b, unsigned acc) {
+    asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 1, 1; }"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+// tf32 x tf32 -> fp32, K = 8, both operands K-major
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], unsigned long long a, unsigned long long b, unsigned acc) {
+    asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1; }"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
 
-// SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1).  K-major operand on the chunked
-// tile image [k-chunk of 8 elements][row][16 bytes]: lbo = bytes between the two 16-byte K chunks of a k-step (= rows * 16),
-// sbo = bytes between 8-row groups (= 128).  MN-major operand on the same image: lbo = bytes between 8-frame K groups (128),
-// sbo = bytes between 8-channel MN groups (= frames * 16).
-__device__ __forceinline__ unsigned long long smem_desc(unsigned saddr, unsigned lbo, unsigned sbo) {
+// shared-memory matrix descriptor (wgmma): start address, leading / stride byte offsets, layout (0 = no swizzle, 1 = 128B,
+// 2 = 64B, 3 = 32B).  No swizzle, K-major: lbo = bytes between the 16-byte K chunks of a k-step, sbo = bytes between 8-row
+// groups; no swizzle, MN-major: lbo = bytes between 8-deep K groups, sbo = bytes between 8-wide MN groups.  Swizzled K-major:
+// lbo unused, sbo = bytes between 8-row atoms.
+__device__ __forceinline__ unsigned long long wg_desc(unsigned saddr, unsigned lbo, unsigned sbo, unsigned layout = 0) {
     unsigned long long d = 0;
     d |= (unsigned long long)((saddr >> 4) & 0x3fff);
     d |= (unsigned long long)((lbo >> 4) & 0x3fff) << 16;
     d |= (unsigned long long)((sbo >> 4) & 0x3fff) << 32;
-    d |= (unsigned long long)1 << 46;
+    d |= (unsigned long long)layout << 62;
     return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): fp32 accumulate, bf16 x bf16, M x N, majors (0 = K, 1 = MN)
-__host__ __device__ constexpr unsigned make_idesc_bf16(int M, int N, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)a_mn << 15) | ((unsigned)b_mn << 16) | ((unsigned)(N >> 3) << 17) |
-           ((unsigned)(M >> 4) << 24);
 }
 
 // ---- activations for the gate: ex2 / rcp approximations (relative error ~2e-7; the parity bar is 1e-4 on the logits)

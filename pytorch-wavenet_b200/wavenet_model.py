@@ -1,7 +1,7 @@
 """WaveNetModel with the reference's constructor, attributes, state_dict and methods
-(reference wavenet_model.py), running its two hot paths on hand-written sm_100a CUDA kernels:
+(reference wavenet_model.py), running its two hot paths on hand-written sm_90a CUDA kernels:
 
-* ``forward`` / ``wavenet``   -> start gather/GEMM, the residual blocks (256-channel nets: two tcgen05 launches per
+* ``forward`` / ``wavenet``   -> start gather/GEMM, the residual blocks (256-channel nets: two wgmma launches per
                                  block with bf16-pair operands, wn_tc_block_fwd; any other shape: ONE fused fp32 kernel
                                  per block, wn_block_fwd), fused head (wn_start_fwd_*, wn_head_fwd)
 * ``loss.backward()``         -> wn_head_bwd_data, per block wn_tc_block_bwd_data_prec / wn_block_bwd_data for the data
@@ -488,7 +488,7 @@ class _Runtime:
         return logits
 
     def _backward_tb(self, saved, dlogits):
-        """Backward on the chunked pair layout: head (SIMT kernels on the frames layout), then per block two tcgen05 data-
+        """Backward on the chunked pair layout: head (SIMT kernels on the frames layout), then per block two wgmma data-
         gradient launches (wn_tb_block_bwd_data) and one weight-gradient launch (wn_tb_wgrad).  Same frame-range logic as
         stack_backward."""
         m, lib = self.model, native.lib()

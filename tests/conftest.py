@@ -2,7 +2,6 @@
 import os
 import sys
 
-import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -14,7 +13,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -29,7 +28,9 @@ def pytest_collection_modifyitems(config, items):
 
 
 def load_golden(name):
-    return np.load(os.path.join(GOLDEN, name), allow_pickle=False)
+    """The arrays of tests/golden/<name> (fixtures over 900 KB are stored in shards, see golden_store.py)."""
+    import golden_store
+    return golden_store.load(os.path.join(GOLDEN, name))
 
 
 @pytest.fixture(scope="session")

@@ -26,6 +26,8 @@ import torch.nn.functional as F
 
 REF = "/root/reference"
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(HERE))
+import golden_store  # noqa: E402  (fixtures over 900 KB are written as shards)
 
 
 def import_reference():
@@ -170,7 +172,7 @@ def main():
         arrs.update({"kw_" + k: v for k, v in kw.items()})
         if name != "cfg1":
             arrs.update({"w:" + k: v for k, v in w.items()})  # small nets: ship the weights too
-        np.savez_compressed(os.path.join(HERE, f"net_{name}.npz"), **arrs)
+        golden_store.save(os.path.join(HERE, f"net_{name}.npz"), arrs, compressed=True)
         out[name] = (fwd.shape, float(fwd.abs().max()))
 
     # ---------------- cfg 2 shape (10x5, 256 ch): seeded init is reproduced by ctor order; ship outputs only
@@ -201,9 +203,10 @@ def main():
     m = torch.load(snap, map_location="cpu", weights_only=False)                      # shim 5
     m.cpu()
     sd = state_arrays(m)
-    np.savez(os.path.join(HERE, "snapshot_chaconne_state.npz"), layers=m.layers, blocks=m.blocks,
-             kernel_size=m.kernel_size, classes=m.classes, output_length=m.output_length,
-             receptive_field=m.receptive_field, **{"w:" + k: v for k, v in sd.items()})
+    golden_store.save(os.path.join(HERE, "snapshot_chaconne_state.npz"),
+                      dict(layers=m.layers, blocks=m.blocks, kernel_size=m.kernel_size, classes=m.classes,
+                           output_length=m.output_length, receptive_field=m.receptive_field,
+                           **{"w:" + k: v for k, v in sd.items()}))
     data = np.load(os.path.join(REF, "train_samples", "bach_chaconne", "dataset.npz"))["arr_0"]
     rf = m.receptive_field
     off = 960000

@@ -128,7 +128,7 @@ def test_cfg3_full_size_vs_oracle():
     rt = m._runtime()
     with torch.no_grad():
         y1 = m.forward_indices(idx[3:4].cuda())
-        assert rt.last_block_mode == "tb"                      # the fused tcgen05 block kernel is the default here
+        assert rt.last_block_mode == "tb"                      # the fused wgmma block kernel is the default here
         err = rel_err(y1.cpu().numpy(), want)
         assert err < TOL, f"cfg3 full size vs oracle: {err:.3e}"
         y8 = m.forward_indices(idx.cuda()).view(8, -1, 256)

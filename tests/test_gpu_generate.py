@@ -294,7 +294,7 @@ def test_batched_cluster_kernel_cfg2(golden):
     # the default for several streams of this net is this kernel
     d, ld = m.generate_fast_batch(60, first, temperature=1.0, uniforms=uni, return_logits=True)
     assert np.array_equal(d, idx6) and np.array_equal(ld, lg6)
-    # 64 streams (8 clusters: more than the 7 sixteen-CTA clusters a B200 holds, so the 8-CTA-cluster variant runs) equal
+    # 64 streams (8 clusters: where fewer sixteen-CTA clusters are co-resident, the 8-CTA-cluster variant runs) equal
     # the same streams run 11 at a time
     first64 = np.concatenate([first] * 6)[:64]
     uni64 = np.concatenate([uni] * 6)[:64]

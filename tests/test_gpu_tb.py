@@ -1,4 +1,4 @@
-"""The fused tensor-core block (csrc/tc_block.cu: tcgen05 cta_group::2, chunked bf16-pair activations, one launch per
+"""The fused tensor-core block (csrc/tc_block.cu: wgmma, chunked bf16-pair activations, one launch per
 residual block) against the CPU oracle, the golden outputs of the unmodified reference and the exact-fp32 SIMT blocks."""
 import ctypes
 
@@ -124,8 +124,8 @@ def test_tb_mode_requires_supported_shape(golden):
     (1, 1100, 6, 1, False, 37),        # no biases; most frames lie outside the receptive cone of the outputs
 ])
 def test_fused_backward_matches_oracle_and_simt(B, L, layers, blocks, bias, out_len):
-    """Training step through the chunked-pair kernels (forward with saved activations, tcgen05 data gradients, MN-major
-    tcgen05 weight gradients) vs autograd over the CPU oracle and vs the exact-fp32 SIMT kernels."""
+    """Training step through the chunked-pair kernels (forward with saved activations, wgmma data gradients, MN-major
+    wgmma weight gradients) vs autograd over the CPU oracle and vs the exact-fp32 SIMT kernels."""
     import torch.nn.functional as F
     import wavenet_model as wmod
     kw = dict(layers=layers, blocks=blocks, dilation_channels=256, residual_channels=256, skip_channels=256,

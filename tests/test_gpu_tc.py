@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05) residual blocks vs the exact-fp32 SIMT blocks, the golden reference outputs and the CPU oracle.
+"""Tensor-core (wgmma) residual blocks vs the exact-fp32 SIMT blocks, the golden reference outputs and the CPU oracle.
 Both operand splits -- bf16 pairs (default) and 3xTF32 -- must hold the same 1e-4 parity bar (expected around 1e-6)."""
 import numpy as np
 import pytest

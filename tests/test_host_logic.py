@@ -101,23 +101,38 @@ def test_snapshot_state_loads(golden):
     assert m.parameter_count() == 1834592 and m.receptive_field == 3070
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/snapshots/chaconne_model_2017-12-28_16-44-12"),
-                    reason="reference checkout not present (build container only)")
-def test_reference_pickle_unpickles_into_this_class():
-    """The reference snapshots are whole-object pickles of wavenet_model.WaveNetModel; with this package on the
-    path they restore into THIS class (wavenet_model.py:330-346 load_latest_model_from / load_to_cpu)."""
-    m = wmod.load_to_cpu("/root/reference/snapshots/chaconne_model_2017-12-28_16-44-12")
-    assert type(m) is wmod.WaveNetModel and m.receptive_field == 3070 and m.dtype == torch.FloatTensor
+def test_reference_pickle_unpickles_into_this_class(golden):
+    """The reference's snapshots are whole-object pickles of wavenet_model.WaveNetModel (torch.save(self.model, ...),
+    reference wavenet_training.py:88); with this package on the path they restore into THIS class
+    (wavenet_model.py:330-346 load_latest_model_from / load_to_cpu).  tests/golden/tiny_snapshot.pt is such a pickle of a
+    small reference net, written by tests/golden/make_tiny_snapshot.py."""
+    from conftest import GOLDEN
+    m = wmod.load_to_cpu(os.path.join(GOLDEN, "tiny_snapshot.pt"))
+    io = golden("tiny_snapshot_io.npz")
+    assert type(m) is wmod.WaveNetModel and m.receptive_field == int(io["receptive_field"]) and m.dtype == torch.FloatTensor
     assert type(m.dilated_queues[0]).__module__ == "wavenet_modules"
     assert m._runtime() is m._runtime()
+    # the restored parameters are the reference's: the oracle forward on them reproduces the reference's own output
+    kw = dict(layers=m.layers, blocks=m.blocks, dilation_channels=m.dilation_channels, residual_channels=m.residual_channels,
+              skip_channels=m.skip_channels, end_channels=m.end_conv_1.out_channels, classes=m.classes,
+              output_length=m.output_length, kernel_size=m.kernel_size, bias=m.start_conv.bias is not None)
+    params = {k: v.detach() for k, v in m.state_dict().items()}
+    with torch.no_grad():
+        y = O.forward(params, O.NetSpec(**kw), O.one_hot(torch.from_numpy(io["idx"]), m.classes)).numpy()
+    assert np.abs(y - io["fwd"]).max() <= 1e-6 * np.abs(io["fwd"]).max()
 
 
 def test_no_cpu_fallback():
     m = wmod.WaveNetModel(layers=2, blocks=1, dilation_channels=4, residual_channels=4, skip_channels=4, end_channels=4)
     with torch.no_grad(), pytest.raises(RuntimeError, match="CUDA"):
         m(torch.zeros(1, 256, 16))
-    with pytest.raises(RuntimeError, match="CUDA"):
+    if torch.cuda.is_available():
+        # a CPU-resident model samples through its CUDA copy (the reference's scripts sample from a CPU copy), never on the CPU
         m.generate_fast(4)
+        assert m.__dict__["_shadow"][1].start_conv.weight.is_cuda
+    else:
+        with pytest.raises(RuntimeError, match="CUDA"):
+            m.generate_fast(4)
     with pytest.raises(RuntimeError, match="CUDA"):
         m.generate(4)
 

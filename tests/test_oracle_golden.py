@@ -8,6 +8,16 @@ from oracle import wavenet_oracle as O
 from helpers import spec_from_golden, params_from_golden, weight_checksum, rel_err
 
 NETS_WITH_WEIGHTS = ["odd_bias", "k3", "deep"]
+GOLDEN_THREADS = 8      # torch CPU threads of the recorded reference run: CPU kernels split their sums by thread count
+
+
+@pytest.fixture(autouse=True)
+def _golden_thread_count():
+    """Bit-for-bit comparisons need the reference run's summation order, whatever the host's core count."""
+    saved = torch.get_num_threads()
+    torch.set_num_threads(GOLDEN_THREADS)
+    yield
+    torch.set_num_threads(saved)
 
 
 # ---------------------------------------------------------------- reference tests/test_modules.py:8-29

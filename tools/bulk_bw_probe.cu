@@ -2,7 +2,7 @@
 // the way the batched sampler does?  112 CTAs; CTA b walks the regions of "rank" b % 16 (7 CTAs share every region, as the 7
 // clusters of the sampler do) of a buffer of `footprint` MB, in images of `img` KB split into `chunk` KB copies, with `depth`
 // images in flight.  Prints bytes per cycle per SM.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bulk_bw_probe tools/bulk_bw_probe.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bulk_bw_probe tools/bulk_bw_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

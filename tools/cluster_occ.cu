@@ -1,6 +1,6 @@
 // cluster_occ.cu -- how many thread-block clusters of a given size are co-resident on this GPU when every CTA needs a
 // whole SM's shared memory (the sampler kernels' situation)?
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o cluster_occ tools/cluster_occ.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o cluster_occ tools/cluster_occ.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void dummy(int* p) { extern __shared__ int s[]; if (p) p[0] = s[0]; }

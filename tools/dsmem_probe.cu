@@ -11,7 +11,7 @@
 //      st.async.v4 per destination: a whole 512-byte block per instruction
 // Each round every CTA publishes V=16 values (x8 in E) to all 16 CTAs and needs all 256 values of the round before it may
 // publish the next one.  Prints cycles per round.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dsmem_probe tools/dsmem_probe.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dsmem_probe tools/dsmem_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

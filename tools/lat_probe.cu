@@ -1,9 +1,9 @@
-// lat_probe.cu -- micro-measurements behind the sampler's exchange design (run on the B200 box):
+// lat_probe.cu -- micro-measurements behind the sampler's exchange design (run on an H100):
 //   1. flag ping-pong between two CTAs (store -> visible -> load) : one-way exchange latency through L2
 //   2. all-to-all round among G CTAs: each CTA publishes V {value,tag} pairs, every CTA collects all G*V pairs
 //      variants: who polls (all threads / one warp), vector width, nanosleep backoff
 //   3. atomic-counter grid barrier round
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o lat_probe tools/lat_probe.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lat_probe tools/lat_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
