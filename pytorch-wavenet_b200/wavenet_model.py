@@ -629,6 +629,18 @@ class _Runtime:
         return grads
 
     # ------------------------------------------------------------------ training-path backward
+    def ffma_bwd_weights(self, i):
+        """Weight rows of layer i for wn_block_bwd_data: d_wrs_rows [(R+S)][wn_n2p(D)] (residual_conv.weight rows, then
+        skip_conv.weight rows) and d_wfg_bwd [k*2D][wn_n2p(R)] (row j*2D + n: [filter; gate].weight[n, :, j]), zero padded."""
+        lib, P = native.lib(), self._params()
+        m = self.model
+        R, D, k = m.residual_channels, m.dilation_channels, m.kernel_size
+        pad_cols = lambda w2d, n: torch.nn.functional.pad(w2d, (0, n - w2d.shape[1])).contiguous()
+        (wf, _), (wg, _), (wr, _), (wsk, _) = P["filt"][i], P["gate"][i], P["res"][i], P["skip"][i]
+        wrs_rows = pad_cols(torch.cat([wr.detach()[:, :, 0], wsk.detach()[:, :, 0]], 0), lib.wn_n2p(D))
+        wfg_bwd = pad_cols(torch.cat([wf.detach(), wg.detach()], 0).permute(2, 0, 1).reshape(k * 2 * D, R), lib.wn_n2p(R))
+        return wrs_rows, wfg_bwd
+
     def stack_backward(self, saved, dlogits):
         """Gradients of all parameters given d(loss)/d(logits) (B*out_len, classes).  Data gradients run on the
         wn_*_bwd_data kernels, the weight gradients on wn_tc_wgrad / wn_wgrad over the buffers those kernels produce
@@ -742,9 +754,7 @@ class _Runtime:
                     wdz, wdh = W["tc_bwd_layers"][i]
                     native.check(lib.wn_tc_block_bwd_data(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), stream), f"tc block bwd {i}")
             else:
-                wrs_rows = pad_cols(torch.cat([wr.detach()[:, :, 0], wsk.detach()[:, :, 0]], 0), lib.wn_n2p(D))
-                wfg_bwd = pad_cols(torch.cat([wf.detach(), wg.detach()], 0).permute(2, 0, 1).reshape(k * 2 * D, R),
-                                   lib.wn_n2p(R))
+                wrs_rows, wfg_bwd = self.ffma_bwd_weights(i)
                 a.d_wrs_rows, a.d_wfg_bwd = wrs_rows.data_ptr(), wfg_bwd.data_ptr()
                 native.check(lib.wn_block_bwd_data(ctypes.byref(a), stream), f"block bwd {i}")
             # weight gradients: plain GEMMs over (frames x channels) slices

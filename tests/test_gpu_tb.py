@@ -122,6 +122,9 @@ def test_tb_mode_requires_supported_shape(golden):
     (2, 420, 3, 2, True, 150),
     (3, 700, 4, 2, True, 300),         # several 256-frame items, gradients start inside an item
     (1, 1100, 6, 1, False, 37),        # no biases; most frames lie outside the receptive cone of the outputs
+    (2, 2200, 10, 1, True, 300),       # the benchmark's depth: dilations to 512 cross CTA and item boundaries; the
+                                       # gradients start at frame 1900, inside an item (the reference needs a folded
+                                       # length >= 2 at d = 512, so L >= ~2050)
 ])
 def test_fused_backward_matches_oracle_and_simt(B, L, layers, blocks, bias, out_len):
     """Training step through the chunked-pair kernels (forward with saved activations, wgmma data gradients, MN-major
@@ -177,6 +180,7 @@ def test_fused_backward_matches_oracle_and_simt(B, L, layers, blocks, bias, out_
     (256, 2, 700, 4, 2, 300),
     (512, 2, 600, 3, 2, 200),
     (512, 1, 1300, 6, 1, 64),
+    (512, 2, 2200, 10, 1, 300),        # dilations to 512, gradients from frame 1900 (inside an item)
 ])
 def test_single_pass_bf16_forward_backward(channels, B, L, layers, blocks, out_len):
     import torch.nn.functional as F

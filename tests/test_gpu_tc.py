@@ -147,6 +147,50 @@ def test_tc_backward_matches_simt_backward_and_oracle():
     assert not bad, bad[:12]
 
 
+@pytest.mark.parametrize("R,D,S,k,bwd", [
+    (256, 256, 256, 3, "tc"),          # three taps
+    (512, 256, 256, 2, "tc"),          # R != S: the residual / skip split of the output tiles
+    (256, 256, 512, 2, "tc"),
+    (256, 128, 256, 2, "ffma"),        # D % 256 != 0: tensor-core forward, FFMA backward
+])
+def test_auto_mode_two_launch_shapes_match_oracle(R, D, S, k, bwd):
+    """Nets the fused block does not cover take the two-launch tensor-core blocks under block_mode="auto"; a training step
+    through the runtime (dispatch, packs, buffers, the per-layer backward) against the oracle and its autograd."""
+    import torch.nn.functional as F
+    import wavenet_model as wmod
+    B, L, out_len = 2, 500, 90
+    kw = dict(layers=3, blocks=2, dilation_channels=D, residual_channels=R, skip_channels=S, end_channels=256,
+              classes=256, output_length=out_len, kernel_size=k, bias=True)
+    torch.manual_seed(13)
+    m = wmod.WaveNetModel(**kw)
+    spec = O.NetSpec(**kw)
+    idx = torch.randint(0, 256, (B, L), generator=torch.Generator().manual_seed(6))
+    tgt = torch.randint(0, 256, (B * out_len,), generator=torch.Generator().manual_seed(7))
+    m.load_state_dict(separate_head_relu_ties(m.state_dict(), spec, O.one_hot(idx, 256), out_len), strict=True)
+    p = {n: v.detach().clone().requires_grad_(True) for n, v in m.state_dict().items()}
+    want = O.forward(p, spec, O.one_hot(idx, 256))
+    F.cross_entropy(want, tgt).backward()
+    m = m.cuda()
+    rt = m._runtime()
+    assert rt.block_mode == "auto"
+    y = m.forward_indices(idx.cuda())
+    F.cross_entropy(y, tgt.cuda()).backward()
+    assert rt.last_block_mode == "tc" and rt.last_bwd_mode == bwd
+    e = rel_err(y.detach().cpu().numpy(), want.detach().numpy())
+    bad = []
+    for n, v in m.named_parameters():
+        g = p[n].grad
+        if g is None or float(g.abs().max()) == 0:
+            assert float(v.grad.abs().max()) == 0, n
+            continue
+        eg = rel_err(v.grad.cpu().numpy(), g.numpy())
+        if not eg < 1e-4:
+            bad.append((n, eg))
+    print(f"auto mode R={R} D={D} S={S} k={k}: logits {e:.2e}, backward {rt.last_bwd_mode}")
+    assert e < 1e-4, e
+    assert not bad, bad[:10]
+
+
 def test_packed_weights_follow_parameter_writes():
     """ADVICE r1: the packed-weight cache is keyed on tensor versions, which writes through ``p.data`` do not bump (the
     reference's optimizers.py:100 updates that way).  A backward invalidates the cache; so does the explicit call."""

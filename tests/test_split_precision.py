@@ -10,17 +10,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from block_ref import split_bf16, split_tf32
 from oracle import wavenet_oracle as O
-
-
-def split_bf16(t):
-    hi = t.to(torch.bfloat16).to(torch.float32)
-    return hi, (t - hi).to(torch.bfloat16).to(torch.float32)
-
-
-def split_tf32(t):
-    hi = ((t.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)      # cvt.rna.tf32.f32: nearest, ties away
-    return hi, t - hi
 
 
 def conv(inp, w, dilation, mode):
