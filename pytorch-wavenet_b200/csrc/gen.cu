@@ -2256,6 +2256,10 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int rank = (int)cluster_rank(), cl = blockIdx.x / CS, NS = p.NS, NL = p.n_layers;
     const int v0 = rank * VR;                           // first virtual rank of this CTA
+    // live streams of this cluster: slots 0 .. n_live-1.  A stream's bytes in every exchanged block are contiguous (64 at
+    // s * 64: cl8_unit_off, and the [stream][16] fp32 logits), so only the first 64 * n_live bytes of each block travel.
+    const int n_live = min(SB, NS - cl * SB);
+    const unsigned XVEC = 64u * (unsigned)n_live * NV;  // bytes of one exchange round that land in each CTA
     const int o0 = v0 * NV;                             // first channel this CTA owns in every stage vector
 
     {
@@ -2273,8 +2277,11 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
+    // Every exchange barrier expects the live bytes only.  The columns of empty stream slots are then never written by
+    // peers and may hold stale values or sampling scratch: harmless, since MMA columns (= streams) are independent, and
+    // every reduction and store works per (row, stream) and is guarded by fs_on / hs_g < NS.
     if (tid == 0)
-        for (int i = 0; i < 7; ++i) mbar_expect_tx(xbar + i, VEC);             // arm phase 0 of every exchange barrier
+        for (int i = 0; i < 7; ++i) mbar_expect_tx(xbar + i, XVEC);            // arm phase 0 of every exchange barrier
     for (int l = tid; l < NL; l += GEN_NT) {
         const int len = lay_s[l].ring_len;
         slot_s[l] = (p.t0 + len - 1) % len;
@@ -2286,8 +2293,10 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     const unsigned char* img_head = p.cl8_img + 3 * img_kind * NL + (size_t)v0 * CL8_IMGH;
 
     // push the staged blocks `sb` into blocks v0 .. v0+VR-1 of vector `vec` of every CTA of the cluster: the pusher warp
-    // (warp 9) reads each 512-byte block back (16 bytes per lane) and issues ONE st.async.v4 per destination -- a whole
-    // block per instruction, its bytes credited to the destination's mbarrier.  The alternatives tools/dsmem_probe.cu
+    // (warp 9) reads the live part of each 512-byte block back (16 bytes per lane, lanes 0 .. 4*n_live-1) and issues ONE
+    // st.async.v4 per destination and lane -- a whole block per instruction when all 8 streams are live, its bytes
+    // credited to the destination's mbarrier.  With one live stream a round moves 64 bytes per (source, destination)
+    // instead of 512 (tools/dsmem_probe.cu: I against H).  The alternatives tools/dsmem_probe.cu
     // compares are one cp.async.bulk per destination (which also occupies the SM's bulk-copy engine and needs a proxy
     // fence after staging), per-lane 8-byte stores from the worker warps, and a multicast copy from a global staging slot
     // (which needs a fence after the global stores).  The workers only signal "staged" (bar.arrive on barrier 2) and
@@ -2297,6 +2306,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
 #pragma unroll
     for (int d = 0; d < CS; ++d) rdelta[d] = (warp == GEN_WARPS + 1) ? mapa_u32(sm_base, (unsigned)d) - sm_base : 0u;
     auto push = [&](int sb, unsigned char* vec, int bar_i) {
+        if (lane >= 4 * n_live) return;
 #pragma unroll
         for (int vr = 0; vr < VR; ++vr) {
             const uint4 v = *reinterpret_cast<const uint4*>(stg + (sb * VR + vr) * BLK + lane * 16);
@@ -2423,7 +2433,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     auto xwait = [&](int i) {
         mbar_wait_bounded(xbar + i, (xpar >> i) & 1u);
         xpar ^= 1u << i;
-        if (tid == 0) mbar_expect_tx(xbar + i, VEC);
+        if (tid == 0) mbar_expect_tx(xbar + i, XVEC);
     };
     // one k-step of this warp's m-tile: A fragments (hi, lo) from the stage image, B fragments of the 8 streams from a block
     const int mt = warp & 1, kq = warp >> 1;

@@ -9,6 +9,9 @@
 //   G  like F with 1 KB per (source, destination)
 //   H  the payload of F staged in local shared memory, then ONE warp reads it back (16 B per lane) and issues one
 //      st.async.v4 per destination: a whole 512-byte block per instruction
+//   I  like H with 64 B per destination (lanes 0-3 only): the payload of one live stream out of 8
+//   J  like H with one mbarrier per source block; warp w reads blocks 4*(w/2)..+3, each as soon as its own barrier fires
+//   K  I and J together: 64 B per destination, one mbarrier per source block
 // Each round every CTA publishes V=16 values (x8 in E) to all 16 CTAs and needs all 256 values of the round before it may
 // publish the next one.  Prints cycles per round.
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dsmem_probe tools/dsmem_probe.cu
@@ -47,15 +50,23 @@ __global__ void __launch_bounds__(NT, 1) probe(int rounds, long long* cycles, fl
     __shared__ __align__(16) unsigned long long pairs[2][CL * V];      // A, B: {value, tag}
     __shared__ __align__(16) float vals[2][8][CL * V + 4];             // C, D, E: plain values ([stream][channel])
     __shared__ unsigned long long bar[2];
+    __shared__ unsigned long long jbar[2][CL];                           // J, K: one barrier per source block
     __shared__ __align__(128) float stage[2][256];                       // F, G: this CTA's contribution, staged
     __shared__ __align__(128) float blocks[2][CL][256];                  // F, G: received contributions, one block per source
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, rank = (int)crank();
     for (int i = tid; i < 2 * CL * V; i += NT) (&pairs[0][0])[i] = 0ull;
-    if (tid == 0) { mbar_init(bar, 1); mbar_init(bar + 1, 1); }
+    if (tid == 0) {
+        mbar_init(bar, 1); mbar_init(bar + 1, 1);
+        for (int i = 0; i < 2 * CL; ++i) mbar_init(&jbar[0][0] + i, 1);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
-    const unsigned bytes = (MODE == 4 || MODE == 5 || MODE == 7) ? 8 * CL * V * 4 : (MODE == 6) ? 16 * CL * V * 4 : CL * V * 4;
-    if (tid == 0) { mbar_expect(bar, bytes); mbar_expect(bar + 1, bytes); }
+    const unsigned bytes = (MODE == 4 || MODE == 5 || MODE == 7 || MODE == 9) ? 8 * CL * V * 4 : (MODE == 6) ? 16 * CL * V * 4 : CL * V * 4;
+    const unsigned jbytes = (MODE == 9) ? 512 : 64;                      // J, K: bytes per source block
+    if (tid == 0) {
+        mbar_expect(bar, bytes); mbar_expect(bar + 1, bytes);
+        for (int i = 0; i < 2 * CL; ++i) mbar_expect(&jbar[0][0] + i, jbytes);
+    }
     csync();
     float acc = 0.f;
     unsigned par[2] = {0, 0};
@@ -115,10 +126,28 @@ __global__ void __launch_bounds__(NT, 1) probe(int rounds, long long* cycles, fl
             if (tid == 0) mbar_expect(bar + b, bytes);
             acc += blocks[b][tid >> 4][tid & 15];
             __syncthreads();
-        } else if (MODE == 7) {
+        } else if (MODE == 9 || MODE == 10) {
             if (tid < 128) stage[b][tid] = myv;
             __syncthreads();
-            if (warp == 0) {
+            if (warp == 0 && (MODE == 9 || lane < 4)) {
+                const uint4 v = *reinterpret_cast<const uint4*>(&stage[b][lane * 4]);
+                const unsigned la = s32(&blocks[b][rank][lane * 4]), lb = s32(&jbar[b][rank]);
+#pragma unroll
+                for (int d = 0; d < CL; ++d) st_async4(mapa(la, d), v, mapa(lb, d));
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int src = 4 * (warp >> 1) + i;
+                mbar_wait(&jbar[b][src], par[b]);
+                if ((warp & 1) == 0 && lane == 0) mbar_expect(&jbar[b][src], jbytes);
+                acc += blocks[b][src][lane & 15];
+            }
+            par[b] ^= 1;
+            __syncthreads();
+        } else if (MODE == 7 || MODE == 8) {
+            if (tid < 128) stage[b][tid] = myv;
+            __syncthreads();
+            if (warp == 0 && (MODE == 7 || lane < 4)) {
                 const uint4 v = *reinterpret_cast<const uint4*>(&stage[b][lane * 4]);
                 const unsigned la = s32(&blocks[b][rank][lane * 4]), lb = s32(bar + b);
 #pragma unroll
@@ -179,6 +208,9 @@ int main() {
         run<5>("F bulk copy smem->dsmem, 512 B x 16 destinations", rounds, clusters);
         run<6>("G bulk copy smem->dsmem, 1 KB x 16 destinations", rounds, clusters);
         run<7>("H one warp: LDS.128 + st.async.v4, 512 B per instruction per destination", rounds, clusters);
+        run<8>("I like H, 64 B per destination (lanes 0-3: one live stream)", rounds, clusters);
+        run<9>("J like H, one mbarrier per source block, read as they land", rounds, clusters);
+        run<10>("K I + J: 64 B per destination, one mbarrier per source block", rounds, clusters);
     }
     return 0;
 }
