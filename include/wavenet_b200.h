@@ -219,6 +219,29 @@ typedef struct wn_tb_wgrad_args {
 } wn_tb_wgrad_args;
 int    wn_tb_wgrad(const wn_tb_wgrad_args* a, void* stream);
 
+/* ---------------------------------------------------------------- (T) global conditioning
+ * One condition vector h (G,) per sequence (WaveNet paper section 2.5) shifts every layer's pre-activations:
+ *     z[t] = tanh(Wf * x + bf + Vf h) * sigmoid(Wg * x + bg + Vg h)
+ * For one sequence, bf + Vf h and bg + Vg h are just that sequence's filter / gate biases.  The kernels read them from a
+ * CONDITION TABLE instead of bf / bg, so a conditioned epilogue does the same work as an unconditioned one:
+ *     d_cond [n_layers][n_items][2D] fp32: bf + Vf h in [0, D), bg + Vg h in [D, 2D)   (items = sequences or sampler streams)
+ * wn_cond_table builds it for all layers in one launch: d_ptrs is a DEVICE table [n_layers][4] of {Vf, Vg, bf, bg} (Vf / Vg
+ * are the (D, G, 1) weights of the 1x1 conditioning convolutions; biases may be 0), d_h (n_items, G) fp32.  Each entry is a
+ * sequential fp32 sum over g plus the bias, so one-hot rows (class labels) give exactly bias + one column of V, and V = 0
+ * gives exactly the bias.
+ * The *_cond entry points are the plain ones plus the table; a NULL table is the plain entry point.  wn_block_fwd_cond and
+ * wn_tb_block_fwd_cond take ONE layer's slice [B][2D] (2 * channels), wn_tb_stack_fwd_cond the whole table [n_layers][B][2D].
+ * wn_cond_frame_sums is the reduction behind the gradient of V:  dV[n][g] = sum_b h[b][g] * d_out[b][n] with
+ *     d_out[b][n] = sum_{gz <= t < L} dfg[b][t][n]                            (n < C = 2D; deterministic; no atomics)
+ * over the filter/gate pre-activation gradient of the backward: pair = 0 for the frames layout (B, L, C) fp32 of
+ * wn_block_bwd_data, pair = 1 for the chunked pair layout (B, 2, C/8, L, 8) bf16 of wn_tb_block_bwd_data (hi + lo). */
+int wn_cond_table(const float* const* d_ptrs, int n_layers, int D, int G, const float* d_h, int n_items, float* d_out,
+                  void* stream);
+int wn_block_fwd_cond(const wn_block_args* a, const float* d_cond, void* stream);
+int wn_tb_block_fwd_cond(const wn_tb_block_args* a, const float* d_cond, void* stream);
+int wn_tb_stack_fwd_cond(const wn_tb_stack_args* a, const float* d_cond, void* stream);
+int wn_cond_frame_sums(const void* d_dfg, int pair, int B, int L, int C, int gz, float* d_out, void* stream);
+
 /* ---------------------------------------------------------------- (T) head
  * replaces relu -> end_conv_1 -> relu -> end_conv_2 (wavenet_model.py:167-169) and forward()'s
  * slice/transpose/view (:191-196): logits (B*out_len, classes) for the LAST out_len frames only.
@@ -398,6 +421,12 @@ int wn_gen_set_mode(wn_gen_handle* h, int mode);
 /* The parameter tensors given to wn_gen_create were written in place (an optimizer step): kernels 1-5 read them on every
  * launch and need nothing; kernel 6 keeps pre-split copies, which the next wn_gen_reset rebuilds after this call. */
 int wn_gen_weights_changed(wn_gen_handle* h);
+/* Global conditioning of the sampler: d_cond is a condition table [n_layers][n_streams][2D] (see wn_cond_table); every
+ * kernel takes entry (layer, stream) as that stream's filter / gate biases.  Because the table holds bf + Vf h | bg + Vg h,
+ * it must be rebuilt (wn_cond_table) after ANY change of Vf, Vg, bf or bg -- an optimizer step that updates the biases
+ * included -- before the next wn_gen_run.  The table is read on every launch
+ * and must stay alive while the handle samples with it; NULL clears it (unconditioned sampling). */
+int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond);
 /* Synchronise the stream and report whether a launch aborted (a CTA waited > ~3 s for a tag): 0 = fine. */
 int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer

@@ -6,6 +6,8 @@
   INDICES (uint8) instead of a (classes, item_length) float one-hot matrix.  ``WaveNetModel.forward_indices`` gathers the
   start_conv column of each index on the GPU, which is bit-identical to the dense convolution on the one-hot input and
   moves 1 byte per sample over PCIe / HBM instead of 1 KB.
+* ``condition_on_file=True`` makes items ``(x, file_index, target)``: the index of the array that holds the item's last
+  target sample, a class label for training a model conditioned on the file (``WaveNetModel(condition_channels=...)``).
 * ``write_wav``  16-bit PCM writer for generated audio (the reference calls librosa.output.write_wav, generate_script.py:35;
   librosa is not a dependency here).
 Building a dataset from audio files (``create_dataset``) needs librosa exactly as in the reference and raises without it.
@@ -60,13 +62,15 @@ class WavenetDataset(torch.utils.data.Dataset):
     (reference audio_data.py:12-131: same item index -> sample offset map, same cross-file reads)."""
 
     def __init__(self, dataset_file, item_length, target_length, file_location=None, classes=256, sampling_rate=16000,
-                 mono=True, normalize=False, dtype=np.uint8, train=True, test_stride=100, one_hot=True):
+                 mono=True, normalize=False, dtype=np.uint8, train=True, test_stride=100, one_hot=True,
+                 condition_on_file=False):
         self.dataset_file = dataset_file
         self._item_length = item_length
         self._test_stride = test_stride
         self.target_length = target_length
         self.classes = classes
         self.one_hot = one_hot
+        self.condition_on_file = condition_on_file
         self.mono = self.normalize = self.sampling_rate = self.dtype = None      # unknown for an existing file, as upstream
         if not os.path.isfile(dataset_file):
             assert file_location is not None, "no location for dataset files specified"
@@ -123,15 +127,22 @@ class WavenetDataset(torch.utils.data.Dataset):
             return np.asarray(first[pos:pos + n])
         return np.concatenate((np.asarray(first[pos:]), np.asarray(self.data['arr_' + str(fi + 1)][:spill])))
 
+    def file_index(self, idx):
+        """Index of the array that holds the last target sample of item ``idx``."""
+        return bisect.bisect_right(self.start_samples, self._sample_index(idx) + self._item_length) - 1
+
     def __getitem__(self, idx):
         sample = self._read(self._sample_index(idx), self._item_length + 1)
         target = torch.from_numpy(sample[-self.target_length:].astype(np.int64)).unsqueeze(0)
         if not self.one_hot:
-            return torch.from_numpy(sample[:self._item_length].astype(np.uint8)), target
-        example = torch.from_numpy(sample[:self._item_length].astype(np.int64))
-        one_hot = torch.zeros(self.classes, self._item_length)
-        one_hot.scatter_(0, example.unsqueeze(0), 1.)
-        return one_hot, target
+            x = torch.from_numpy(sample[:self._item_length].astype(np.uint8))
+        else:
+            example = torch.from_numpy(sample[:self._item_length].astype(np.int64))
+            x = torch.zeros(self.classes, self._item_length)
+            x.scatter_(0, example.unsqueeze(0), 1.)
+        if self.condition_on_file:
+            return x, torch.tensor(self.file_index(idx), dtype=torch.int64), target
+        return x, target
 
     def __len__(self):
         test_length = math.floor(self._length / self._test_stride)

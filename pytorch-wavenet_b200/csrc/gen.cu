@@ -58,6 +58,7 @@ struct GenParams {
     int wslot_floats, n_wslots;                // weight prefetch ring in shared memory (0 slots: read weights via L2)
     long long* trace;       // optional: clock64 stamps of CTA 0 / thread 0 during the last evaluation (wn_gen_read_trace)
     const unsigned char* cl8_img;              // batched cluster kernel: fragment-ordered bf16 hi/lo weight images (cl8_pack_kernel)
+    const float* cond;      // optional condition table [n_layers][NS][2D]: each stream's filter / gate biases (bf + Vf h | bg + Vg h)
 };
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -196,13 +197,14 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
                 const float* w = ((it & 1) ? L.wg : L.wf) + (size_t)c * K1;
                 const float* bp = (it & 1) ? L.bg : L.bf;
                 const float bias = bp ? __ldg(bp + c) : 0.f;
+                const float* cb = p.cond ? p.cond + (size_t)l * NS * 2 * D + ((it & 1) ? D : 0) + c : nullptr;
                 for (int s0 = 0; s0 < NS; s0 += SB) {
                     float acc[SB];
                     row_dot<SB>(w, regA, K1, NS, s0, lane, acc);
                     if (lane == 0) {
 #pragma unroll
                         for (int j = 0; j < SB; ++j)
-                            if (s0 + j < NS) pre[it * NS + s0 + j] = acc[j] + bias;
+                            if (s0 + j < NS) pre[it * NS + s0 + j] = acc[j] + (cb ? __ldg(cb + (size_t)(s0 + j) * 2 * D) : bias);
                     }
                 }
             }
@@ -630,8 +632,9 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
             uint2* zl = p.zLL + ((size_t)(par * NL + l) * NS) * D;
             for (int i = tid; i < nD * NS; i += GEN_NT) {
                 const int ci = i / NS, s = i - ci * NS, c = oD + ci;
-                const float f = sum_parts(2 * ci, nw, s) + (L.bf ? __ldg(L.bf + c) : 0.f);
-                const float g = sum_parts(2 * ci + 1, nw, s) + (L.bg ? __ldg(L.bg + c) : 0.f);
+                const float* cb = p.cond ? p.cond + ((size_t)l * NS + s) * 2 * D : nullptr;     // this stream's biases
+                const float f = sum_parts(2 * ci, nw, s) + (cb ? __ldg(cb + c) : (L.bf ? __ldg(L.bf + c) : 0.f));
+                const float g = sum_parts(2 * ci + 1, nw, s) + (cb ? __ldg(cb + D + c) : (L.bg ? __ldg(L.bg + c) : 0.f));
                 st_pair(zl + (size_t)s * D + c, tanh_(f) * sigmoid_(g), tag);
             }
             // ---- stage 2: residual rows (-> next layer's ring slot t) and skip rows (-> running sums)
@@ -1185,8 +1188,13 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_fast(const GenParam
                 const float* pf = part + stage_par * GEN_WARPS + (2 * tid) * HS1;
                 float f = pf[0], g = pf[HS1];
                 for (int q = 1; q < HS1; ++q) { f += pf[q]; g += pf[HS1 + q]; }
-                f += L.bf ? __ldg(L.bf + c) : 0.f;
-                g += L.bg ? __ldg(L.bg + c) : 0.f;
+                if (p.cond) {                                      // one stream: the table is [n_layers][1][2D]
+                    f += __ldg(p.cond + (size_t)l * 2 * D + c);
+                    g += __ldg(p.cond + (size_t)l * 2 * D + D + c);
+                } else {
+                    f += L.bf ? __ldg(L.bf + c) : 0.f;
+                    g += L.bg ? __ldg(L.bg + c) : 0.f;
+                }
                 st_pair(zl + c, tanh_(f) * sigmoid_(g), tag);
             }
             TR();          // 4: z published
@@ -1566,8 +1574,9 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
                 for (int jj = 0; jj < CL_ROWS / 2; ++jj)
                     if (2 * jj < rw1 && ((lane >> 4) == (jj & 1))) {
                         const int ci = (warp * rw1 >> 1) + jj, c = oD + ci;
-                        const float f = acc[2 * jj] + (L.bf ? __ldg(L.bf + c) : 0.f);
-                        const float g = acc[2 * jj + 1] + (L.bg ? __ldg(L.bg + c) : 0.f);
+                        const float* cb = p.cond ? p.cond + ((size_t)l * NS + stream) * 2 * D : nullptr;
+                        const float f = acc[2 * jj] + (cb ? __ldg(cb + c) : (L.bf ? __ldg(L.bf + c) : 0.f));
+                        const float g = acc[2 * jj + 1] + (cb ? __ldg(cb + D + c) : (L.bg ? __ldg(L.bg + c) : 0.f));
                         st_remote_pair(zbuf + c, (unsigned)dst, tanh_(f) * sigmoid_(g), tag_z);
                     }
             }
@@ -1943,8 +1952,13 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams 
                 const float* pf = part + stage_par * GEN_WARPS + (2 * vi) * HS1;
                 float f = pf[0], g = pf[HS1];
                 for (int q = 1; q < HS1; ++q) { f += pf[q]; g += pf[HS1 + q]; }
-                f += L.bf ? __ldg(L.bf + c) : 0.f;
-                g += L.bg ? __ldg(L.bg + c) : 0.f;
+                if (p.cond) {                                      // one stream: the table is [n_layers][1][2D]
+                    f += __ldg(p.cond + (size_t)l * 2 * D + c);
+                    g += __ldg(p.cond + (size_t)l * 2 * D + D + c);
+                } else {
+                    f += L.bf ? __ldg(L.bf + c) : 0.f;
+                    g += L.bg ? __ldg(L.bg + c) : 0.f;
+                }
                 const float zv = tanh_(f) * sigmoid_(g);
                 st_remote_pair(zb + c, (unsigned)(tid & 15), zv, tag_z);
                 if ((tid & 15) == 0) st_pair(zl + c, zv, rtag);
@@ -2227,7 +2241,9 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
 // a CTA of a CS-cluster owns VR = 16 / CS consecutive virtual ranks and walks them one after the other in every stage.  Only
 // few clusters of 16 CTAs are co-resident (tools/cluster_occ.cu) but about twice as many clusters of 8: CS = 8 runs 64 streams
 // (8 clusters) in one wave on 64 SMs, at twice the per-CTA work -- the step is bound by the exchange latency, not by it.
-template <int CS>
+// COND: the filter / gate biases come from the condition table (a separate instantiation: the per-layer branch costs the
+// unconditioned single-stream kernel ~6 % of its time per sample).
+template <int CS, bool COND>
 __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
     extern __shared__ __align__(128) unsigned char smb[];
     constexpr int W = CL8_W, SB = CL8_SB, NV = 16, BLK = CL8_BLK, VEC = CL8_VEC, VR = CL / CS, NVC = NV * VR;
@@ -2564,7 +2580,10 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             unsigned char* xc = Xcur + (l & 1) * VEC;
             unsigned char* zb = Xz + (l & 1) * VEC;
             // biases of this thread's outputs: requested now, used one or two stages later
-            const float b_f = (fin_a && L.bf) ? __ldg(L.bf + fch) : 0.f, b_g = (fin_a && L.bg) ? __ldg(L.bg + fch) : 0.f;
+            // conditioned: the stream's own filter / gate biases, from the condition table
+            const float* cb = COND ? p.cond + ((size_t)l * NS + fsg) * 2 * W : nullptr;
+            const float b_f = COND ? ((fin_a && fs_on) ? __ldg(cb + fch) : 0.f) : ((fin_a && L.bf) ? __ldg(L.bf + fch) : 0.f);
+            const float b_g = COND ? ((fin_a && fs_on) ? __ldg(cb + W + fch) : 0.f) : ((fin_a && L.bg) ? __ldg(L.bg + fch) : 0.f);
             const float b_r = (fin_a && L.br) ? __ldg(L.br + fch) : 0.f, b_s = (fin_s && L.bs) ? __ldg(L.bs + fch) : 0.f;
             // ================= stage 1: m-tile 0 = filter rows, 1 = gate rows; k-steps 4*kq+i of the old taps, then of h
             {
@@ -3123,11 +3142,11 @@ static int launch_gen_cluster(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     return 0;
 }
 
-template <int CS>
+template <int CS, bool COND>
 static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, int* max_clusters_out, bool launch) {
     const size_t smem = (CS == 16) ? h->smem_cl8 : h->smem_cl8_8;
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * CS));
     cfg.blockDim = dim3(GEN_NT + 64 + (CS == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
@@ -3141,18 +3160,18 @@ static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, in
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS>, &cfg));
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND>, &cfg));
     if (max_clusters_out) *max_clusters_out = max_clusters;
     if (!launch) return 0;
     WN_REQUIRE(max_clusters >= 1, WN_E_UNSUPP, "wn_gen_run: a %d-CTA cluster cannot be scheduled on this device", CS);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS>, p));   // clusters are independent: more than fit run in waves
+    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND>, p));   // clusters are independent: more than fit run in waves
     return 0;
 }
 // Cluster size: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8 (15 clusters fit instead of 7).
 static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     if (h->cl8_cs == 0) {
         int fit16 = 0;
-        const int rc = launch_gen_cl8_cs<16>(h, p, st, &fit16, false);
+        const int rc = launch_gen_cl8_cs<16, false>(h, p, st, &fit16, false);
         if (rc) return rc;
         const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
         h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
@@ -3161,7 +3180,9 @@ static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
             if (v == 16 || (v == 8 && h->cl8_8_ok)) h->cl8_cs = v;
         }
     }
-    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16>(h, p, st, nullptr, true) : launch_gen_cl8_cs<8>(h, p, st, nullptr, true);
+    if (p.cond)
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true>(h, p, st, nullptr, true) : launch_gen_cl8_cs<8, true>(h, p, st, nullptr, true);
+    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false>(h, p, st, nullptr, true) : launch_gen_cl8_cs<8, false>(h, p, st, nullptr, true);
 }
 
 // 64 CTAs as 4 clusters of 16, all co-resident (the clusters exchange through the L2 while they run): launched with the
@@ -3227,6 +3248,12 @@ extern "C" int wn_gen_set_mode(wn_gen_handle* h, int mode) {
 extern "C" int wn_gen_weights_changed(wn_gen_handle* h) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_weights_changed: null handle");
     h->cl8_packed = false;          // the next wn_gen_reset splits the weights again
+    return 0;
+}
+
+extern "C" int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_condition: null handle");
+    h->base.cond = d_cond;
     return 0;
 }
 

@@ -68,6 +68,7 @@ struct BlockParams {
     int in_start, out_start, skip_start, skip_init;
     int N1p, N2p, Kz;       // Kz = z channels incl. padding = N1p/2
     float* fg_save;         // optional (B,L,2D): tanh / sigmoid outputs for the backward
+    const float* cond;      // optional (B,2D): per-sequence filter / gate biases [bf + Vf h | bg + Vg h], used instead of bfg
 };
 
 template <int TM>
@@ -101,7 +102,16 @@ __global__ void __launch_bounds__(NT, 1) block_fwd_kernel(const BlockParams p) {
         mainloop<TM, false>(acc, al, nullptr, p.wfg_t, p.N1p, ch * NC, al.K, As, Bs);
         const float4 bf4 = __ldg(reinterpret_cast<const float4*>(p.bfg + ch * NC + tx * 4));
         const float4 bg4 = __ldg(reinterpret_cast<const float4*>(p.bfg + ch * NC + 64 + tx * 4));
-        const float bfv[4] = {bf4.x, bf4.y, bf4.z, bf4.w}, bgv[4] = {bg4.x, bg4.y, bg4.z, bg4.w};
+        float bfv[4] = {bf4.x, bf4.y, bf4.z, bf4.w}, bgv[4] = {bg4.x, bg4.y, bg4.z, bg4.w};
+        if (p.cond != nullptr) {                                   // conditioned: this sequence's own biases
+            const float* cb = p.cond + (size_t)b * 2 * p.D;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int c = ch * 64 + tx * 4 + q;
+                bfv[q] = c < p.D ? __ldg(cb + c) : 0.f;
+                bgv[q] = c < p.D ? __ldg(cb + p.D + c) : 0.f;
+            }
+        }
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             float* zrow = Zs + (size_t)(ch * 64 + tx * 4 + q) * (TM + ZPAD);
@@ -435,7 +445,9 @@ extern "C" int wn_start_fwd_index_i64(const int64_t* d_idx, const float* d_w_t, 
     return start_index_impl<int64_t>(d_idx, d_w_t, d_b_p, d_h, B, classes, L, R, stream);
 }
 
-extern "C" int wn_block_fwd(const wn_block_args* a, void* stream) {
+extern "C" int wn_block_fwd(const wn_block_args* a, void* stream) { return wn_block_fwd_cond(a, nullptr, stream); }
+
+extern "C" int wn_block_fwd_cond(const wn_block_args* a, const float* d_cond, void* stream) {
     WN_REQUIRE(a, WN_E_BADARG, "wn_block_fwd: null args");
     WN_REQUIRE(a->d_h_in && a->d_h_out && a->d_skip && a->d_wfg_t && a->d_bfg && a->d_wrs_t && a->d_brs, WN_E_BADARG,
                "wn_block_fwd: null pointer");
@@ -454,6 +466,7 @@ extern "C" int wn_block_fwd(const wn_block_args* a, void* stream) {
     p.in_start = a->in_start; p.out_start = a->out_start; p.skip_start = a->skip_start; p.skip_init = a->skip_init;
     p.N1p = n1p_of(a->D); p.N2p = n2p_of(a->R + a->S); p.Kz = p.N1p / 2;
     p.fg_save = a->d_fg_save;
+    p.cond = d_cond;
     const int tm = pick_tm(p.Kz, smem_limit_bytes());
     WN_REQUIRE(tm > 0, WN_E_UNSUPP, "wn_block_fwd: dilation_channels=%d does not fit shared memory", a->D);
     const size_t smem = two_phase_smem(tm, p.Kz);

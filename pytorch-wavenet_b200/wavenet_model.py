@@ -153,6 +153,24 @@ class _Packs:
             rt._ptr_table_cache = cached
         return cached[1]
 
+    def cond_table(self, h, stream):
+        """Condition table [n_layers][N][2D] for the (N, G) fp32 condition rows ``h`` (wn_cond_table): every item's filter /
+        gate biases bf + Vf h | bg + Vg h, which the conditioned kernels read instead of bf / bg."""
+        rt, lib, m = self.rt, native.lib(), self.rt.model
+        nl, D = m.layers * m.blocks, m.dilation_channels
+        P = rt._params()
+        rows = [[native.ptr(t) or 0 for t in (m.filter_cond_convs[i].weight, m.gate_cond_convs[i].weight,
+                                              P["filt"][i][1], P["gate"][i][1])] for i in range(nl)]
+        key = tuple(map(tuple, rows))
+        cached = rt.__dict__.get("_cond_ptr_cache")
+        if cached is None or cached[0] != key:
+            cached = (key, torch.tensor(rows, dtype=torch.int64, device=rt.device()))
+            rt._cond_ptr_cache = cached
+        out = torch.empty(nl, h.shape[0], 2 * D, device=rt.device(), dtype=torch.float32)
+        native.check(lib.wn_cond_table(cached[1].data_ptr(), nl, D, h.shape[1], h.data_ptr(), h.shape[0], out.data_ptr(),
+                                       stream), "condition table")
+        return out
+
     def _build_tb(self, stream):
         rt, lib = self.rt, native.lib()
         R, nl = self._dims()[0], self._dims()[6]
@@ -273,10 +291,11 @@ class _Runtime:
         return self.packed
 
     # ------------------------------------------------------------------ training-path forward
-    def stack_forward(self, x, out_len, index_input=False, save=None):
+    def stack_forward(self, x, out_len, index_input=False, save=None, cond=None):
         """x: (B, classes, L) float32 one-hot/dense, or (B, L) uint8/int64 indices when index_input.
         Returns logits (B*out_len, classes) for the last out_len frames (out_len=None: all T_final frames).
-        save: optional dict; filled with what the backward needs (every layer's input, tanh/sigmoid outputs, skip)."""
+        save: optional dict; filled with what the backward needs (every layer's input, tanh/sigmoid outputs, skip).
+        cond: the (B, G) fp32 condition rows of a conditioned model (WaveNetModel._condition), else None."""
         m, lib = self.model, native.lib()
         dev = self.device()
         if x.device != dev:
@@ -314,8 +333,18 @@ class _Runtime:
         if self.block_mode == "tb" and not use_tb:
             raise RuntimeError("wavenet_b200: the fused tensor-core block needs R = D = S in (256, 512), kernel_size = 2 "
                                f"(got {R},{D},{S},{k})")
+        ctab = None
+        if cond is not None:
+            if self.block_mode == "tc" or (self.fast_tf32 and not use_tb):
+                raise RuntimeError("wavenet_b200: a conditioned model runs on the fused tensor-core blocks (block_mode 'tb' / "
+                                   "'auto') or the FFMA blocks ('ffma'); the two-launch 'tc' blocks have no conditioned kernel")
+            if cond.shape[0] != B:
+                raise RuntimeError(f"wavenet_b200: {cond.shape[0]} condition rows for a batch of {B}")
+            ctab = W.cond_table(cond, stream)
+            if save is not None:
+                save["cond"] = cond
         if use_tb:
-            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save)
+            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save, ctab)
         if save is not None:
             h_all = torch.empty(n_layers + 1, B, L, R, **f32)      # h_all[i] = input of layer i
             fg_all = torch.empty(n_layers, B, L, 2 * D, **f32)     # tanh / sigmoid outputs
@@ -335,7 +364,7 @@ class _Runtime:
         else:
             native.check(lib.wn_start_fwd_dense(x.data_ptr(), ws_t.data_ptr(), bs_p.data_ptr(), h0.data_ptr(),
                                                 B, Cc, L, R, stream), "start")
-        use_tc = self.block_mode != "ffma" and bool(lib.wn_tc_supported(R, D, S, k))     # "auto" with autograd / "tb" n/a
+        use_tc = self.block_mode != "ffma" and ctab is None and bool(lib.wn_tc_supported(R, D, S, k))     # "auto" / "tb" n/a
         if self.block_mode == "tc" and not use_tc:
             raise RuntimeError(f"wavenet_b200: tensor-core blocks need R%256==0, S%256==0, D%128==0 (got {R},{S},{D})")
         self.last_block_mode = "tc" if use_tc else "ffma"
@@ -368,7 +397,10 @@ class _Runtime:
             else:
                 wfg, bfg, wrs, brs = W["layers"][i]
                 a.d_wfg_t, a.d_bfg, a.d_wrs_t, a.d_brs = wfg.data_ptr(), bfg.data_ptr(), wrs.data_ptr(), brs.data_ptr()
-                native.check(lib.wn_block_fwd(ctypes.byref(a), stream), f"block {i}")
+                if ctab is None:
+                    native.check(lib.wn_block_fwd(ctypes.byref(a), stream), f"block {i}")
+                else:
+                    native.check(lib.wn_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream), f"block {i}")
             if save is None:
                 src, dst = dst, src
             elif i + 1 < n_layers:
@@ -388,7 +420,7 @@ class _Runtime:
                         index_input=index_input, B=B, L=L)
         return logits
 
-    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None):
+    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None, ctab=None):
         """Forward on the fused tensor-core blocks (wn_tb_block_fwd): chunked bf16-pair activations, one launch per residual
         block, z resident on the SM (csrc/tc_block.cu).  With ``save`` every layer's input pair and tanh/sigmoid outputs are
         kept for _backward_tb."""
@@ -446,7 +478,10 @@ class _Runtime:
             sa.d_flags = flags.data_ptr()
             sa.n_layers, sa.channels, sa.precision, sa.B, sa.L, sa.skip_start = n_layers, R, prec, B, L, plan.skip_start
             sa.dilations, sa.in_start, sa.out_start = ints(dil), ints(plan.in_start), outs
-            native.check(lib.wn_tb_stack_fwd(ctypes.byref(sa), stream), "tb stack")
+            if ctab is None:
+                native.check(lib.wn_tb_stack_fwd(ctypes.byref(sa), stream), "tb stack")
+            else:
+                native.check(lib.wn_tb_stack_fwd_cond(ctypes.byref(sa), ctab.data_ptr(), stream), "tb stack")
             n_block_launches = 1
         else:
             a = native.TbBlockArgs()
@@ -459,7 +494,10 @@ class _Runtime:
                 a.dilation, a.in_start, a.out_start, a.skip_init = d, plan.in_start[i], plan.out_start[i], int(i == 0)
                 if save is not None:
                     a.d_fg_save = fg_all[i].data_ptr()
-                native.check(lib.wn_tb_block_fwd(ctypes.byref(a), stream), f"tb block {i}")
+                if ctab is None:
+                    native.check(lib.wn_tb_block_fwd(ctypes.byref(a), stream), f"tb block {i}")
+                else:
+                    native.check(lib.wn_tb_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream), f"tb block {i}")
                 if save is None:
                     src, dst = dst, src
                 elif i + 1 < n_layers:
@@ -603,8 +641,10 @@ class _Runtime:
             if bf is not None:
                 bsum = dfg[:, :, :, gz:, :].float().sum((0, 1, 3)).reshape(2 * D)
                 grads[f"filter_convs.{i}.bias"], grads[f"gate_convs.{i}.bias"] = bsum[:D].clone(), bsum[D:].clone()
+            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 1, gz, stream)
             if reducer is not None:
                 reducer.reduce_flat_async(bucket)
+                reducer.reduce_async(cgrads)
                 if bf is not None or br is not None or bs is not None:
                     reducer.reduce_async([grads.get(f"{n}.{i}.bias") for n in ("filter_convs", "gate_convs", "residual_convs",
                                                                               "skip_convs")])
@@ -627,6 +667,21 @@ class _Runtime:
             reducer.reduce_async([grads["start_conv.weight"], grads.get("start_conv.bias")])
             reducer.wait_all()
         return grads
+
+    def cond_weight_grads(self, saved, grads, i, dfg, pair, gz, stream):
+        """Gradients of layer i's conditioning weights: dV[n][g] = sum_b h[b][g] * sum_{t >= gz} dfg[b][t][n]
+        (wn_cond_frame_sums per sequence, then the contraction over the batch).  Returns them, or [] when unconditioned."""
+        h = saved.get("cond")
+        if h is None:
+            return []
+        B, L, D = saved["B"], saved["L"], self.model.dilation_channels
+        sums = torch.empty(B, 2 * D, device=h.device, dtype=torch.float32)
+        native.check(native.lib().wn_cond_frame_sums(dfg.data_ptr(), pair, B, L, 2 * D, gz, sums.data_ptr(), stream),
+                     "condition frame sums")
+        dv = torch.einsum("bn,bg->ng", sums, h)
+        gf, gg = dv[:D].unsqueeze(-1).contiguous(), dv[D:].unsqueeze(-1).contiguous()
+        grads[f"filter_cond_convs.{i}.weight"], grads[f"gate_cond_convs.{i}.weight"] = gf, gg
+        return [gf, gg]
 
     # ------------------------------------------------------------------ training-path backward
     def ffma_bwd_weights(self, i):
@@ -802,9 +857,10 @@ class _Runtime:
             if bf is not None:
                 bsum = dfg[:, gz:, :].sum((0, 1))
                 grads[f"filter_convs.{i}.bias"], grads[f"gate_convs.{i}.bias"] = bsum[:D].clone(), bsum[D:].clone()
+            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 0, gz, stream)
             if reducer is not None:
                 reducer.reduce_async([grads.get(f"{n}.{i}.{wb}") for n in ("filter_convs", "gate_convs", "residual_convs",
-                                                                         "skip_convs") for wb in ("weight", "bias")])
+                                                                         "skip_convs") for wb in ("weight", "bias")] + cgrads)
             dh_out, gs_out = dh_in, gs_in
         # ---------------- start conv
         dh0 = dh_out[:, gs_out:, :]
@@ -887,9 +943,10 @@ class _Runtime:
         return t0 + args.n_evals
 
     def generate(self, num_samples, first, temperature, regularize, uniforms=None, forced=None,
-                 want_logits=False, callbacks=None):
+                 want_logits=False, callbacks=None, cond=None):
         """first: (NS, n_given) int array.  Returns (indices (NS, num_samples) int64 ndarray, logits or None, t_end).
-        callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done."""
+        callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done.
+        cond: the (NS, G) fp32 condition rows of a conditioned model, else None."""
         m = self.model
         dev = self.device()
         self.step_session = None             # a generate_fast run restarts the device queues (wavenet_model.py:250)
@@ -898,6 +955,10 @@ class _Runtime:
         if n_given < 1:
             raise RuntimeError("first_samples must hold at least one sample")
         s = self.sampler(NS)
+        # the condition table is read by every launch of this run: the sampler entry keeps it alive
+        s["cond"] = None if cond is None else self.packed_weights(torch.cuda.current_stream(dev).cuda_stream).cond_table(
+            cond, torch.cuda.current_stream(dev).cuda_stream)
+        native.check(native.lib().wn_gen_set_condition(s["handle"], native.ptr(s["cond"])), "gen condition")
         d_first = torch.from_numpy(first).to(dev, non_blocking=True)
         d_out = torch.zeros(NS, max(num_samples, 1), device=dev, dtype=torch.int32)
         d_uni = d_forced = d_logits = None
@@ -940,11 +1001,11 @@ class _StackFunction(torch.autograd.Function):
     """forward()/wavenet() as one autograd node: parameters in, logits out; the input carries no gradient."""
 
     @staticmethod
-    def forward(ctx, model, x, out_len, index_input, *params):
+    def forward(ctx, model, x, out_len, index_input, cond, *params):
         saved = {}
         rt = model._runtime()
         with torch.no_grad(), torch.cuda.device(rt.device()):
-            y = rt.stack_forward(x, out_len, index_input=index_input, save=saved)
+            y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond)
         ctx.model, ctx.saved = model, saved
         ctx.names = [n for n, _ in model.named_parameters()]
         return y
@@ -959,7 +1020,7 @@ class _StackFunction(torch.autograd.Function):
             g = rt.stack_backward(ctx.saved, dlogits)
         ctx.saved = None
         rt.invalidate()          # an optimizer step follows; it may write through p.data, which no version counter sees
-        return (None, None, None, None) + tuple(g.get(n) for n in ctx.names)
+        return (None, None, None, None, None) + tuple(g.get(n) for n in ctx.names)
 
 
 class WaveNetModel(nn.Module):
@@ -978,6 +1039,9 @@ class WaveNetModel(nn.Module):
         kernel_size (Int):          Size of the dilation kernel
         dtype:                      Parameter type of this model (kept for API compatibility)
         bias (Bool):                bias on start/filter/gate/residual/skip convs (the head always has bias)
+        condition_channels (Int):   G > 0: global conditioning (WaveNet paper section 2.5) on one (G,) vector h per
+                                    sequence, a class label or a dense embedding; every layer adds Vf h / Vg h to its
+                                    filter / gate pre-activations (``filter_cond_convs`` / ``gate_cond_convs``, 1x1, no bias)
 
     Shape:
         - Input: (N, classes, L) float32 one-hot, L >= receptive_field + output_length - 1 recommended
@@ -985,7 +1049,8 @@ class WaveNetModel(nn.Module):
     """
 
     def __init__(self, layers=10, blocks=4, dilation_channels=32, residual_channels=32, skip_channels=256,
-                 end_channels=256, classes=256, output_length=32, kernel_size=2, dtype=torch.FloatTensor, bias=False):
+                 end_channels=256, classes=256, output_length=32, kernel_size=2, dtype=torch.FloatTensor, bias=False,
+                 condition_channels=0):
         super(WaveNetModel, self).__init__()
         self.layers = layers
         self.blocks = blocks
@@ -1022,6 +1087,14 @@ class WaveNetModel(nn.Module):
                 d *= 2
         self.end_conv_1 = nn.Conv1d(skip_channels, end_channels, 1, bias=True)
         self.end_conv_2 = nn.Conv1d(end_channels, classes, 1, bias=True)
+        # created last, so that a seeded construction gives every other parameter the value an unconditioned net gets
+        self.condition_channels = condition_channels
+        if condition_channels > 0:
+            self.filter_cond_convs = nn.ModuleList()
+            self.gate_cond_convs = nn.ModuleList()
+            for _ in range(layers * blocks):
+                self.filter_cond_convs.append(nn.Conv1d(condition_channels, dilation_channels, 1, bias=False))
+                self.gate_cond_convs.append(nn.Conv1d(condition_channels, dilation_channels, 1, bias=False))
 
         self.output_length = output_length
         self.receptive_field = receptive_field
@@ -1042,14 +1115,17 @@ class WaveNetModel(nn.Module):
         return state
 
     # ------------------------------------------------------------------ training-time path
-    def wavenet(self, input, dilation_func=None):
+    def wavenet(self, input, dilation_func=None, condition=None):
         """All T_final output columns, (N, classes, T_final), like the reference's wavenet() with wavenet_dilate.
         With ``dilation_func=self.queue_dilate`` it advances the fast-generation state by the one-hot column(s)
         in ``input`` and returns the logits of the last one as (1, classes, 1)."""
         if dilation_func is not None and getattr(dilation_func, "__func__", None) is WaveNetModel.queue_dilate:
+            if getattr(self, "condition_channels", 0):
+                raise NotImplementedError("wavenet_b200: wavenet(x, queue_dilate) exists for the reference's unconditioned "
+                                          "models; sample a conditioned model with generate_fast(..., condition=)")
             return self._queue_step(input)
         n = input.size(0)
-        y = self._stack(input, None)
+        y = self._stack(input, None, condition=condition)
         return y.view(n, -1, self.classes).transpose(1, 2).contiguous()
 
     def wavenet_dilate(self, input, dilation, init_dilation, i):
@@ -1060,26 +1136,62 @@ class WaveNetModel(nn.Module):
         queue.enqueue(input.data[0])
         return queue.dequeue(num_deq=self.kernel_size, dilation=dilation).unsqueeze(0)
 
-    def _stack(self, input, out_len, index_input=False):
+    def _condition(self, condition, n):
+        """The (n, G) float32 condition rows on the model's device for ``condition`` -- an int array / tensor (n,) of
+        labels in [0, G) (one-hot rows) or a float (n, G) of dense vectors -- or None for an unconditioned model.  Raises
+        when a conditioned model gets no condition, an unconditioned one gets one, or the shape / labels are wrong."""
+        G = getattr(self, "condition_channels", 0)          # whole-model pickles made before conditioning existed lack it
+        if not G:
+            if condition is not None:
+                raise ValueError("this model has no conditioning (condition_channels=0) but a condition was given")
+            return None
+        if condition is None:
+            raise ValueError(f"this model is conditioned on {G} channels: pass condition= (labels (N,) or vectors (N, {G}))")
+        if torch.is_tensor(condition) and condition.requires_grad and torch.is_grad_enabled():
+            raise NotImplementedError("wavenet_b200: no gradient with respect to the condition (the backward computes the "
+                                      "conditioning weights' gradients only); detach it, or learn the embedding as V itself "
+                                      "by passing labels")
+        try:
+            c = condition.detach() if torch.is_tensor(condition) else torch.as_tensor(np.asarray(condition))
+        except (TypeError, ValueError, RuntimeError) as e:
+            raise ValueError(f"condition must hold int labels or float vectors: {e}") from None
+        if c.dtype.is_floating_point:
+            if tuple(c.shape) != (n, G):
+                raise ValueError(f"a dense condition must be a float ({n}, {G}) array, got shape {tuple(c.shape)}")
+            c = c.to(torch.float32)
+        elif c.dtype in (torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64):
+            if tuple(c.shape) != (n,):
+                raise ValueError(f"condition labels must be an int ({n},) array, got shape {tuple(c.shape)}")
+            c = c.to(torch.int64)
+            if n and (int(c.min()) < 0 or int(c.max()) >= G):
+                raise ValueError(f"condition labels must lie in [0, {G}), got [{int(c.min())}, {int(c.max())}]")
+            c = torch.nn.functional.one_hot(c, G).to(torch.float32)
+        else:
+            raise ValueError(f"condition must hold int labels or float vectors, got {c.dtype}")
+        return c.to(self._runtime().device()).contiguous()
+
+    def _stack(self, input, out_len, index_input=False, condition=None):
+        cond = self._condition(condition, input.size(0))
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             if input.requires_grad:
                 raise NotImplementedError("wavenet_b200: no gradient with respect to the input (it is one-hot data)")
-            return _StackFunction.apply(self, input, out_len, index_input, *self.parameters())
+            return _StackFunction.apply(self, input, out_len, index_input, cond, *self.parameters())
         rt = self._runtime()
         with torch.cuda.device(rt.device()):       # native launches go to the CURRENT device: make it the model's
-            return rt.stack_forward(input, out_len, index_input=index_input)
+            return rt.stack_forward(input, out_len, index_input=index_input, cond=cond)
 
-    def forward(self, input):
-        """(N, classes, L) -> (N * output_length, classes): logits of the last ``output_length`` frames."""
-        return self._stack(input, self.output_length)
+    def forward(self, input, condition=None):
+        """(N, classes, L) -> (N * output_length, classes): logits of the last ``output_length`` frames.
+        condition: for a conditioned model, labels (N,) or vectors (N, G) (see _condition)."""
+        return self._stack(input, self.output_length, condition=condition)
 
-    def forward_indices(self, indices):
+    def forward_indices(self, indices, condition=None):
         """Same as ``forward(one_hot(indices))`` bit for bit, from (N, L) uint8 / int64 mu-law indices:
         start_conv on a one-hot column is a gather of one weight column (SURVEY.md section 8, row a4 / f2)."""
-        return self._stack(indices, self.output_length, index_input=True)
+        return self._stack(indices, self.output_length, index_input=True, condition=condition)
 
     # ------------------------------------------------------------------ generation
-    def generate(self, num_samples, first_samples=None, temperature=1.):
+    def generate(self, num_samples, first_samples=None, temperature=1., condition=None):
         """The slow sampler (reference wavenet_model.py:198-235): every new sample re-evaluates the whole stack on a window
         of the last ``receptive_field`` samples.  The reference's own body cannot run (``self.scope`` at :209 does not exist
         and :230-235 concatenates Long and Float tensors); this restates its evident intent with the same schedule: the
@@ -1095,10 +1207,11 @@ class WaveNetModel(nn.Module):
         seq = list(first.tolist())
         rt = self._runtime()
         dev = rt.device()
+        cond = self._condition(self._one_condition(condition), 1)
         with torch.no_grad(), torch.cuda.device(dev):
             for _ in range(num_samples):
                 window = torch.tensor(seq[-rf:], dtype=torch.int64, device=dev).view(1, rf)
-                x = rt.stack_forward(window, 1, index_input=True)[0]
+                x = rt.stack_forward(window, 1, index_input=True, cond=cond)[0]
                 if temperature > 0:
                     prob = torch.softmax(x / temperature, dim=0).cpu().numpy()
                     seq.append(int(np.random.choice(self.classes, p=prob)))
@@ -1107,6 +1220,14 @@ class WaveNetModel(nn.Module):
         self.train()
         generated = (np.asarray(seq, dtype=np.float64) / self.classes) * 2. - 1
         return mu_law_expansion(generated, self.classes)
+
+    @staticmethod
+    def _one_condition(condition):
+        """The condition of ONE stream (a label, or a (G,) vector) as a batch of one: (1,) or (1, G)."""
+        if condition is None:
+            return None
+        c = condition.detach().cpu().numpy() if torch.is_tensor(condition) else np.asarray(condition)
+        return c.reshape(1) if c.ndim == 0 else (c.reshape(1, -1) if c.ndim == 1 and c.dtype.kind == "f" else c)
 
     def _first_array(self, first_samples):
         if first_samples is None:
@@ -1128,7 +1249,8 @@ class WaveNetModel(nn.Module):
                                 residual_channels=self.residual_channels, skip_channels=self.skip_channels,
                                 end_channels=self.end_conv_1.out_channels, classes=self.classes,
                                 output_length=self.output_length, kernel_size=self.kernel_size,
-                                bias=self.start_conv.bias is not None)
+                                bias=self.start_conv.bias is not None,
+                                condition_channels=getattr(self, "condition_channels", 0))
             twin.load_state_dict(self.state_dict())
             sh = (key, twin.cuda())
             self.__dict__["_shadow"] = sh
@@ -1137,23 +1259,25 @@ class WaveNetModel(nn.Module):
         return sh[1]
 
     def generate_fast(self, num_samples, first_samples=None, temperature=1., regularize=0.,
-                      progress_callback=None, progress_interval=100):
+                      progress_callback=None, progress_interval=100, condition=None):
         """Fast-WaveNet sampling; returns the mu-law expanded waveform, float64 ndarray of ``num_samples`` values.
 
         Same schedule as the reference (wavenet_model.py:237-315): the queues are reset, the given samples warm
         them up, then every step feeds the chosen sample back.  ``temperature > 0`` draws from the softmax with
         numpy's GLOBAL RNG (one ``random_sample()`` per sample, which is what ``np.random.choice`` consumes), so
         ``np.random.seed(s)`` reproduces the reference's stream; ``temperature == 0`` takes the argmax.
+        ``condition``: a conditioned model's label or (G,) vector for this stream.
         """
         if self.start_conv.weight.device.type != "cuda":
             twin = self._cuda_shadow()
             audio = twin.generate_fast(num_samples, first_samples=first_samples, temperature=temperature,
                                        regularize=regularize, progress_callback=progress_callback,
-                                       progress_interval=progress_interval)
+                                       progress_interval=progress_interval, condition=condition)
             for q, tq in zip(self.dilated_queues, twin.dilated_queues):
                 q.data, q.in_pos, q.out_pos = tq.data, tq.in_pos, tq.out_pos
             self.train()
             return audio
+        cond = self._condition(self._one_condition(condition), 1)
         self.eval()
         first = self._first_array(first_samples)
         num_given = first.shape[0]
@@ -1168,27 +1292,28 @@ class WaveNetModel(nn.Module):
                     callbacks.append((num_given - 1 + i, lambda i=i: progress_callback(i + num_given, total)))
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
-            idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks)
+            idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond)
         self._export_queues()
         self.train()
         generated = (idx[0] / self.classes) * 2. - 1
         return mu_law_expansion(generated, self.classes)
 
     def generate_fast_batch(self, num_samples, first_samples, temperature=1., regularize=0., uniforms=None,
-                            forced=None, return_logits=False):
+                            forced=None, return_logits=False, condition=None):
         """``n_streams`` independent generate_fast runs batched in one kernel (the reference has a single stream,
         wavenet_model.py:179).  first_samples: (n_streams, n_given) ints.  Returns int64 indices
         (n_streams, num_samples) [and the per-step logits].  Run through the same sampler kernel, stream s equals a
         single-stream run bit for bit (256-wide nets run the tensor-core cluster kernel for any number of streams; other
         nets a latency kernel for one stream and one thread-block cluster per stream otherwise, which differ at rounding
-        level)."""
-        self.eval()
+        level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream."""
         first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
         first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
+        cond = self._condition(condition, first.shape[0])
+        self.eval()
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, logits, _ = rt.generate(num_samples, first, temperature, regularize, uniforms=uniforms,
-                                         forced=forced, want_logits=return_logits)
+                                         forced=forced, want_logits=return_logits, cond=cond)
         self._export_queues()
         self.train()
         return (idx, logits) if return_logits else idx
@@ -1231,6 +1356,7 @@ class WaveNetModel(nn.Module):
                     or ses["sampler"] is not rt.samplers.get(1):
                 s = rt.sampler(1)
                 native.check(native.lib().wn_gen_reset(s["handle"], torch.cuda.current_stream(dev).cuda_stream), "gen reset")
+                native.check(native.lib().wn_gen_set_condition(s["handle"], None), "gen condition")
                 ses = dict(sampler=s, t=0, inp=torch.zeros(1, dtype=torch.int32, device=dev),
                            out=torch.zeros(1, dtype=torch.int32, device=dev),
                            logits=torch.zeros(self.classes, dtype=torch.float32, device=dev))

@@ -6,6 +6,8 @@ same constructor, ``train`` / ``validate`` and ``generate_audio`` -- SURVEY.md s
 * the default optimizer is ``FusedAdam`` (wn_adam_step: torch.optim.Adam's update for all tensors in one launch); any
   ``torch.optim`` class can still be passed, as in the reference;
 * items may be class INDICES (``WavenetDataset(one_hot=False)``): they go through ``model.forward_indices``;
+* items may be ``(x, condition, target)`` for a conditioned model (``WavenetDataset(condition_on_file=True)``): the
+  condition (labels or vectors, one per item) goes to the model with its batch;
 * when ``torch.distributed`` is initialised the loop is data parallel: the dataset is sharded with a DistributedSampler and
   gradients are averaged over the ranks block by block while the backward runs (data_parallel.make_data_parallel).
 The Tensorboard side of the reference's Logger (model_logging.py) is out of scope; ``Logger`` here prints.
@@ -163,11 +165,19 @@ class WavenetTrainer:
     def _device(self):
         return next(self.model.parameters()).device
 
-    def _logits(self, x):
+    def _logits(self, x, condition=None):
         dev = self._device()
         if x.dtype in (torch.uint8, torch.int64) and x.dim() == 2:
-            return self.model.forward_indices(x.to(dev, non_blocking=True))
-        return self.model(x.to(dev, torch.float32, non_blocking=True))
+            return self.model.forward_indices(x.to(dev, non_blocking=True), condition=condition)
+        return self.model(x.to(dev, torch.float32, non_blocking=True), condition=condition)
+
+    @staticmethod
+    def _unpack(batch):
+        """(x, target) or (x, condition, target) -> x, condition or None, target"""
+        if len(batch) == 3:
+            return batch[0], batch[1], batch[2]
+        x, target = batch
+        return x, None, target
 
     def _loader(self, batch_size, shuffle):
         sampler = None
@@ -188,9 +198,10 @@ class WavenetTrainer:
             if self.world > 1:
                 self.dataloader.sampler.set_epoch(current_epoch)
             tic = time.time()
-            for (x, target) in iter(self.dataloader):
+            for batch in iter(self.dataloader):
+                x, condition, target = self._unpack(batch)
                 target = target.view(-1).to(self._device(), non_blocking=True)
-                loss = fused_cross_entropy(self._logits(x), target)
+                loss = fused_cross_entropy(self._logits(x, condition), target)
                 self.optimizer.zero_grad()
                 loss.backward()
                 if self.clip is not None:
@@ -216,9 +227,10 @@ class WavenetTrainer:
         total_loss, accurate, batches = 0.0, 0, 0
         loader = self._loader(self.dataloader.batch_size if self.dataloader is not None else 32, shuffle=False)
         with torch.no_grad():
-            for (x, target) in iter(loader):
+            for batch in iter(loader):
+                x, condition, target = self._unpack(batch)
                 target = target.view(-1).to(self._device())
-                output = self._logits(x)
+                output = self._logits(x, condition)
                 total_loss += float(torch.nn.functional.cross_entropy(output, target))
                 accurate += int((output.argmax(1) == target).sum())
                 batches += 1
