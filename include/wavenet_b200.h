@@ -242,6 +242,35 @@ int wn_tb_block_fwd_cond(const wn_tb_block_args* a, const float* d_cond, void* s
 int wn_tb_stack_fwd_cond(const wn_tb_stack_args* a, const float* d_cond, void* stream);
 int wn_cond_frame_sums(const void* d_dfg, int pair, int B, int L, int C, int gz, float* d_out, void* stream);
 
+/* ---------------------------------------------------------------- (T) local conditioning
+ * A frame-rate condition series y (C channels, one frame per `hop` positions: repeat upsampling, WaveNet paper section 2.5)
+ * shifts the pre-activations of position t by Uf y[t / hop] / Ug y[t / hop]:
+ *     z[t] = tanh(Wf * x + bf + Vf h + Uf y[t / hop]) * sigmoid(Wg * x + bg + Vg h + Ug y[t / hop])
+ * so for one sequence it is a filter / gate bias that changes every hop positions.  The condition table gains a frame axis:
+ *     d_cond [n_layers][n_items][n_frames][2D] fp32        (the global table is the case n_frames = 1)
+ * wn_cond_table_frames builds it for all layers in one launch:
+ *     out[l][i][f][c] = base[l][i][c] + (sum_k U_l[c][k] * y[i][k][f])
+ * d_base is the global table [n_layers][n_items][2D] of wn_cond_table (sum_g V h + b) for a model with both kinds of
+ * conditioning, or NULL: base[l][i][c] = b_l[c] from d_ptrs (laid out as for wn_cond_table; only the bias slots are read).
+ * d_u_packed [n_layers][C][wn_n1p(D)] (16-byte aligned) holds each layer's Uf / Ug (the (D, C, 1) weights of the local 1x1
+ * convolutions) packed by wn_pack_gate_weights with R = C, k = 1 and no biases; d_y (n_items, C, y_ld) fp32 with frames
+ * contiguous: frames [0, n_frames) of each item are read.  The U term is a sequential fp32 sum from k = 0 (register-tiled SGEMM
+ * core, no TF32), the same sum wn_cond_table forms over g: U = 0 gives exactly the global table, U = V = 0 exactly the biases.
+ * The *_cond_frames entry points take ONE layer's slice [B][n_frames][2D] (wn_block_fwd_cond_frames, wn_tb_block_fwd_cond_frames)
+ * or the whole table (wn_tb_stack_fwd_cond_frames); position t of a sequence reads frame t / hop.  They require hop >= 1 and
+ * n_frames >= ceil(L / hop); the tensor-core entry points read float2 pairs and need a 16-byte aligned table, the FFMA one
+ * reads single floats.
+ * wn_cond_segment_sums is the reduction behind the gradient of U:  dU[n][k] = sum_b sum_f y[b][k][f] * d_out[b][f][n] with
+ *     d_out[b][f][n] = sum over t in [max(gz, f * hop), min(L, (f + 1) * hop)) of dfg[b][t][n]      (n < C = 2D)
+ * on both dfg layouts (pair as for wn_cond_frame_sums); deterministic (no atomics); a frame with no position >= gz gives 0. */
+int wn_cond_table_frames(const float* const* d_ptrs, const float* d_u_packed, int n_layers, int D, const float* d_base, int C,
+                         const float* d_y, int y_ld, int n_items, int n_frames, float* d_out, void* stream);
+int wn_block_fwd_cond_frames(const wn_block_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+int wn_tb_block_fwd_cond_frames(const wn_tb_block_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+int wn_tb_stack_fwd_cond_frames(const wn_tb_stack_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+int wn_cond_segment_sums(const void* d_dfg, int pair, int B, int L, int C, int gz, int hop, int n_frames, float* d_out,
+                         void* stream);
+
 /* ---------------------------------------------------------------- (T) head
  * replaces relu -> end_conv_1 -> relu -> end_conv_2 (wavenet_model.py:167-169) and forward()'s
  * slice/transpose/view (:191-196): logits (B*out_len, classes) for the LAST out_len frames only.
@@ -427,6 +456,12 @@ int wn_gen_weights_changed(wn_gen_handle* h);
  * included -- before the next wn_gen_run.  The table is read on every launch
  * and must stay alive while the handle samples with it; NULL clears it (unconditioned sampling). */
 int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond);
+/* Local conditioning of the sampler: d_cond is a table window [n_layers][n_streams][n_frames][2D] (wn_cond_table_frames) of the
+ * frames [frame0, frame0 + n_frames); evaluation t (position t: it reads sample t and predicts sample t + 1) takes row
+ * t / hop - frame0 of its stream as the filter / gate biases.  wn_gen_run returns WN_E_BADARG when an evaluation of the
+ * launch falls outside the window, so a long run is sampled window by window, each launch continuing through t0.  The same
+ * lifetime rules as wn_gen_set_condition apply; NULL clears the table, and the last wn_gen_set_condition* call wins. */
+int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond, int frame0, int n_frames, int hop);
 /* Synchronise the stream and report whether a launch aborted (a CTA waited > ~3 s for a tag): 0 = fine. */
 int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer

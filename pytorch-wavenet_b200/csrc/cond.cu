@@ -4,7 +4,11 @@
 // For one sequence b the condition h_b only adds Vf h_b / Vg h_b to the filter / gate biases, so the block kernels take a
 // table [layer][item][2D] of each item's biases bf + Vf h_b | bg + Vg h_b and read it instead of bf / bg: the epilogues do the
 // same work as unconditioned ones.  The backward's data gradients do not change (they read the saved tanh / sigmoid).
-#include "common.cuh"
+//
+// Local conditioning adds Uf y_f / Ug y_f for a frame-rate series y (repeat upsampling: frame f covers positions
+// [f * hop, (f + 1) * hop)), so the table gains a frame axis, [layer][item][frame][2D]; the global table is its n_frames = 1
+// case.  The U term is a GEMM per layer (M = items * frames, K = C, N = 2D) on the register-tiled fp32 SGEMM core.
+#include "sgemm_core.cuh"
 #include <cuda_bf16.h>
 
 namespace wn {
@@ -76,6 +80,109 @@ __global__ void __launch_bounds__(32 * FS) frame_sums_kernel(const void* __restr
     }
 }
 
+// A row m = frame t0 + m of one item of y (C, ld) fp32 (frames contiguous per channel), zero past n_frames / C.
+struct FrameLoader {
+    const float* y;
+    int C, ld, t0, nf;
+    static constexpr bool vec = false;
+    __device__ __forceinline__ float load1(int m, int kidx) const {
+        const int t = t0 + m;
+        return (kidx < C && t < nf) ? __ldg(y + (size_t)kidx * ld + t) : 0.f;
+    }
+    __device__ __forceinline__ float4 load4(int, int) const { return make_float4(0.f, 0.f, 0.f, 0.f); }
+};
+
+// out[l][i][f][c] = base[l][i][c] + (sum_k U_l[c][k] * y[i][k][f]).  base is the global table (wn_cond_table: sum_g V h + b),
+// computed once per item; without one (no global term) base[l][i][c] = b_l[c].  CTA = TMF frames of one item of one layer
+// (blockIdx.x, .y, .z); the U term is mainloop() over the layer's packed U [C][n1p(D)] (wn_pack_gate_weights, k = 1: 128-column
+// chunks of 64 filter | 64 gate channels), a sequential fp32 sum over k from 0 -- the same sum table_kernel forms over g.  So
+// U = 0 gives exactly the global table (base + 0) and U = V = 0 exactly the biases.
+constexpr int TMF = 64;
+__global__ void __launch_bounds__(NT) table_frames_kernel(const float* const* __restrict__ ptrs, const float* __restrict__ upk,
+                                                          int D, const float* __restrict__ base, int C,
+                                                          const float* __restrict__ y, int y_ld, int n_items, int n_frames,
+                                                          float* __restrict__ out) {
+    using T = Tile<TMF>;
+    __shared__ __align__(16) float As[2 * KS * TMF];
+    __shared__ __align__(16) float Bs[2 * KS * NC];
+    const int l = blockIdx.z, item = blockIdx.y, f0 = blockIdx.x * TMF;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int n1p = n1p_of(D);
+    const float* bf = ptrs[4 * l + 2];
+    const float* bg = ptrs[4 * l + 3];
+    const float* bi = base ? base + ((size_t)l * n_items + item) * 2 * D : nullptr;      // this item's global row
+    FrameLoader al;
+    al.y = y + (size_t)item * C * y_ld; al.C = C; al.ld = y_ld; al.t0 = f0; al.nf = n_frames;
+    float* o = out + ((size_t)l * n_items + item) * n_frames * 2 * D;
+    for (int ch = 0; ch < n1p / NC; ++ch) {
+        float acc[T::MI][8];
+#pragma unroll
+        for (int i = 0; i < T::MI; ++i)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+        mainloop<TMF, false>(acc, al, nullptr, upk + (size_t)l * C * n1p, n1p, ch * NC, C, As, Bs);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int c = ch * 64 + tx * 4 + q;
+            if (c >= D) continue;
+            const float b_f = bi ? __ldg(bi + c) : (bf ? __ldg(bf + c) : 0.f);
+            const float b_g = bi ? __ldg(bi + D + c) : (bg ? __ldg(bg + c) : 0.f);
+#pragma unroll
+            for (int i = 0; i < T::MI; ++i) {
+                const int f = f0 + T::row(ty, i);
+                if (f >= n_frames) continue;
+                o[(size_t)f * 2 * D + c] = acc[i][q] + b_f;
+                o[(size_t)f * 2 * D + D + c] = acc[i][4 + q] + b_g;
+            }
+        }
+    }
+}
+
+// out[b][f][c] = sum over t in [max(gz, f * hop), min(L, (f + 1) * hop)) of dfg[b][t][c]: frame_sums_kernel's block and
+// summation order over each frame's segment (blockIdx.y strides over the frames, blockIdx.z = b).  Empty segments give 0.
+template <bool PAIR>
+__global__ void __launch_bounds__(32 * FS) segment_sums_kernel(const void* __restrict__ src, int L, int C, int gz, int hop,
+                                                               int n_frames, float* __restrict__ out) {
+    __shared__ float part[FS][33];
+    const int x = threadIdx.x, y = threadIdx.y, b = blockIdx.z;
+    for (int f = blockIdx.y; f < n_frames; f += gridDim.y) {
+        const long long s0 = (long long)f * hop, s1 = s0 + hop;
+        const int lo = (int)(s0 < gz ? gz : (s0 > L ? L : s0)), hi = (int)(s1 > L ? L : s1);
+        float* o = out + ((size_t)b * n_frames + f) * C;
+        float acc = 0.f;
+        if constexpr (PAIR) {
+            const int e = x & 7, q = x >> 3, ck = blockIdx.x;
+            const __nv_bfloat16* hp = reinterpret_cast<const __nv_bfloat16*>(src) + ((size_t)b * 2 * (C / 8) + ck) * L * 8 + e;
+            const __nv_bfloat16* lp = hp + (size_t)(C / 8) * L * 8;
+            for (int t = lo + 4 * y + q; t < hi; t += 4 * FS) acc += __bfloat162float(hp[(size_t)t * 8]) + __bfloat162float(lp[(size_t)t * 8]);
+            part[y][x] = acc;
+            __syncthreads();
+            if (y == 0 && x < 8) {
+                float s = 0.f;
+                for (int k = 0; k < FS; ++k)
+#pragma unroll
+                    for (int qq = 0; qq < 4; ++qq) s += part[k][8 * qq + x];
+                o[ck * 8 + x] = s;
+            }
+        } else {
+            const int c = blockIdx.x * 32 + x;
+            if (c < C) {
+                const float* p = reinterpret_cast<const float*>(src) + (size_t)b * L * C + c;
+                for (int t = lo + y; t < hi; t += FS) acc += __ldg(p + (size_t)t * C);
+            }
+            part[y][x] = acc;
+            __syncthreads();
+            if (y == 0 && c < C) {
+                float s = part[0][x];
+#pragma unroll
+                for (int k = 1; k < FS; ++k) s += part[k][x];
+                o[c] = s;
+            }
+        }
+        __syncthreads();                                   // part[] is reused by the next frame
+    }
+}
+
 }  // namespace cond
 }  // namespace wn
 
@@ -99,6 +206,36 @@ extern "C" int wn_cond_frame_sums(const void* d_dfg, int pair, int B, int L, int
     cudaStream_t st = (cudaStream_t)stream;
     if (pair) cond::frame_sums_kernel<true><<<dim3(C / 8, B), block, 0, st>>>(d_dfg, L, C, gz, d_out);
     else cond::frame_sums_kernel<false><<<dim3((C + 31) / 32, B), block, 0, st>>>(d_dfg, L, C, gz, d_out);
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int wn_cond_table_frames(const float* const* d_ptrs, const float* d_u_packed, int n_layers, int D,
+                                    const float* d_base, int C, const float* d_y, int y_ld, int n_items, int n_frames, float* d_out,
+                                    void* stream) {
+    WN_REQUIRE(d_ptrs && d_u_packed && d_y && d_out, WN_E_BADARG, "wn_cond_table_frames: null pointer");
+    // U is read as float4 (its rows are wn_n1p(D) floats, a multiple of 4); y, base and out are read / written per float
+    WN_REQUIRE((uintptr_t)d_u_packed % 16 == 0 && ((uintptr_t)d_y | (uintptr_t)d_base | (uintptr_t)d_out) % 4 == 0, WN_E_BADARG,
+               "wn_cond_table_frames: U must be 16-byte aligned, y, the base table and the output 4-byte aligned");
+    WN_REQUIRE(n_layers > 0 && D > 0 && C > 0 && n_items > 0 && n_frames > 0 && y_ld >= n_frames && n_items <= 65535 &&
+                   n_layers <= 65535, WN_E_BADARG, "wn_cond_table_frames: bad sizes");
+    const dim3 grid((unsigned)ceil_div(n_frames, cond::TMF), (unsigned)n_items, (unsigned)n_layers);
+    cond::table_frames_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(d_ptrs, d_u_packed, D, d_base, C, d_y, y_ld, n_items,
+                                                                    n_frames, d_out);
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int wn_cond_segment_sums(const void* d_dfg, int pair, int B, int L, int C, int gz, int hop, int n_frames, float* d_out,
+                                    void* stream) {
+    WN_REQUIRE(d_dfg && d_out, WN_E_BADARG, "wn_cond_segment_sums: null pointer");
+    WN_REQUIRE(B > 0 && B <= 65535 && L > 0 && C > 0 && gz >= 0 && hop >= 1 && n_frames > 0 && (!pair || C % 8 == 0), WN_E_BADARG,
+               "wn_cond_segment_sums: bad sizes");
+    const dim3 block(32, cond::FS);
+    const unsigned gy = (unsigned)(n_frames < 65535 ? n_frames : 65535);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (pair) cond::segment_sums_kernel<true><<<dim3(C / 8, gy, B), block, 0, st>>>(d_dfg, L, C, gz, hop, n_frames, d_out);
+    else cond::segment_sums_kernel<false><<<dim3((C + 31) / 32, gy, B), block, 0, st>>>(d_dfg, L, C, gz, hop, n_frames, d_out);
     WN_CUDA(cudaGetLastError());
     return 0;
 }

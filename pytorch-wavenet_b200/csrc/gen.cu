@@ -59,7 +59,15 @@ struct GenParams {
     long long* trace;       // optional: clock64 stamps of CTA 0 / thread 0 during the last evaluation (wn_gen_read_trace)
     const unsigned char* cl8_img;              // batched cluster kernel: fragment-ordered bf16 hi/lo weight images (cl8_pack_kernel)
     const float* cond;      // optional condition table [n_layers][NS][2D]: each stream's filter / gate biases (bf + Vf h | bg + Vg h)
+    // local conditioning (cond_hop > 0): cond is a window [n_layers][NS][cond_frames][2D] of frames [cond_frame0, +cond_frames);
+    // evaluation t reads row t / cond_hop - cond_frame0.  cond_sstride = floats per stream (2D for a global table).
+    int cond_hop, cond_frame0, cond_frames, cond_sstride;
 };
+
+// This evaluation's condition table: the window row of t's frame under local conditioning (once per evaluation).
+__device__ __forceinline__ const float* cond_at(const GenParams& p, int t, int D) {
+    return p.cond_hop ? p.cond + (size_t)(t / p.cond_hop - p.cond_frame0) * 2 * D : p.cond;
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -158,6 +166,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
 
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;                           // absolute evaluation counter == time
+        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);              // sample number this evaluation chooses
         // ---- input index of this evaluation
@@ -197,14 +206,14 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
                 const float* w = ((it & 1) ? L.wg : L.wf) + (size_t)c * K1;
                 const float* bp = (it & 1) ? L.bg : L.bf;
                 const float bias = bp ? __ldg(bp + c) : 0.f;
-                const float* cb = p.cond ? p.cond + (size_t)l * NS * 2 * D + ((it & 1) ? D : 0) + c : nullptr;
+                const float* cb = ct ? ct + (size_t)l * NS * p.cond_sstride + ((it & 1) ? D : 0) + c : nullptr;
                 for (int s0 = 0; s0 < NS; s0 += SB) {
                     float acc[SB];
                     row_dot<SB>(w, regA, K1, NS, s0, lane, acc);
                     if (lane == 0) {
 #pragma unroll
                         for (int j = 0; j < SB; ++j)
-                            if (s0 + j < NS) pre[it * NS + s0 + j] = acc[j] + (cb ? __ldg(cb + (size_t)(s0 + j) * 2 * D) : bias);
+                            if (s0 + j < NS) pre[it * NS + s0 + j] = acc[j] + (cb ? __ldg(cb + (size_t)(s0 + j) * p.cond_sstride) : bias);
                     }
                 }
             }
@@ -590,6 +599,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         const int t = p.t0 + ev;
         const unsigned tag = (unsigned)t + 1u;
         const int par = t & 1;
+        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);
         if (t < p.n_given) {
@@ -632,7 +642,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
             uint2* zl = p.zLL + ((size_t)(par * NL + l) * NS) * D;
             for (int i = tid; i < nD * NS; i += GEN_NT) {
                 const int ci = i / NS, s = i - ci * NS, c = oD + ci;
-                const float* cb = p.cond ? p.cond + ((size_t)l * NS + s) * 2 * D : nullptr;     // this stream's biases
+                const float* cb = ct ? ct + ((size_t)l * NS + s) * p.cond_sstride : nullptr;     // this stream's biases
                 const float f = sum_parts(2 * ci, nw, s) + (cb ? __ldg(cb + c) : (L.bf ? __ldg(L.bf + c) : 0.f));
                 const float g = sum_parts(2 * ci + 1, nw, s) + (cb ? __ldg(cb + D + c) : (L.bg ? __ldg(L.bg + c) : 0.f));
                 st_pair(zl + (size_t)s * D + c, tanh_(f) * sigmoid_(g), tag);
@@ -1093,6 +1103,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_fast(const GenParam
         const int t = p.t0 + ev;
         const unsigned tag = (unsigned)t + 1u;
         const int par = t & 1;
+        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);
         if (tid == 0) {
@@ -1188,9 +1199,9 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_fast(const GenParam
                 const float* pf = part + stage_par * GEN_WARPS + (2 * tid) * HS1;
                 float f = pf[0], g = pf[HS1];
                 for (int q = 1; q < HS1; ++q) { f += pf[q]; g += pf[HS1 + q]; }
-                if (p.cond) {                                      // one stream: the table is [n_layers][1][2D]
-                    f += __ldg(p.cond + (size_t)l * 2 * D + c);
-                    g += __ldg(p.cond + (size_t)l * 2 * D + D + c);
+                if (ct) {                                          // one stream: the table is [n_layers][1][(frames)][2D]
+                    f += __ldg(ct + (size_t)l * p.cond_sstride + c);
+                    g += __ldg(ct + (size_t)l * p.cond_sstride + D + c);
                 } else {
                     f += L.bf ? __ldg(L.bf + c) : 0.f;
                     g += L.bg ? __ldg(L.bg + c) : 0.f;
@@ -1493,6 +1504,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;
         const unsigned rtag = (unsigned)t + 1u;                  // ring tag of time t
+        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);
         if (tid == 0) {
@@ -1574,7 +1586,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
                 for (int jj = 0; jj < CL_ROWS / 2; ++jj)
                     if (2 * jj < rw1 && ((lane >> 4) == (jj & 1))) {
                         const int ci = (warp * rw1 >> 1) + jj, c = oD + ci;
-                        const float* cb = p.cond ? p.cond + ((size_t)l * NS + stream) * 2 * D : nullptr;
+                        const float* cb = ct ? ct + ((size_t)l * NS + stream) * p.cond_sstride : nullptr;
                         const float f = acc[2 * jj] + (cb ? __ldg(cb + c) : (L.bf ? __ldg(L.bf + c) : 0.f));
                         const float g = acc[2 * jj + 1] + (cb ? __ldg(cb + D + c) : (L.bg ? __ldg(L.bg + c) : 0.f));
                         st_remote_pair(zbuf + c, (unsigned)dst, tanh_(f) * sigmoid_(g), tag_z);
@@ -1870,6 +1882,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams 
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;
         const unsigned rtag = (unsigned)t + 1u;                  // tag of time t in the L2 buffers (ring history, exchange vectors)
+        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const int par = t & 1;
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);
@@ -1952,9 +1965,9 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams 
                 const float* pf = part + stage_par * GEN_WARPS + (2 * vi) * HS1;
                 float f = pf[0], g = pf[HS1];
                 for (int q = 1; q < HS1; ++q) { f += pf[q]; g += pf[HS1 + q]; }
-                if (p.cond) {                                      // one stream: the table is [n_layers][1][2D]
-                    f += __ldg(p.cond + (size_t)l * 2 * D + c);
-                    g += __ldg(p.cond + (size_t)l * 2 * D + D + c);
+                if (ct) {                                          // one stream: the table is [n_layers][1][(frames)][2D]
+                    f += __ldg(ct + (size_t)l * p.cond_sstride + c);
+                    g += __ldg(ct + (size_t)l * p.cond_sstride + D + c);
                 } else {
                     f += L.bf ? __ldg(L.bf + c) : 0.f;
                     g += L.bg ? __ldg(L.bg + c) : 0.f;
@@ -2242,8 +2255,9 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
 // few clusters of 16 CTAs are co-resident (tools/cluster_occ.cu) but about twice as many clusters of 8: CS = 8 runs 64 streams
 // (8 clusters) in one wave on 64 SMs, at twice the per-CTA work -- the step is bound by the exchange latency, not by it.
 // COND: the filter / gate biases come from the condition table (a separate instantiation: the per-layer branch costs the
-// unconditioned single-stream kernel ~6 % of its time per sample).
-template <int CS, bool COND>
+// unconditioned single-stream kernel ~6 % of its time per sample).  FRAMES (with COND): the table is a local-conditioning
+// window, and each evaluation reads its frame's rows (a third instantiation, so the other two carry no trace of it).
+template <int CS, bool COND, bool FRAMES>
 __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
     extern __shared__ __align__(128) unsigned char smb[];
     constexpr int W = CL8_W, SB = CL8_SB, NV = 16, BLK = CL8_BLK, VEC = CL8_VEC, VR = CL / CS, NVC = NV * VR;
@@ -2539,6 +2553,9 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         const bool want_head = (t >= p.n_given - 1);
         const int samp = t - (p.n_given - 1);
         const bool tr_on = p.trace != nullptr && blockIdx.x == 0 && tid == 0 && ev == p.n_evals - 1;
+        // FRAMES: this stream's rows of evaluation t's frame; layer l's row is l * NS * cond_sstride further
+        const float* cs_t = nullptr;
+        if constexpr (FRAMES) cs_t = cond_at(p, t, W) + (size_t)fsg * p.cond_sstride;
         int tr_n = 0;
 #define TR8() do { if (tr_on && tr_n < 2040) p.trace[tr_n++] = clock64(); } while (0)
         if (tr_on) p.trace[2040] = clock64();             // whole-evaluation stamps live at [2040..2047]
@@ -2581,7 +2598,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             unsigned char* zb = Xz + (l & 1) * VEC;
             // biases of this thread's outputs: requested now, used one or two stages later
             // conditioned: the stream's own filter / gate biases, from the condition table
-            const float* cb = COND ? p.cond + ((size_t)l * NS + fsg) * 2 * W : nullptr;
+            const float* cb = FRAMES ? cs_t + (size_t)l * NS * p.cond_sstride : (COND ? p.cond + ((size_t)l * NS + fsg) * 2 * W : nullptr);
             const float b_f = COND ? ((fin_a && fs_on) ? __ldg(cb + fch) : 0.f) : ((fin_a && L.bf) ? __ldg(L.bf + fch) : 0.f);
             const float b_g = COND ? ((fin_a && fs_on) ? __ldg(cb + W + fch) : 0.f) : ((fin_a && L.bg) ? __ldg(L.bg + fch) : 0.f);
             const float b_r = (fin_a && L.br) ? __ldg(L.br + fch) : 0.f, b_s = (fin_s && L.bs) ? __ldg(L.bs + fch) : 0.f;
@@ -3142,11 +3159,11 @@ static int launch_gen_cluster(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     return 0;
 }
 
-template <int CS, bool COND>
+template <int CS, bool COND, bool FRAMES>
 static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, int* max_clusters_out, bool launch) {
     const size_t smem = (CS == 16) ? h->smem_cl8 : h->smem_cl8_8;
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * CS));
     cfg.blockDim = dim3(GEN_NT + 64 + (CS == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
@@ -3160,18 +3177,18 @@ static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, in
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND>, &cfg));
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND, FRAMES>, &cfg));
     if (max_clusters_out) *max_clusters_out = max_clusters;
     if (!launch) return 0;
     WN_REQUIRE(max_clusters >= 1, WN_E_UNSUPP, "wn_gen_run: a %d-CTA cluster cannot be scheduled on this device", CS);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND>, p));   // clusters are independent: more than fit run in waves
+    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND, FRAMES>, p));   // clusters are independent: more than fit run in waves
     return 0;
 }
 // Cluster size: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8 (15 clusters fit instead of 7).
 static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     if (h->cl8_cs == 0) {
         int fit16 = 0;
-        const int rc = launch_gen_cl8_cs<16, false>(h, p, st, &fit16, false);
+        const int rc = launch_gen_cl8_cs<16, false, false>(h, p, st, &fit16, false);
         if (rc) return rc;
         const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
         h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
@@ -3180,9 +3197,14 @@ static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
             if (v == 16 || (v == 8 && h->cl8_8_ok)) h->cl8_cs = v;
         }
     }
+    if (p.cond && p.cond_hop)
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true>(h, p, st, nullptr, true)
+                               : launch_gen_cl8_cs<8, true, true>(h, p, st, nullptr, true);
     if (p.cond)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true>(h, p, st, nullptr, true) : launch_gen_cl8_cs<8, true>(h, p, st, nullptr, true);
-    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false>(h, p, st, nullptr, true) : launch_gen_cl8_cs<8, false>(h, p, st, nullptr, true);
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false>(h, p, st, nullptr, true)
+                               : launch_gen_cl8_cs<8, true, false>(h, p, st, nullptr, true);
+    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false>(h, p, st, nullptr, true)
+                           : launch_gen_cl8_cs<8, false, false>(h, p, st, nullptr, true);
 }
 
 // 64 CTAs as 4 clusters of 16, all co-resident (the clusters exchange through the L2 while they run): launched with the
@@ -3254,6 +3276,20 @@ extern "C" int wn_gen_weights_changed(wn_gen_handle* h) {
 extern "C" int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_condition: null handle");
     h->base.cond = d_cond;
+    h->base.cond_hop = h->base.cond_frame0 = 0;
+    h->base.cond_frames = 1;
+    h->base.cond_sstride = 2 * h->shape.D;
+    return 0;
+}
+
+extern "C" int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond, int frame0, int n_frames, int hop) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_condition_frames: null handle");
+    if (d_cond == nullptr) return wn_gen_set_condition(h, nullptr);
+    WN_REQUIRE(frame0 >= 0 && n_frames >= 1 && hop >= 1, WN_E_BADARG,
+               "wn_gen_set_condition_frames: bad window (frame0 %d, %d frames, hop %d)", frame0, n_frames, hop);
+    h->base.cond = d_cond;
+    h->base.cond_hop = hop; h->base.cond_frame0 = frame0; h->base.cond_frames = n_frames;
+    h->base.cond_sstride = n_frames * 2 * h->shape.D;
     return 0;
 }
 
@@ -3278,6 +3314,12 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                a->n_given, a->n_samples);
     WN_REQUIRE(!(a->temperature > 0.f) || a->d_uniforms, WN_E_BADARG, "wn_gen_run: temperature > 0 needs d_uniforms");
     if (a->n_evals == 0) return 0;
+    if (h->base.cond && h->base.cond_hop) {
+        const int f_lo = a->t0 / h->base.cond_hop, f_hi = (a->t0 + a->n_evals - 1) / h->base.cond_hop;
+        WN_REQUIRE(f_lo >= h->base.cond_frame0 && f_hi < h->base.cond_frame0 + h->base.cond_frames, WN_E_BADARG,
+                   "wn_gen_run: evaluations [%d,%d) read frames [%d,%d], outside the condition window [%d,%d)", a->t0,
+                   a->t0 + a->n_evals, f_lo, f_hi, h->base.cond_frame0, h->base.cond_frame0 + h->base.cond_frames);
+    }
     cudaStream_t st = (cudaStream_t)stream;
     const int bars_per_eval = 2 * h->shape.n_layers + 2;
     int done = 0;

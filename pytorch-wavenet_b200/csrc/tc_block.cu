@@ -84,6 +84,7 @@ struct alignas(128) LayerDesc {
     float4* fg_save;               // optional chunked (B, 2CH/4, L, 4) fp32: tanh outputs in chunks [0,CH/4), sigmoid after
     int war_layer;                 // >= 0: every item of that earlier layer must be complete before this layer writes h_out
     const float* cond;             // conditioned launches: [B][2CH] per-sequence filter / gate biases [bf + Vf h | bg + Vg h]
+    int cond_frames, cond_hop;     // locally conditioned launches: cond is [B][cond_frames][2CH], position t reads frame t / cond_hop
 };
 static_assert(sizeof(LayerDesc) % 128 == 0, "LayerDesc array elements must keep the tensor map aligned");
 
@@ -136,8 +137,9 @@ __device__ __forceinline__ void slab_mma(float (&acc)[2][64], unsigned a, unsign
 // the global item list is layer-major and dealt round-robin to the CTA pairs, an item waits (in its producer) for the items of
 // the previous layer that wrote the frames it reads, and announces itself when its epilogues have stored -- no launch gaps and
 // no idle tail between layers.  COND: every sequence has its own filter / gate biases, read from the condition table instead of
-// bf / bg (a separate instantiation, so the unconditioned kernels carry no trace of it).
-template <typename C, bool MULTI, bool COND>
+// bf / bg (a separate instantiation, so the unconditioned kernels carry no trace of it).  FRAMES (with COND): the table has a frame
+// axis (local conditioning), and each of a thread's two rows reads its own frame's row of it.
+template <typename C, bool MULTI, bool COND, bool FRAMES>
 __global__ void __launch_bounds__(NTHREADS, 1)
 block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_constant__ CUtensorMap mapW, const BlockParams p) {
     constexpr int CH = C::CH, NST = C::NST;
@@ -243,7 +245,7 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
             // pass A reads the filter / gate biases: this item's row of the condition table under COND.  Pass B re-reads the
             // layer's residual / skip biases from the descriptor, so only one bias pointer is live across the MMAs.
             const float* bias = COND ? Ld.cond : Ld.bias;
-            const int q2b = COND ? q2 + b * 2 * CH : q2;          // this thread's column, in this item's row under COND
+            const int q2b = (COND && !FRAMES) ? q2 + b * 2 * CH : q2;   // this thread's column, in this item's row under COND
             float* fg_save = reinterpret_cast<float*>(Ld.fg_save);
             const int skip_init = Ld.skip_init;
             // ---------------- pass A + gate: z = tanh(F + bf) * sigmoid(G + bg) -> shared-memory operand image (+ optional saves)
@@ -254,15 +256,32 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
                     slab_mma<C>(acc, st + a_off, SLOT / 2, st + SLOT, sl == 0);
                     mbar_arrive(empty + s);
                 }
+                // FRAMES: the table rows of this thread's two rows' frames, derived after the n-tile's MMAs so that nothing new is
+                // live across them; rows past L (last tile) read the last frame's row
+                const float* fr[2] = {nullptr, nullptr};
+                if constexpr (FRAMES) {
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const int t = tf + r0 + 8 * r, tc = t < p.L ? t : p.L - 1;
+                        fr[r] = bias + ((size_t)b * Ld.cond_frames + tc / Ld.cond_hop) * 2 * CH + j * 128 + q2;
+                    }
+                }
 #pragma unroll
                 for (int nb = 0; nb < 16; ++nb) {
                     const int ch = j * 128 + 8 * nb + q2;                      // first of this thread's two dilation channels
                     const float* bq = COND ? bias + j * 128 + 8 * nb + q2b : bias + ch;
-                    const float2 bf = __ldg(reinterpret_cast<const float2*>(bq));
-                    const float2 bg = __ldg(reinterpret_cast<const float2*>(bq + CH));
+                    float2 bf, bg;
+                    if constexpr (!FRAMES) {
+                        bf = __ldg(reinterpret_cast<const float2*>(bq));
+                        bg = __ldg(reinterpret_cast<const float2*>(bq + CH));
+                    }
 #pragma unroll
                     for (int r = 0; r < 2; ++r) {
                         const int row = r0 + 8 * r, t = tf + row;
+                        if constexpr (FRAMES) {
+                            bf = __ldg(reinterpret_cast<const float2*>(fr[r] + 8 * nb));
+                            bg = __ldg(reinterpret_cast<const float2*>(fr[r] + 8 * nb + CH));
+                        }
                         const float f0 = tanh_fast(acc[0][4 * nb + 2 * r] + bf.x), f1 = tanh_fast(acc[0][4 * nb + 2 * r + 1] + bf.y);
                         const float g0 = sigmoid_fast(acc[1][4 * nb + 2 * r] + bg.x), g1 = sigmoid_fast(acc[1][4 * nb + 2 * r + 1] + bg.y);
                         if (fg_save != nullptr && t < p.L) {
@@ -581,7 +600,8 @@ static int launch_cfg(cudaLaunchConfig_t& cfg, int grid, size_t smem, cudaStream
 
 template <typename C>
 static int fill_layer(tb::LayerDesc& d, const void* h_in, void* h_out, const float* bias4, float* fg_save, int layer, int B, int L,
-                      int dilation, int in_start, int out_start, int skip_init, int item_base, const float* cond) {
+                      int dilation, int in_start, int out_start, int skip_init, int item_base, const float* cond,
+                      int cond_frames = 0, int cond_hop = 0) {
     memset(&d, 0, sizeof(d));
     if (int rc = tb::make_pair_map(&d.mapH, h_in, B, L, C::CH, in_start, tb::BM, C::KC, C::PLANES)) return rc;
     d.t_begin = out_start; d.in_start = in_start; d.dil = dilation; d.skip_init = skip_init;
@@ -592,42 +612,57 @@ static int fill_layer(tb::LayerDesc& d, const void* h_in, void* h_out, const flo
     d.bias = bias4; d.h_in = (const uint4*)h_in; d.h_out = (uint4*)h_out; d.fg_save = (float4*)fg_save;
     d.war_layer = -1;
     d.cond = cond;
+    d.cond_frames = cond_frames; d.cond_hop = cond_hop;
     return 0;
 }
 
-template <typename C, bool COND>
-static int launch_block(const wn_tb_block_args* a, const float* cond, cudaStream_t st) {
+template <typename C, bool COND, bool FRAMES>
+static int launch_block(const wn_tb_block_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
     int dev = 0, sms = 0;
     WN_CUDA(cudaGetDevice(&dev));
     WN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     tb::LayerDesc d;
     CUtensorMap mW;
     if (int rc = fill_layer<C>(d, a->d_h_in, a->d_h_out, a->d_bias4, a->d_fg_save, a->layer, a->B, a->L, a->dilation, a->in_start,
-                               a->out_start, a->skip_init, 0, cond)) return rc;
+                               a->out_start, a->skip_init, 0, cond, n_frames, hop)) return rc;
     if (int rc = tb::make_wrows_map(&mW, a->d_w_all, (long long)a->n_layers * C::WROWS_LAYER)) return rc;
     tb::BlockParams p;
     memset(&p, 0, sizeof(p));
     p.B = a->B; p.L = a->L; p.skip_start = a->skip_start; p.n_layers = 1; p.total_items = d.n_items;
     p.skip = (float4*)a->d_skip;
-    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, false, COND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, false, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
     int grid = 2 * p.total_items;
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
     launch_cfg(cfg, grid, C::SMEM_BYTES, st);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, false, COND>, d, mW, p));
+    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, false, COND, FRAMES>, d, mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;
 }
 
 template <typename C>
-static int launch_block_c(const wn_tb_block_args* a, const float* cond, cudaStream_t st) {
-    return cond ? launch_block<C, true>(a, cond, st) : launch_block<C, false>(a, nullptr, st);
+static int launch_block_c(const wn_tb_block_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
+    if (cond && hop > 0) return launch_block<C, true, true>(a, cond, n_frames, hop, st);
+    return cond ? launch_block<C, true, false>(a, cond, 0, 0, st) : launch_block<C, false, false>(a, nullptr, 0, 0, st);
 }
 
 extern "C" int wn_tb_block_fwd(const wn_tb_block_args* a, void* stream) { return wn_tb_block_fwd_cond(a, nullptr, stream); }
 
+static int tb_block_fwd_impl(const wn_tb_block_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+
 extern "C" int wn_tb_block_fwd_cond(const wn_tb_block_args* a, const float* d_cond, void* stream) {
+    return tb_block_fwd_impl(a, d_cond, 0, 0, stream);
+}
+
+extern "C" int wn_tb_block_fwd_cond_frames(const wn_tb_block_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
+    WN_REQUIRE(a && d_cond, WN_E_BADARG, "wn_tb_block_fwd_cond_frames: null pointer");
+    WN_REQUIRE(hop >= 1 && a->L > 0 && n_frames >= ceil_div(a->L, hop), WN_E_BADARG,
+               "wn_tb_block_fwd_cond_frames: %d frames of hop %d do not cover %d positions", n_frames, hop, a->L);
+    return tb_block_fwd_impl(a, d_cond, n_frames, hop, stream);
+}
+
+static int tb_block_fwd_impl(const wn_tb_block_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
     WN_REQUIRE(a, WN_E_BADARG, "wn_tb_block_fwd: null args");
     WN_REQUIRE(a->d_h_in && a->d_h_out && a->d_skip && a->d_w_all && a->d_bias4, WN_E_BADARG, "wn_tb_block_fwd: null pointer");
     WN_REQUIRE(wn_tb_precision_supported(a->channels, a->precision), WN_E_UNSUPP, "wn_tb_block_fwd: %d channels with precision %d is not supported",
@@ -638,9 +673,9 @@ extern "C" int wn_tb_block_fwd_cond(const wn_tb_block_args* a, const float* d_co
     WN_REQUIRE(((uintptr_t)a->d_h_in | (uintptr_t)a->d_h_out | (uintptr_t)a->d_skip | (uintptr_t)a->d_w_all | (uintptr_t)d_cond) % 16 == 0,
                WN_E_BADARG, "wn_tb_block_fwd: buffers must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
-    if (a->precision == WN_PREC_BF16_PAIRS) return launch_block_c<tb::Cfg<256, true>>(a, d_cond, st);
-    if (a->channels == 256) return launch_block_c<tb::Cfg<256, false>>(a, d_cond, st);
-    return launch_block_c<tb::Cfg<512, false>>(a, d_cond, st);
+    if (a->precision == WN_PREC_BF16_PAIRS) return launch_block_c<tb::Cfg<256, true>>(a, d_cond, n_frames, hop, st);
+    if (a->channels == 256) return launch_block_c<tb::Cfg<256, false>>(a, d_cond, n_frames, hop, st);
+    return launch_block_c<tb::Cfg<512, false>>(a, d_cond, n_frames, hop, st);
 }
 
 // ---------------------------------------------------------------------------------------------- the whole stack in one launch
@@ -651,8 +686,8 @@ extern "C" long long wn_tb_stack_items(int n_layers, int B, int L, const int* ou
     return n;
 }
 
-template <typename C, bool COND>
-static int launch_stack(const wn_tb_stack_args* a, const float* cond, cudaStream_t st) {
+template <typename C, bool COND, bool FRAMES>
+static int launch_stack(const wn_tb_stack_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
     int dev = 0, sms = 0;
     WN_CUDA(cudaGetDevice(&dev));
     WN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -663,7 +698,8 @@ static int launch_stack(const wn_tb_stack_args* a, const float* cond, cudaStream
         float* fg = a->d_fg_all ? a->d_fg_all + (size_t)i * a->B * (2 * C::CH) * a->L : nullptr;
         if (int rc = fill_layer<C>(desc[i], a->h_ptrs[i], const_cast<void*>(a->h_ptrs[i + 1]), a->d_bias_all + (size_t)i * 4 * C::CH, fg, i, a->B, a->L,
                                    a->dilations[i], a->in_start[i], a->out_start[i], i == 0, base,
-                                   COND ? cond + (size_t)i * a->B * 2 * C::CH : nullptr)) return rc;
+                                   COND ? cond + (size_t)i * a->B * (FRAMES ? n_frames : 1) * 2 * C::CH : nullptr,
+                                   n_frames, hop)) return rc;
         WN_REQUIRE(a->in_start[i] >= 0 && a->out_start[i] >= a->in_start[i] && a->out_start[i] < a->L && a->skip_start >= a->out_start[i],
                    WN_E_BADARG, "wn_tb_stack_fwd: bad frame ranges of layer %d", i);
         WN_REQUIRE(a->h_ptrs[i] && a->h_ptrs[i + 1] && a->h_ptrs[i] != a->h_ptrs[i + 1] && (uintptr_t)a->h_ptrs[i + 1] % 16 == 0,
@@ -685,26 +721,40 @@ static int launch_stack(const wn_tb_stack_args* a, const float* cond, cudaStream
     p.skip = (float4*)a->d_skip;
     p.layers = (const tb::LayerDesc*)a->d_desc;
     p.item_done = a->d_flags; p.layer_done = a->d_flags + base;
-    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, true, COND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, true, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
     // every CTA must be resident (items wait for items of other CTAs): one CTA per SM, at most sms/2 pairs
     int grid = 2 * base;
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
     launch_cfg(cfg, grid, C::SMEM_BYTES, st);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, true, COND>, desc[0], mW, p));
+    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, true, COND, FRAMES>, desc[0], mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;
 }
 
 template <typename C>
-static int launch_stack_c(const wn_tb_stack_args* a, const float* cond, cudaStream_t st) {
-    return cond ? launch_stack<C, true>(a, cond, st) : launch_stack<C, false>(a, nullptr, st);
+static int launch_stack_c(const wn_tb_stack_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
+    if (cond && hop > 0) return launch_stack<C, true, true>(a, cond, n_frames, hop, st);
+    return cond ? launch_stack<C, true, false>(a, cond, 0, 0, st) : launch_stack<C, false, false>(a, nullptr, 0, 0, st);
 }
 
 extern "C" int wn_tb_stack_fwd(const wn_tb_stack_args* a, void* stream) { return wn_tb_stack_fwd_cond(a, nullptr, stream); }
 
+static int tb_stack_fwd_impl(const wn_tb_stack_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+
 extern "C" int wn_tb_stack_fwd_cond(const wn_tb_stack_args* a, const float* d_cond, void* stream) {
+    return tb_stack_fwd_impl(a, d_cond, 0, 0, stream);
+}
+
+extern "C" int wn_tb_stack_fwd_cond_frames(const wn_tb_stack_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
+    WN_REQUIRE(a && d_cond, WN_E_BADARG, "wn_tb_stack_fwd_cond_frames: null pointer");
+    WN_REQUIRE(hop >= 1 && a->L > 0 && n_frames >= ceil_div(a->L, hop), WN_E_BADARG,
+               "wn_tb_stack_fwd_cond_frames: %d frames of hop %d do not cover %d positions", n_frames, hop, a->L);
+    return tb_stack_fwd_impl(a, d_cond, n_frames, hop, stream);
+}
+
+static int tb_stack_fwd_impl(const wn_tb_stack_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
     WN_REQUIRE(a, WN_E_BADARG, "wn_tb_stack_fwd: null args");
     WN_REQUIRE(a->h_ptrs && a->d_skip && a->d_w_all && a->d_bias_all && a->d_desc && a->d_flags && a->dilations && a->in_start && a->out_start,
                WN_E_BADARG, "wn_tb_stack_fwd: null pointer");
@@ -714,7 +764,7 @@ extern "C" int wn_tb_stack_fwd_cond(const wn_tb_stack_args* a, const float* d_co
                WN_E_BADARG, "wn_tb_stack_fwd: bad sizes (d_desc must be 128-byte aligned)");
     WN_REQUIRE((uintptr_t)d_cond % 16 == 0, WN_E_BADARG, "wn_tb_stack_fwd: the condition table must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
-    if (a->precision == WN_PREC_BF16_PAIRS) return launch_stack_c<tb::Cfg<256, true>>(a, d_cond, st);
-    if (a->channels == 256) return launch_stack_c<tb::Cfg<256, false>>(a, d_cond, st);
-    return launch_stack_c<tb::Cfg<512, false>>(a, d_cond, st);
+    if (a->precision == WN_PREC_BF16_PAIRS) return launch_stack_c<tb::Cfg<256, true>>(a, d_cond, n_frames, hop, st);
+    if (a->channels == 256) return launch_stack_c<tb::Cfg<256, false>>(a, d_cond, n_frames, hop, st);
+    return launch_stack_c<tb::Cfg<512, false>>(a, d_cond, n_frames, hop, st);
 }

@@ -69,6 +69,7 @@ struct BlockParams {
     int N1p, N2p, Kz;       // Kz = z channels incl. padding = N1p/2
     float* fg_save;         // optional (B,L,2D): tanh / sigmoid outputs for the backward
     const float* cond;      // optional (B,2D): per-sequence filter / gate biases [bf + Vf h | bg + Vg h], used instead of bfg
+    int cond_frames, cond_hop;   // cond_hop > 0: cond is (B, cond_frames, 2D), frame t / cond_hop holds frame t's biases
 };
 
 template <int TM>
@@ -103,6 +104,27 @@ __global__ void __launch_bounds__(NT, 1) block_fwd_kernel(const BlockParams p) {
         const float4 bf4 = __ldg(reinterpret_cast<const float4*>(p.bfg + ch * NC + tx * 4));
         const float4 bg4 = __ldg(reinterpret_cast<const float4*>(p.bfg + ch * NC + 64 + tx * 4));
         float bfv[4] = {bf4.x, bf4.y, bf4.z, bf4.w}, bgv[4] = {bg4.x, bg4.y, bg4.z, bg4.w};
+        if (p.cond != nullptr && p.cond_hop > 0) {                 // locally conditioned: every frame's own biases
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                float* zrow = Zs + (size_t)(ch * 64 + tx * 4 + q) * (TM + ZPAD);
+                const int c = ch * 64 + tx * 4 + q;
+#pragma unroll
+                for (int i = 0; i < MI; ++i) {
+                    const int t = t0 + T::row(ty, i), tc = t < p.L ? t : p.L - 1;     // rows past L read the last frame
+                    const float* cb = p.cond + ((size_t)b * p.cond_frames + tc / p.cond_hop) * 2 * p.D;
+                    const float f = tanhf(acc[i][q] + (c < p.D ? __ldg(cb + c) : 0.f));
+                    const float g = sigmoidf_(acc[i][4 + q] + (c < p.D ? __ldg(cb + p.D + c) : 0.f));
+                    zrow[T::row(ty, i)] = f * g;
+                    if (p.fg_save != nullptr && t < p.L && c < p.D) {
+                        float* dst = p.fg_save + ((size_t)b * p.L + t) * (2 * p.D);
+                        dst[c] = f;
+                        dst[p.D + c] = g;
+                    }
+                }
+            }
+            continue;
+        }
         if (p.cond != nullptr) {                                   // conditioned: this sequence's own biases
             const float* cb = p.cond + (size_t)b * 2 * p.D;
 #pragma unroll
@@ -447,7 +469,21 @@ extern "C" int wn_start_fwd_index_i64(const int64_t* d_idx, const float* d_w_t, 
 
 extern "C" int wn_block_fwd(const wn_block_args* a, void* stream) { return wn_block_fwd_cond(a, nullptr, stream); }
 
+static int block_fwd_impl(const wn_block_args* a, const float* d_cond, int n_frames, int hop, void* stream);
+
 extern "C" int wn_block_fwd_cond(const wn_block_args* a, const float* d_cond, void* stream) {
+    return block_fwd_impl(a, d_cond, 0, 0, stream);
+}
+
+extern "C" int wn_block_fwd_cond_frames(const wn_block_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
+    WN_REQUIRE(a && d_cond, WN_E_BADARG, "wn_block_fwd_cond_frames: null pointer");
+    WN_REQUIRE(hop >= 1 && a->L > 0 && n_frames >= ceil_div(a->L, hop), WN_E_BADARG,
+               "wn_block_fwd_cond_frames: %d frames of hop %d do not cover %d positions", n_frames, hop, a->L);
+    WN_REQUIRE((uintptr_t)d_cond % 4 == 0, WN_E_BADARG, "wn_block_fwd_cond_frames: the condition table must be 4-byte aligned");
+    return block_fwd_impl(a, d_cond, n_frames, hop, stream);
+}
+
+static int block_fwd_impl(const wn_block_args* a, const float* d_cond, int n_frames, int hop, void* stream) {
     WN_REQUIRE(a, WN_E_BADARG, "wn_block_fwd: null args");
     WN_REQUIRE(a->d_h_in && a->d_h_out && a->d_skip && a->d_wfg_t && a->d_bfg && a->d_wrs_t && a->d_brs, WN_E_BADARG,
                "wn_block_fwd: null pointer");
@@ -467,6 +503,7 @@ extern "C" int wn_block_fwd_cond(const wn_block_args* a, const float* d_cond, vo
     p.N1p = n1p_of(a->D); p.N2p = n2p_of(a->R + a->S); p.Kz = p.N1p / 2;
     p.fg_save = a->d_fg_save;
     p.cond = d_cond;
+    p.cond_frames = n_frames; p.cond_hop = hop;
     const int tm = pick_tm(p.Kz, smem_limit_bytes());
     WN_REQUIRE(tm > 0, WN_E_UNSUPP, "wn_block_fwd: dilation_channels=%d does not fit shared memory", a->D);
     const size_t smem = two_phase_smem(tm, p.Kz);

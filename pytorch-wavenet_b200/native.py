@@ -164,6 +164,12 @@ SIGNATURES = {
     "wn_tb_block_fwd_cond": (C.c_int, [C.POINTER(TbBlockArgs), C.c_void_p, C.c_void_p]),
     "wn_tb_stack_fwd_cond": (C.c_int, [C.POINTER(TbStackArgs), C.c_void_p, C.c_void_p]),
     "wn_cond_frame_sums": (C.c_int, [C.c_void_p] + [C.c_int] * 5 + [C.c_void_p] * 2),
+    "wn_cond_table_frames": (C.c_int, [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_void_p, C.c_int, C.c_void_p] + [C.c_int] * 3
+                             + [C.c_void_p] * 2),
+    "wn_block_fwd_cond_frames": (C.c_int, [C.POINTER(BlockArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "wn_tb_block_fwd_cond_frames": (C.c_int, [C.POINTER(TbBlockArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "wn_tb_stack_fwd_cond_frames": (C.c_int, [C.POINTER(TbStackArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "wn_cond_segment_sums": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p] * 2),
     "wn_wgrad_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "wn_wgrad": (C.c_int, [C.POINTER(WgradArgs), C.c_void_p]),
     "wn_tc_wgrad_supported": (C.c_int, [C.c_int, C.c_int]),
@@ -191,6 +197,7 @@ SIGNATURES = {
     "wn_gen_set_mode": (C.c_int, [C.c_void_p, C.c_int]),
     "wn_gen_weights_changed": (C.c_int, [C.c_void_p]),
     "wn_gen_set_condition": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "wn_gen_set_condition_frames": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3),
     "wn_gen_kernel_id": (C.c_int, [C.c_void_p]),
     "wn_gen_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_read_trace": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_void_p]),

@@ -171,6 +171,40 @@ class _Packs:
                                        stream), "condition table")
         return out
 
+    def _build_local_u(self, stream):
+        """Every layer's local-conditioning weights Uf | Ug, packed [n_layers][C][wn_n1p(D)] for wn_cond_table_frames."""
+        rt, lib, m = self.rt, native.lib(), self.rt.model
+        nl, D, C = m.layers * m.blocks, m.dilation_channels, m.local_condition_channels
+        n1p = lib.wn_n1p(D)
+        out = torch.empty(nl, C, n1p, device=rt.device(), dtype=torch.float32)
+        bias = torch.empty(n1p, device=rt.device(), dtype=torch.float32)
+        for i in range(nl):
+            native.check(lib.wn_pack_gate_weights(m.filter_local_convs[i].weight.data_ptr(), m.gate_local_convs[i].weight.data_ptr(),
+                                                  None, None, C, D, 1, out[i].data_ptr(), bias.data_ptr(), stream), "pack local U")
+        return out
+
+    def cond_table_frames(self, h, y, f0, n_frames, stream):
+        """Condition table [n_layers][N][n_frames][2D] of a locally conditioned model (wn_cond_table_frames) for frames
+        [f0, f0 + n_frames) of the (N, C, F) fp32 series ``y``, with the (N, G) condition rows ``h`` of a globally conditioned
+        one (else None): bf + Vf h + Uf y_f | bg + Vg h + Ug y_f for every item and frame.  The global part is the global
+        table (cond_table), built once per item."""
+        rt, lib, m = self.rt, native.lib(), self.rt.model
+        nl, D = m.layers * m.blocks, m.dilation_channels
+        P = rt._params()
+        base = None if h is None else self.cond_table(h, stream)
+        rows = [[0, 0, native.ptr(P["filt"][i][1]) or 0, native.ptr(P["gate"][i][1]) or 0] for i in range(nl)]
+        key = tuple(map(tuple, rows))
+        cached = rt.__dict__.get("_lcond_ptr_cache")
+        if cached is None or cached[0] != key:
+            cached = (key, torch.tensor(rows, dtype=torch.int64, device=rt.device()))
+            rt._lcond_ptr_cache = cached
+        N, C, F = y.shape
+        out = torch.empty(nl, N, n_frames, 2 * D, device=rt.device(), dtype=torch.float32)
+        native.check(lib.wn_cond_table_frames(cached[1].data_ptr(), self["local_u"].data_ptr(), nl, D, native.ptr(base), C,
+                                              y.data_ptr() + 4 * f0, F, N, n_frames, out.data_ptr(), stream),
+                     "local condition table")
+        return out
+
     def _build_tb(self, stream):
         rt, lib = self.rt, native.lib()
         R, nl = self._dims()[0], self._dims()[6]
@@ -233,6 +267,7 @@ class _Runtime:
         self.fast_tf32 = False       # opt-in single-pass TF32 blocks (~1e-3 on the logits: outside the parity bar)
         self.tc_precision = "bf16x2"  # tensor-core operand split: "tf32x3" (3xTF32) or "bf16x2" (bf16 pairs, 2x the MMA rate)
         self.wgrad_mode = "tc"        # weight gradients: "tc" (tensor cores where the shape allows), "native" (fp32 FMA), "cublas"
+        self.local_table_bytes = 256 << 20   # sampler: largest local-conditioning table window (at least one frame is built)
 
     # ------------------------------------------------------------------ weights
     def _params(self):
@@ -291,11 +326,12 @@ class _Runtime:
         return self.packed
 
     # ------------------------------------------------------------------ training-path forward
-    def stack_forward(self, x, out_len, index_input=False, save=None, cond=None):
+    def stack_forward(self, x, out_len, index_input=False, save=None, cond=None, local=None):
         """x: (B, classes, L) float32 one-hot/dense, or (B, L) uint8/int64 indices when index_input.
         Returns logits (B*out_len, classes) for the last out_len frames (out_len=None: all T_final frames).
         save: optional dict; filled with what the backward needs (every layer's input, tanh/sigmoid outputs, skip).
-        cond: the (B, G) fp32 condition rows of a conditioned model (WaveNetModel._condition), else None."""
+        cond: the (B, G) fp32 condition rows of a conditioned model (WaveNetModel._condition), else None.
+        local: (y, hop) of a locally conditioned model, y the (B, C, F) fp32 series (WaveNetModel._local_condition), else None."""
         m, lib = self.model, native.lib()
         dev = self.device()
         if x.device != dev:
@@ -333,18 +369,28 @@ class _Runtime:
         if self.block_mode == "tb" and not use_tb:
             raise RuntimeError("wavenet_b200: the fused tensor-core block needs R = D = S in (256, 512), kernel_size = 2 "
                                f"(got {R},{D},{S},{k})")
-        ctab = None
-        if cond is not None:
+        ctab, frames = None, None
+        if cond is not None or local is not None:
             if self.block_mode == "tc" or (self.fast_tf32 and not use_tb):
                 raise RuntimeError("wavenet_b200: a conditioned model runs on the fused tensor-core blocks (block_mode 'tb' / "
                                    "'auto') or the FFMA blocks ('ffma'); the two-launch 'tc' blocks have no conditioned kernel")
-            if cond.shape[0] != B:
+            if cond is not None and cond.shape[0] != B:
                 raise RuntimeError(f"wavenet_b200: {cond.shape[0]} condition rows for a batch of {B}")
-            ctab = W.cond_table(cond, stream)
+            if local is None:
+                ctab = W.cond_table(cond, stream)
+            else:
+                y, hop = local
+                if y.shape[0] != B or y.shape[2] < -(-L // hop):
+                    raise RuntimeError(f"wavenet_b200: a local condition of shape {tuple(y.shape)} does not cover a batch of {B} "
+                                       f"x {L} positions at hop {hop}")
+                frames = (-(-L // hop), hop)          # the table holds the frames the L positions read
+                ctab = W.cond_table_frames(cond, y, 0, frames[0], stream)
             if save is not None:
                 save["cond"] = cond
+                if local is not None:
+                    save["local"] = local
         if use_tb:
-            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save, ctab)
+            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save, ctab, frames)
         if save is not None:
             h_all = torch.empty(n_layers + 1, B, L, R, **f32)      # h_all[i] = input of layer i
             fg_all = torch.empty(n_layers, B, L, 2 * D, **f32)     # tanh / sigmoid outputs
@@ -399,6 +445,9 @@ class _Runtime:
                 a.d_wfg_t, a.d_bfg, a.d_wrs_t, a.d_brs = wfg.data_ptr(), bfg.data_ptr(), wrs.data_ptr(), brs.data_ptr()
                 if ctab is None:
                     native.check(lib.wn_block_fwd(ctypes.byref(a), stream), f"block {i}")
+                elif frames is not None:
+                    native.check(lib.wn_block_fwd_cond_frames(ctypes.byref(a), ctab[i].data_ptr(), frames[0], frames[1], stream),
+                                 f"block {i}")
                 else:
                     native.check(lib.wn_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream), f"block {i}")
             if save is None:
@@ -420,7 +469,7 @@ class _Runtime:
                         index_input=index_input, B=B, L=L)
         return logits
 
-    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None, ctab=None):
+    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None, ctab=None, frames=None):
         """Forward on the fused tensor-core blocks (wn_tb_block_fwd): chunked bf16-pair activations, one launch per residual
         block, z resident on the SM (csrc/tc_block.cu).  With ``save`` every layer's input pair and tanh/sigmoid outputs are
         kept for _backward_tb."""
@@ -480,6 +529,9 @@ class _Runtime:
             sa.dilations, sa.in_start, sa.out_start = ints(dil), ints(plan.in_start), outs
             if ctab is None:
                 native.check(lib.wn_tb_stack_fwd(ctypes.byref(sa), stream), "tb stack")
+            elif frames is not None:
+                native.check(lib.wn_tb_stack_fwd_cond_frames(ctypes.byref(sa), ctab.data_ptr(), frames[0], frames[1], stream),
+                             "tb stack")
             else:
                 native.check(lib.wn_tb_stack_fwd_cond(ctypes.byref(sa), ctab.data_ptr(), stream), "tb stack")
             n_block_launches = 1
@@ -496,6 +548,9 @@ class _Runtime:
                     a.d_fg_save = fg_all[i].data_ptr()
                 if ctab is None:
                     native.check(lib.wn_tb_block_fwd(ctypes.byref(a), stream), f"tb block {i}")
+                elif frames is not None:
+                    native.check(lib.wn_tb_block_fwd_cond_frames(ctypes.byref(a), ctab[i].data_ptr(), frames[0], frames[1], stream),
+                                 f"tb block {i}")
                 else:
                     native.check(lib.wn_tb_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream), f"tb block {i}")
                 if save is None:
@@ -641,7 +696,8 @@ class _Runtime:
             if bf is not None:
                 bsum = dfg[:, :, :, gz:, :].float().sum((0, 1, 3)).reshape(2 * D)
                 grads[f"filter_convs.{i}.bias"], grads[f"gate_convs.{i}.bias"] = bsum[:D].clone(), bsum[D:].clone()
-            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 1, gz, stream)
+            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 1, gz, stream) + \
+                self.local_weight_grads(saved, grads, i, dfg, 1, gz, stream)
             if reducer is not None:
                 reducer.reduce_flat_async(bucket)
                 reducer.reduce_async(cgrads)
@@ -681,6 +737,30 @@ class _Runtime:
         dv = torch.einsum("bn,bg->ng", sums, h)
         gf, gg = dv[:D].unsqueeze(-1).contiguous(), dv[D:].unsqueeze(-1).contiguous()
         grads[f"filter_cond_convs.{i}.weight"], grads[f"gate_cond_convs.{i}.weight"] = gf, gg
+        return [gf, gg]
+
+    def local_weight_grads(self, saved, grads, i, dfg, pair, gz, stream):
+        """Gradients of layer i's local-conditioning weights, dU[n][k] = sum_b sum_f y[b][k][f] * S[b][f][n] with S the
+        per-frame sums of dfg over the positions >= gz (wn_cond_segment_sums), and this layer's share of the gradient of the
+        series, dy[b][k][f] += sum_n S[b][f][n] * U[n][k] (kept in saved["local_dy"]; layers add in a fixed order, last to
+        first).  Returns [dUf, dUg], or [] when the model is not locally conditioned."""
+        local = saved.get("local")
+        if local is None:
+            return []
+        y, hop = local
+        m = self.model
+        B, L, D = saved["B"], saved["L"], m.dilation_channels
+        nf = -(-L // hop)
+        S = torch.empty(B, nf, 2 * D, device=y.device, dtype=torch.float32)
+        native.check(native.lib().wn_cond_segment_sums(dfg.data_ptr(), pair, B, L, 2 * D, gz, hop, nf, S.data_ptr(), stream),
+                     "condition segment sums")
+        yf = y[:, :, :nf]
+        du = torch.einsum("bfn,bkf->nk", S, yf)
+        gf, gg = du[:D].unsqueeze(-1).contiguous(), du[D:].unsqueeze(-1).contiguous()
+        grads[f"filter_local_convs.{i}.weight"], grads[f"gate_local_convs.{i}.weight"] = gf, gg
+        if "local_dy" in saved:
+            U = torch.cat([m.filter_local_convs[i].weight.detach(), m.gate_local_convs[i].weight.detach()], 0)[:, :, 0]
+            saved["local_dy"][:, :, :nf] += torch.einsum("bfn,nk->bkf", S, U)
         return [gf, gg]
 
     # ------------------------------------------------------------------ training-path backward
@@ -857,7 +937,8 @@ class _Runtime:
             if bf is not None:
                 bsum = dfg[:, gz:, :].sum((0, 1))
                 grads[f"filter_convs.{i}.bias"], grads[f"gate_convs.{i}.bias"] = bsum[:D].clone(), bsum[D:].clone()
-            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 0, gz, stream)
+            cgrads = self.cond_weight_grads(saved, grads, i, dfg, 0, gz, stream) + \
+                self.local_weight_grads(saved, grads, i, dfg, 0, gz, stream)
             if reducer is not None:
                 reducer.reduce_async([grads.get(f"{n}.{i}.{wb}") for n in ("filter_convs", "gate_convs", "residual_convs",
                                                                          "skip_convs") for wb in ("weight", "bias")] + cgrads)
@@ -943,10 +1024,12 @@ class _Runtime:
         return t0 + args.n_evals
 
     def generate(self, num_samples, first, temperature, regularize, uniforms=None, forced=None,
-                 want_logits=False, callbacks=None, cond=None):
+                 want_logits=False, callbacks=None, cond=None, local=None):
         """first: (NS, n_given) int array.  Returns (indices (NS, num_samples) int64 ndarray, logits or None, t_end).
         callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done.
-        cond: the (NS, G) fp32 condition rows of a conditioned model, else None."""
+        cond: the (NS, G) fp32 condition rows of a conditioned model, else None.
+        local: (y, hop) of a locally conditioned model, y the (NS, C, F) fp32 series, else None.  The condition table is
+        built window by window (at most ``local_table_bytes`` each), and launches are split at the window boundaries."""
         m = self.model
         dev = self.device()
         self.step_session = None             # a generate_fast run restarts the device queues (wavenet_model.py:250)
@@ -955,10 +1038,11 @@ class _Runtime:
         if n_given < 1:
             raise RuntimeError("first_samples must hold at least one sample")
         s = self.sampler(NS)
+        stream = torch.cuda.current_stream(dev).cuda_stream
         # the condition table is read by every launch of this run: the sampler entry keeps it alive
-        s["cond"] = None if cond is None else self.packed_weights(torch.cuda.current_stream(dev).cuda_stream).cond_table(
-            cond, torch.cuda.current_stream(dev).cuda_stream)
-        native.check(native.lib().wn_gen_set_condition(s["handle"], native.ptr(s["cond"])), "gen condition")
+        if local is None:
+            s["cond"] = None if cond is None else self.packed_weights(stream).cond_table(cond, stream)
+            native.check(native.lib().wn_gen_set_condition(s["handle"], native.ptr(s["cond"])), "gen condition")
         d_first = torch.from_numpy(first).to(dev, non_blocking=True)
         d_out = torch.zeros(NS, max(num_samples, 1), device=dev, dtype=torch.int32)
         d_uni = d_forced = d_logits = None
@@ -975,18 +1059,43 @@ class _Runtime:
             d_logits = torch.zeros(NS, max(num_samples, 1), m.classes, device=dev, dtype=torch.float32)
         total_evals = n_given - 1 + num_samples
         common = dict(d_uni=d_uni, d_forced=d_forced, d_logits=d_logits)
+        window = [None]                       # (first frame, frames) of the local-conditioning table the handle holds
+
+        def launch(t, n, reset):
+            """evaluations [t, t + n); under local conditioning split at the table windows' boundaries"""
+            if local is None or n <= 0:
+                return self.generate_resident(s, d_first, n_given, num_samples, temperature, regularize, d_out,
+                                              t0=t, n_evals=max(n, 0), reset=reset, **common)
+            y, hop = local
+            m = self.model
+            per_frame = m.layers * m.blocks * NS * 2 * m.dilation_channels * 4
+            max_frames = max(1, self.local_table_bytes // per_frame)
+            end = t + n
+            while t < end:
+                f = t // hop
+                if window[0] is None or not window[0][0] <= f < window[0][0] + window[0][1]:
+                    nf = min(max_frames, -(-total_evals // hop) - f)
+                    s["cond"] = None          # the previous window's launches are ordered before this stream's new work
+                    s["cond"] = self.packed_weights(stream).cond_table_frames(cond, y, f, nf, stream)
+                    native.check(native.lib().wn_gen_set_condition_frames(s["handle"], s["cond"].data_ptr(), f, nf, hop),
+                                 "gen local condition")
+                    window[0] = (f, nf)
+                stop = min(end, (window[0][0] + window[0][1]) * hop)
+                t = self.generate_resident(s, d_first, n_given, num_samples, temperature, regularize, d_out,
+                                           t0=t, n_evals=stop - t, reset=reset, **common)
+                reset = False
+            return t
+
         t, first_launch = 0, True
         for upto, fn in sorted(callbacks or [], key=lambda c: c[0]):
             n = min(upto + 1, total_evals) - t
             if n > 0 or first_launch:
-                t = self.generate_resident(s, d_first, n_given, num_samples, temperature, regularize, d_out,
-                                           t0=t, n_evals=max(n, 0), reset=first_launch, **common)
+                t = launch(t, n, first_launch)
                 first_launch = False
             torch.cuda.current_stream(dev).synchronize()
             fn()
         if total_evals - t > 0 or first_launch:
-            self.generate_resident(s, d_first, n_given, num_samples, temperature, regularize, d_out,
-                                   t0=t, n_evals=total_evals - t, reset=first_launch, **common)
+            launch(t, total_evals - t, first_launch)
         idx = d_out[:, :num_samples].cpu().numpy().astype(np.int64)      # device->host read; synchronises
         native.check(native.lib().wn_gen_check(s["handle"], torch.cuda.current_stream(dev).cuda_stream), "gen check")
         logits = d_logits[:, :num_samples].cpu().numpy() if want_logits else None
@@ -1001,11 +1110,14 @@ class _StackFunction(torch.autograd.Function):
     """forward()/wavenet() as one autograd node: parameters in, logits out; the input carries no gradient."""
 
     @staticmethod
-    def forward(ctx, model, x, out_len, index_input, cond, *params):
+    def forward(ctx, model, x, out_len, index_input, cond, local_y, local_hop, *params):
         saved = {}
         rt = model._runtime()
+        local = None if local_y is None else (local_y.detach(), local_hop)
         with torch.no_grad(), torch.cuda.device(rt.device()):
-            y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond)
+            y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond, local=local)
+        if local is not None and ctx.needs_input_grad[5]:
+            saved["local_dy"] = torch.zeros_like(local[0])          # the backward adds every layer's share
         ctx.model, ctx.saved = model, saved
         ctx.names = [n for n, _ in model.named_parameters()]
         return y
@@ -1018,9 +1130,10 @@ class _StackFunction(torch.autograd.Function):
         rt = ctx.model._runtime()
         with torch.no_grad(), torch.cuda.device(rt.device()):
             g = rt.stack_backward(ctx.saved, dlogits)
+        dy = ctx.saved.get("local_dy")
         ctx.saved = None
         rt.invalidate()          # an optimizer step follows; it may write through p.data, which no version counter sees
-        return (None, None, None, None, None) + tuple(g.get(n) for n in ctx.names)
+        return (None, None, None, None, None, dy, None) + tuple(g.get(n) for n in ctx.names)
 
 
 class WaveNetModel(nn.Module):
@@ -1042,6 +1155,10 @@ class WaveNetModel(nn.Module):
         condition_channels (Int):   G > 0: global conditioning (WaveNet paper section 2.5) on one (G,) vector h per
                                     sequence, a class label or a dense embedding; every layer adds Vf h / Vg h to its
                                     filter / gate pre-activations (``filter_cond_convs`` / ``gate_cond_convs``, 1x1, no bias)
+        local_condition_channels (Int): C > 0: local conditioning (paper section 2.5) on a (C, F) series y at one frame per
+                                    ``local_condition_hop`` samples (repeat upsampling): position t adds Uf y[:, t // hop] /
+                                    Ug y[:, t // hop] (``filter_local_convs`` / ``gate_local_convs``, 1x1, no bias)
+        local_condition_hop (Int):  samples per frame of the local condition (>= 1; required when C > 0)
 
     Shape:
         - Input: (N, classes, L) float32 one-hot, L >= receptive_field + output_length - 1 recommended
@@ -1050,7 +1167,7 @@ class WaveNetModel(nn.Module):
 
     def __init__(self, layers=10, blocks=4, dilation_channels=32, residual_channels=32, skip_channels=256,
                  end_channels=256, classes=256, output_length=32, kernel_size=2, dtype=torch.FloatTensor, bias=False,
-                 condition_channels=0):
+                 condition_channels=0, local_condition_channels=0, local_condition_hop=None):
         super(WaveNetModel, self).__init__()
         self.layers = layers
         self.blocks = blocks
@@ -1095,6 +1212,18 @@ class WaveNetModel(nn.Module):
             for _ in range(layers * blocks):
                 self.filter_cond_convs.append(nn.Conv1d(condition_channels, dilation_channels, 1, bias=False))
                 self.gate_cond_convs.append(nn.Conv1d(condition_channels, dilation_channels, 1, bias=False))
+        # created after the global ones, for the same reason
+        if local_condition_channels > 0 and (isinstance(local_condition_hop, bool) or not isinstance(local_condition_hop, int)
+                                             or local_condition_hop < 1):
+            raise ValueError(f"local_condition_hop must be an int >= 1 when local_condition_channels > 0, got {local_condition_hop!r}")
+        self.local_condition_channels = local_condition_channels
+        self.local_condition_hop = local_condition_hop if local_condition_channels > 0 else None
+        if local_condition_channels > 0:
+            self.filter_local_convs = nn.ModuleList()
+            self.gate_local_convs = nn.ModuleList()
+            for _ in range(layers * blocks):
+                self.filter_local_convs.append(nn.Conv1d(local_condition_channels, dilation_channels, 1, bias=False))
+                self.gate_local_convs.append(nn.Conv1d(local_condition_channels, dilation_channels, 1, bias=False))
 
         self.output_length = output_length
         self.receptive_field = receptive_field
@@ -1115,17 +1244,18 @@ class WaveNetModel(nn.Module):
         return state
 
     # ------------------------------------------------------------------ training-time path
-    def wavenet(self, input, dilation_func=None, condition=None):
+    def wavenet(self, input, dilation_func=None, condition=None, local_condition=None):
         """All T_final output columns, (N, classes, T_final), like the reference's wavenet() with wavenet_dilate.
         With ``dilation_func=self.queue_dilate`` it advances the fast-generation state by the one-hot column(s)
         in ``input`` and returns the logits of the last one as (1, classes, 1)."""
         if dilation_func is not None and getattr(dilation_func, "__func__", None) is WaveNetModel.queue_dilate:
-            if getattr(self, "condition_channels", 0):
+            if getattr(self, "condition_channels", 0) or getattr(self, "local_condition_channels", 0):
                 raise NotImplementedError("wavenet_b200: wavenet(x, queue_dilate) exists for the reference's unconditioned "
-                                          "models; sample a conditioned model with generate_fast(..., condition=)")
+                                          "models; sample a conditioned model with generate_fast(..., condition=, "
+                                          "local_condition=)")
             return self._queue_step(input)
         n = input.size(0)
-        y = self._stack(input, None, condition=condition)
+        y = self._stack(input, None, condition=condition, local_condition=local_condition)
         return y.view(n, -1, self.classes).transpose(1, 2).contiguous()
 
     def wavenet_dilate(self, input, dilation, init_dilation, i):
@@ -1170,25 +1300,61 @@ class WaveNetModel(nn.Module):
             raise ValueError(f"condition must hold int labels or float vectors, got {c.dtype}")
         return c.to(self._runtime().device()).contiguous()
 
-    def _stack(self, input, out_len, index_input=False, condition=None):
+    def _local_condition(self, local_condition, n, positions):
+        """The (n, C, F) float32 local condition series on the model's device for ``local_condition`` (a float array /
+        tensor), or None for a model without local conditioning.  F must cover ``positions`` positions: F >= ceil(positions /
+        hop).  A tensor that requires grad is returned as it is (moved / cast through autograd), so that it receives its
+        gradient.  Raises like _condition."""
+        C = getattr(self, "local_condition_channels", 0)    # whole-model pickles made before local conditioning lack it
+        if not C:
+            if local_condition is not None:
+                raise ValueError("this model has no local conditioning (local_condition_channels=0) but a local_condition "
+                                 "was given")
+            return None
+        hop = self.local_condition_hop
+        need = -(-positions // hop)
+        if local_condition is None:
+            raise ValueError(f"this model is locally conditioned on {C} channels: pass local_condition= (a float "
+                             f"({n}, {C}, F) series, F >= {need} frames of {hop} samples)")
+        try:
+            y = local_condition if torch.is_tensor(local_condition) else torch.as_tensor(np.asarray(local_condition))
+        except (TypeError, ValueError, RuntimeError) as e:
+            raise ValueError(f"local_condition must be a float array: {e}") from None
+        if not y.dtype.is_floating_point:
+            raise ValueError(f"local_condition must be a float ({n}, {C}, F) array, got {y.dtype}")
+        if y.dim() != 3 or y.shape[0] != n or y.shape[1] != C:
+            raise ValueError(f"local_condition must be a float ({n}, {C}, F) array, got shape {tuple(y.shape)}")
+        if y.shape[2] < need:
+            raise ValueError(f"local_condition has {y.shape[2]} frames; {positions} positions at hop {hop} need at least {need}")
+        if not (y.requires_grad and torch.is_grad_enabled()):
+            y = y.detach()
+        return y.to(self._runtime().device(), torch.float32).contiguous()
+
+    def _stack(self, input, out_len, index_input=False, condition=None, local_condition=None):
         cond = self._condition(condition, input.size(0))
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        y = self._local_condition(local_condition, input.size(0), input.size(-1))
+        hop = None if y is None else self.local_condition_hop
+        if torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or (y is not None and y.requires_grad)):
             if input.requires_grad:
                 raise NotImplementedError("wavenet_b200: no gradient with respect to the input (it is one-hot data)")
-            return _StackFunction.apply(self, input, out_len, index_input, cond, *self.parameters())
+            return _StackFunction.apply(self, input, out_len, index_input, cond, y, hop, *self.parameters())
         rt = self._runtime()
         with torch.cuda.device(rt.device()):       # native launches go to the CURRENT device: make it the model's
-            return rt.stack_forward(input, out_len, index_input=index_input, cond=cond)
+            return rt.stack_forward(input, out_len, index_input=index_input, cond=cond,
+                                    local=None if y is None else (y, hop))
 
-    def forward(self, input, condition=None):
+    def forward(self, input, condition=None, local_condition=None):
         """(N, classes, L) -> (N * output_length, classes): logits of the last ``output_length`` frames.
-        condition: for a conditioned model, labels (N,) or vectors (N, G) (see _condition)."""
-        return self._stack(input, self.output_length, condition=condition)
+        condition: for a conditioned model, labels (N,) or vectors (N, G) (see _condition).
+        local_condition: for a locally conditioned model, a float (N, C, F) series; frame f conditions input positions
+        [f * hop, (f + 1) * hop), and the output at position t predicts sample t + 1 (see _local_condition)."""
+        return self._stack(input, self.output_length, condition=condition, local_condition=local_condition)
 
-    def forward_indices(self, indices, condition=None):
+    def forward_indices(self, indices, condition=None, local_condition=None):
         """Same as ``forward(one_hot(indices))`` bit for bit, from (N, L) uint8 / int64 mu-law indices:
         start_conv on a one-hot column is a gather of one weight column (SURVEY.md section 8, row a4 / f2)."""
-        return self._stack(indices, self.output_length, index_input=True, condition=condition)
+        return self._stack(indices, self.output_length, index_input=True, condition=condition,
+                           local_condition=local_condition)
 
     # ------------------------------------------------------------------ generation
     def generate(self, num_samples, first_samples=None, temperature=1., condition=None):
@@ -1199,6 +1365,9 @@ class WaveNetModel(nn.Module):
         training-path forward on the window, draws with numpy's global RNG (or the argmax for ``temperature == 0``) and
         appends.  Returns the mu-law expanded float64 waveform of the WHOLE sequence (padding + given + generated), as the
         reference's closing lines do.  One device->host sync per sample: use generate_fast for anything but cross-checks."""
+        if getattr(self, "local_condition_channels", 0):
+            raise NotImplementedError("wavenet_b200: the slow generate() has no local conditioning; use "
+                                      "generate_fast(..., local_condition=)")
         self.eval()
         first = np.zeros(1, dtype=np.int64) if first_samples is None else self._first_array(first_samples)
         rf = self.receptive_field
@@ -1250,7 +1419,9 @@ class WaveNetModel(nn.Module):
                                 end_channels=self.end_conv_1.out_channels, classes=self.classes,
                                 output_length=self.output_length, kernel_size=self.kernel_size,
                                 bias=self.start_conv.bias is not None,
-                                condition_channels=getattr(self, "condition_channels", 0))
+                                condition_channels=getattr(self, "condition_channels", 0),
+                                local_condition_channels=getattr(self, "local_condition_channels", 0),
+                                local_condition_hop=getattr(self, "local_condition_hop", None))
             twin.load_state_dict(self.state_dict())
             sh = (key, twin.cuda())
             self.__dict__["_shadow"] = sh
@@ -1259,7 +1430,7 @@ class WaveNetModel(nn.Module):
         return sh[1]
 
     def generate_fast(self, num_samples, first_samples=None, temperature=1., regularize=0.,
-                      progress_callback=None, progress_interval=100, condition=None):
+                      progress_callback=None, progress_interval=100, condition=None, local_condition=None):
         """Fast-WaveNet sampling; returns the mu-law expanded waveform, float64 ndarray of ``num_samples`` values.
 
         Same schedule as the reference (wavenet_model.py:237-315): the queues are reset, the given samples warm
@@ -1267,20 +1438,27 @@ class WaveNetModel(nn.Module):
         numpy's GLOBAL RNG (one ``random_sample()`` per sample, which is what ``np.random.choice`` consumes), so
         ``np.random.seed(s)`` reproduces the reference's stream; ``temperature == 0`` takes the argmax.
         ``condition``: a conditioned model's label or (G,) vector for this stream.
+        ``local_condition``: a locally conditioned model's (C, F) series for this stream; evaluation e (which reads sample
+        e, the given samples first, and predicts sample e + 1) takes frame e // hop, so F >= ceil((n_given - 1 +
+        num_samples) / hop).
         """
         if self.start_conv.weight.device.type != "cuda":
             twin = self._cuda_shadow()
             audio = twin.generate_fast(num_samples, first_samples=first_samples, temperature=temperature,
                                        regularize=regularize, progress_callback=progress_callback,
-                                       progress_interval=progress_interval, condition=condition)
+                                       progress_interval=progress_interval, condition=condition,
+                                       local_condition=local_condition)
             for q, tq in zip(self.dilated_queues, twin.dilated_queues):
                 q.data, q.in_pos, q.out_pos = tq.data, tq.in_pos, tq.out_pos
             self.train()
             return audio
         cond = self._condition(self._one_condition(condition), 1)
-        self.eval()
         first = self._first_array(first_samples)
         num_given = first.shape[0]
+        if local_condition is not None:
+            local_condition = local_condition[None] if torch.is_tensor(local_condition) else np.asarray(local_condition)[None]
+        local = self._local_condition(local_condition, 1, num_given - 1 + num_samples)
+        self.eval()
         total = num_given + num_samples
         callbacks = []
         if progress_callback is not None:
@@ -1292,28 +1470,32 @@ class WaveNetModel(nn.Module):
                     callbacks.append((num_given - 1 + i, lambda i=i: progress_callback(i + num_given, total)))
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
-            idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond)
+            idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond,
+                                    local=None if local is None else (local.detach(), self.local_condition_hop))
         self._export_queues()
         self.train()
         generated = (idx[0] / self.classes) * 2. - 1
         return mu_law_expansion(generated, self.classes)
 
     def generate_fast_batch(self, num_samples, first_samples, temperature=1., regularize=0., uniforms=None,
-                            forced=None, return_logits=False, condition=None):
+                            forced=None, return_logits=False, condition=None, local_condition=None):
         """``n_streams`` independent generate_fast runs batched in one kernel (the reference has a single stream,
         wavenet_model.py:179).  first_samples: (n_streams, n_given) ints.  Returns int64 indices
         (n_streams, num_samples) [and the per-step logits].  Run through the same sampler kernel, stream s equals a
         single-stream run bit for bit (256-wide nets run the tensor-core cluster kernel for any number of streams; other
         nets a latency kernel for one stream and one thread-block cluster per stream otherwise, which differ at rounding
-        level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream."""
+        level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream.
+        local_condition: a locally conditioned model's (n_streams, C, F) series, one per stream (see generate_fast)."""
         first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
         first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
         cond = self._condition(condition, first.shape[0])
+        local = self._local_condition(local_condition, first.shape[0], first.shape[1] - 1 + num_samples)
         self.eval()
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, logits, _ = rt.generate(num_samples, first, temperature, regularize, uniforms=uniforms,
-                                         forced=forced, want_logits=return_logits, cond=cond)
+                                         forced=forced, want_logits=return_logits, cond=cond,
+                                         local=None if local is None else (local.detach(), self.local_condition_hop))
         self._export_queues()
         self.train()
         return (idx, logits) if return_logits else idx
@@ -1357,6 +1539,7 @@ class WaveNetModel(nn.Module):
                 s = rt.sampler(1)
                 native.check(native.lib().wn_gen_reset(s["handle"], torch.cuda.current_stream(dev).cuda_stream), "gen reset")
                 native.check(native.lib().wn_gen_set_condition(s["handle"], None), "gen condition")
+                s["cond"] = None
                 ses = dict(sampler=s, t=0, inp=torch.zeros(1, dtype=torch.int32, device=dev),
                            out=torch.zeros(1, dtype=torch.int32, device=dev),
                            logits=torch.zeros(self.classes, dtype=torch.float32, device=dev))

@@ -7,7 +7,8 @@ same constructor, ``train`` / ``validate`` and ``generate_audio`` -- SURVEY.md s
   ``torch.optim`` class can still be passed, as in the reference;
 * items may be class INDICES (``WavenetDataset(one_hot=False)``): they go through ``model.forward_indices``;
 * items may be ``(x, condition, target)`` for a conditioned model (``WavenetDataset(condition_on_file=True)``): the
-  condition (labels or vectors, one per item) goes to the model with its batch;
+  condition (labels or vectors, one per item) goes to the model with its batch; ``condition`` may also be a dict with keys
+  among ``condition`` and ``local_condition`` (a (C, F) frame-rate series per item), passed as the keyword arguments;
 * when ``torch.distributed`` is initialised the loop is data parallel: the dataset is sharded with a DistributedSampler and
   gradients are averaged over the ranks block by block while the backward runs (data_parallel.make_data_parallel).
 The Tensorboard side of the reference's Logger (model_logging.py) is out of scope; ``Logger`` here prints.
@@ -167,9 +168,16 @@ class WavenetTrainer:
 
     def _logits(self, x, condition=None):
         dev = self._device()
+        if isinstance(condition, dict):              # {"condition": ..., "local_condition": ...}, batched by the default collate
+            unknown = set(condition) - {"condition", "local_condition"}
+            if unknown:
+                raise ValueError(f"a condition dict may hold 'condition' and 'local_condition', not {sorted(unknown)}")
+            kw = dict(condition)
+        else:
+            kw = dict(condition=condition)
         if x.dtype in (torch.uint8, torch.int64) and x.dim() == 2:
-            return self.model.forward_indices(x.to(dev, non_blocking=True), condition=condition)
-        return self.model(x.to(dev, torch.float32, non_blocking=True), condition=condition)
+            return self.model.forward_indices(x.to(dev, non_blocking=True), **kw)
+        return self.model(x.to(dev, torch.float32, non_blocking=True), **kw)
 
     @staticmethod
     def _unpack(batch):
