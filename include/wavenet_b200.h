@@ -271,6 +271,42 @@ int wn_tb_stack_fwd_cond_frames(const wn_tb_stack_args* a, const float* d_cond, 
 int wn_cond_segment_sums(const void* d_dfg, int pair, int B, int L, int C, int gz, int hop, int n_frames, float* d_out,
                          void* stream);
 
+/* ---------------------------------------------------------------- (T) audio-rate local conditioning (learned upsampling)
+ * A learned upsampler brings the frame-rate series to one feature vector c[t] (C channels) per position, and every layer adds
+ *     Uf c[t] / Ug c[t]   to its filter / gate pre-activations.
+ * On the fused tensor-core blocks that is more contraction of pass A, not a table: c enters as K = Cpad more rows after the two
+ * taps, Cpad = C rounded up to the k-slab width (wn_tb_local_padded_channels: 32 with bf16 pairs, 64 single-pass; channels
+ * [C, Cpad) are zero in both c and U, so they add exact zeros).
+ * wn_tb_local_from_channels converts c (B, C, L) fp32, frames contiguous, to the chunked pair layout (B, 2, Cpad/8, L, 8) bf16
+ * with Cpad = wn_tb_local_padded_channels(C, precision), the channel count the forward entry points' tensor map reads.
+ * wn_tb_pack_local_weights packs every layer's [Uf; Ug] (the (channels, C, 1) weights of the local 1x1 convolutions) into ONE
+ * image d_u_all [n_layers][wn_tb_local_weight_bytes_per_layer(C, channels, precision)] with the tiling of the pass-A blocks of
+ * wn_tb_pack_all_weights; d_ptrs is a DEVICE table [n_layers][2] of {Uf, Ug}.
+ * wn_tb_block_fwd_local / wn_tb_stack_fwd_local are wn_tb_block_fwd / wn_tb_stack_fwd plus those K-slabs: d_c_pair is the
+ * converted c of the batch (frames [0, L), shared by all layers), d_u_all the packed image.  The pass-A biases are the layer's
+ * bf | bg, or, with d_cond non-NULL, the global condition table (one layer's slice [B][2 * channels] for the block entry point,
+ * the whole table [n_layers][B][2 * channels] for the stack one; see wn_cond_table).  Rows past L read zeros. */
+int    wn_tb_local_padded_channels(int C, int precision);
+size_t wn_tb_local_weight_bytes_per_layer(int C, int channels, int precision);
+int    wn_tb_local_from_channels(const float* d_c, void* d_c_pair, int B, int C, int L, int precision, void* stream);
+int    wn_tb_pack_local_weights(const float* const* d_ptrs, int n_layers, int C, int channels, int precision, void* d_u_all,
+                                void* stream);
+int    wn_tb_block_fwd_local(const wn_tb_block_args* a, const float* d_cond, const void* d_c_pair, int C, const void* d_u_all,
+                             void* stream);
+int    wn_tb_stack_fwd_local(const wn_tb_stack_args* a, const float* d_cond, const void* d_c_pair, int C, const void* d_u_all,
+                             void* stream);
+/* The backward of the same term, on the pre-activation gradient dfg of wn_tb_block_bwd_data (chunked pairs (B, 2, N/8, L, 8),
+ * N = 2 * channels; read in place as exact fp32 hi + lo) over the positions t >= gz, with c fp32 (B, C, L):
+ *     wn_local_weight_grad:    d_du[n][k] = sum_b sum_{t >= gz} dfg[b][t][n] * c[b][k][t]          ([N][C] = [dUf; dUg])
+ *     wn_local_data_grad_add:  d_dc[b][k][t] += sum_n d_u[n][k] * dfg[b][t][n]   for t >= gz   (d_u [N][C] fp32 = [Uf; Ug];
+ *                              d_dc (B, C, L) fp32; the layers add in turn)
+ * fp32 FMA with fixed summation orders and no atomics: both are deterministic.  d_work: wn_local_weight_grad_workspace_bytes
+ * (N, C) bytes. */
+size_t wn_local_weight_grad_workspace_bytes(int N, int C);
+int    wn_local_weight_grad(const void* d_dfg, int B, int L, int N, int gz, const float* d_c, int C, float* d_work, float* d_du,
+                            void* stream);
+int    wn_local_data_grad_add(const void* d_dfg, int B, int L, int N, int gz, const float* d_u, int C, float* d_dc, void* stream);
+
 /* ---------------------------------------------------------------- (T) head
  * replaces relu -> end_conv_1 -> relu -> end_conv_2 (wavenet_model.py:167-169) and forward()'s
  * slice/transpose/view (:191-196): logits (B*out_len, classes) for the LAST out_len frames only.

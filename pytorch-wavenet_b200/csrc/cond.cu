@@ -183,6 +183,129 @@ __global__ void __launch_bounds__(32 * FS) segment_sums_kernel(const void* __res
     }
 }
 
+
+// ---------------------------------------------------------------------------------------------- audio-rate local conditioning
+// With a learned upsampler every position has its own condition features c[t] (C channels), and the gradients of U and c are
+// contractions with the pre-activation gradient dfg (the backward's chunked pair tensor [b][plane][N/8][t][8], N = 2D, value
+// hi + lo) over the positions t >= gz:
+//     dU[n][k]     = sum_b sum_t dfg[b][t][n] * c[b][k][t]    (local_du_kernel: partial sums per frame split, then a fixed-order
+//                                                              reduction over the splits)
+//     dc[b][k][t] += sum_n U[n][k] * dfg[b][t][n]              (local_dc_kernel: every element has one owner thread)
+// Both read dfg where it is, as exact fp32 hi + lo, and accumulate with fp32 FMAs; neither uses atomics, so both are
+// deterministic.  c and dc are fp32 (B, C, L), U fp32 [N][C].
+constexpr int LT = 64, LS = 32, LMAX_SPLITS = 64;
+
+__device__ __forceinline__ void pair8(const uint4* __restrict__ dfg, size_t hi_idx, size_t plane, float (&v)[8]) {
+    const uint4 h = dfg[hi_idx], l = dfg[hi_idx + plane];
+    const unsigned hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        v[2 * e] = __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
+        v[2 * e + 1] = __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
+    }
+}
+
+__global__ void __launch_bounds__(256) local_du_kernel(const uint4* __restrict__ dfg, const float* __restrict__ c, int L, int N,
+                                                       int C, int gz, int tiles_per_seq, int total_tiles, int tiles_per_split,
+                                                       float* __restrict__ part) {
+    __shared__ __align__(16) float As[LS][LT + 4];     // [frame][n]
+    __shared__ __align__(16) float Bs[LS][LT + 4];     // [frame][k]
+    const int n0 = blockIdx.x * LT, k0 = blockIdx.y * LT, split = blockIdx.z;
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int chunks = N / 8;
+    const size_t plane = (size_t)chunks * L;
+    float acc[4][4] = {};
+    const int first = split * tiles_per_split, last = min(total_tiles, first + tiles_per_split);
+    for (int tile = first; tile < last; ++tile) {
+        const int b = tile / tiles_per_seq, t0 = gz + (tile % tiles_per_seq) * LS;
+        {
+            const int tt = tid % LS, ck = tid / LS, t = t0 + tt, chunk = n0 / 8 + ck;
+            float v[8] = {};
+            if (t < L && chunk < chunks) pair8(dfg, ((size_t)b * 2 * chunks + chunk) * L + t, plane, v);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) As[tt][ck * 8 + e] = v[e];
+        }
+        for (int i = tid; i < LT * LS; i += 256) {
+            const int tt = i % LS, kk = i / LS, t = t0 + tt, k = k0 + kk;
+            Bs[tt][kk] = (t < L && k < C) ? c[((size_t)b * C + k) * L + t] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int tt = 0; tt < LS; ++tt) {
+            const float4 a = *reinterpret_cast<const float4*>(&As[tt][ty * 4]);
+            const float4 w = *reinterpret_cast<const float4*>(&Bs[tt][tx * 4]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], wv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + ty * 4 + i, k = k0 + tx * 4 + j;
+            if (n < N && k < C) part[((size_t)split * N + n) * C + k] = acc[i][j];
+        }
+}
+
+__global__ void local_du_reduce_kernel(const float* __restrict__ part, int splits, int NC, float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= NC) return;
+    float s = 0.f;
+    for (int j = 0; j < splits; ++j) s += part[(size_t)j * NC + i];
+    out[i] = s;
+}
+
+__global__ void __launch_bounds__(256) local_dc_kernel(const uint4* __restrict__ dfg, const float* __restrict__ u, int L, int N,
+                                                       int C, int gz, float* __restrict__ dc) {
+    __shared__ __align__(16) float As[LS][LT + 4];     // [n][frame]
+    __shared__ __align__(16) float Bs[LS][LT + 4];     // [n][k]
+    const int t0 = gz + blockIdx.x * LT, k0 = blockIdx.y * LT, b = blockIdx.z;
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int chunks = N / 8;
+    const size_t plane = (size_t)chunks * L;
+    float acc[4][4] = {};                              // [k][frame]
+    for (int nb = 0; nb < N; nb += LS) {
+        {
+            const int tt = tid % LT, ck = tid / LT, t = t0 + tt, chunk = nb / 8 + ck;
+            float v[8] = {};
+            if (t < L) pair8(dfg, ((size_t)b * 2 * chunks + chunk) * L + t, plane, v);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) As[ck * 8 + e][tt] = v[e];
+        }
+        for (int i = tid; i < LS * LT; i += 256) {
+            const int kk = i % LT, nn = i / LT, k = k0 + kk;
+            Bs[nn][kk] = k < C ? u[(size_t)(nb + nn) * C + k] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int nn = 0; nn < LS; ++nn) {
+            const float4 a = *reinterpret_cast<const float4*>(&As[nn][tx * 4]);
+            const float4 w = *reinterpret_cast<const float4*>(&Bs[nn][ty * 4]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(wv[i], av[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int k = k0 + ty * 4 + i;
+        if (k >= C) continue;
+        float* row = dc + ((size_t)b * C + k) * L;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int t = t0 + tx * 4 + j;
+            if (t < L) row[t] += acc[i][j];
+        }
+    }
+}
+
 }  // namespace cond
 }  // namespace wn
 
@@ -236,6 +359,54 @@ extern "C" int wn_cond_segment_sums(const void* d_dfg, int pair, int B, int L, i
     cudaStream_t st = (cudaStream_t)stream;
     if (pair) cond::segment_sums_kernel<true><<<dim3(C / 8, gy, B), block, 0, st>>>(d_dfg, L, C, gz, hop, n_frames, d_out);
     else cond::segment_sums_kernel<false><<<dim3((C + 31) / 32, gy, B), block, 0, st>>>(d_dfg, L, C, gz, hop, n_frames, d_out);
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// frame splits of the dU partial sums: a function of the shape only, so the reduction order (and the result) is fixed
+static int local_splits(int B, int L, int N, int C, int gz, int* tiles_per_seq, int* total, int* per_split) {
+    *tiles_per_seq = ceil_div(L - gz, cond::LS);
+    *total = B * *tiles_per_seq;
+    const int blocks_xy = ceil_div(N, cond::LT) * ceil_div(C, cond::LT);
+    int s = ceil_div(512, blocks_xy);
+    s = s > cond::LMAX_SPLITS ? cond::LMAX_SPLITS : s;
+    s = s > *total ? *total : s;
+    *per_split = ceil_div(*total, s);
+    return ceil_div(*total, *per_split);
+}
+
+extern "C" size_t wn_local_weight_grad_workspace_bytes(int N, int C) {
+    return N > 0 && C > 0 ? (size_t)cond::LMAX_SPLITS * N * C * sizeof(float) : 0;
+}
+
+extern "C" int wn_local_weight_grad(const void* d_dfg, int B, int L, int N, int gz, const float* d_c, int C, float* d_work,
+                                    float* d_du, void* stream) {
+    WN_REQUIRE(d_dfg && d_c && d_work && d_du, WN_E_BADARG, "wn_local_weight_grad: null pointer");
+    WN_REQUIRE(B > 0 && L > 0 && N > 0 && N % 8 == 0 && C > 0 && gz >= 0 && (uintptr_t)d_dfg % 16 == 0, WN_E_BADARG,
+               "wn_local_weight_grad: bad sizes");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (gz >= L) {
+        WN_CUDA(cudaMemsetAsync(d_du, 0, sizeof(float) * (size_t)N * C, st));
+        return 0;
+    }
+    int tps, total, per;
+    const int splits = local_splits(B, L, N, C, gz, &tps, &total, &per);
+    const dim3 grid((unsigned)ceil_div(N, cond::LT), (unsigned)ceil_div(C, cond::LT), (unsigned)splits);
+    cond::local_du_kernel<<<grid, 256, 0, st>>>((const uint4*)d_dfg, d_c, L, N, C, gz, tps, total, per, d_work);
+    WN_CUDA(cudaGetLastError());
+    cond::local_du_reduce_kernel<<<ceil_div(N * C, 256), 256, 0, st>>>(d_work, splits, N * C, d_du);
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int wn_local_data_grad_add(const void* d_dfg, int B, int L, int N, int gz, const float* d_u, int C, float* d_dc,
+                                      void* stream) {
+    WN_REQUIRE(d_dfg && d_u && d_dc, WN_E_BADARG, "wn_local_data_grad_add: null pointer");
+    WN_REQUIRE(B > 0 && B <= 65535 && L > 0 && N > 0 && N % cond::LS == 0 && C > 0 && gz >= 0 && (uintptr_t)d_dfg % 16 == 0,
+               WN_E_BADARG, "wn_local_data_grad_add: bad sizes");
+    if (gz >= L) return 0;
+    const dim3 grid((unsigned)ceil_div(L - gz, cond::LT), (unsigned)ceil_div(C, cond::LT), (unsigned)B);
+    cond::local_dc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint4*)d_dfg, d_u, L, N, C, gz, d_dc);
     WN_CUDA(cudaGetLastError());
     return 0;
 }

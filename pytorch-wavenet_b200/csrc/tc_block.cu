@@ -133,15 +133,26 @@ __device__ __forceinline__ void slab_mma(float (&acc)[2][64], unsigned a, unsign
     wgmma_keep(acc[1]);
 }
 
+// Audio-rate local conditioning features (learned upsampling) as extra K-slabs of pass A: Uf c[t] | Ug c[t] is more contraction
+// of the filter / gate pre-activations, K = Cpad more rows after the 2 * CH of the two taps.
+struct KslabParams {
+    CUtensorMap mapC;              // c as a chunked pair tensor (B, 2, Cpad/8, L, 8), origin 0; shared by all layers
+    CUtensorMap mapU;              // every layer's packed [Uf; Ug] image (wn_tb_pack_local_weights), 2 KB rows
+    int n_slabs;                   // Cpad / KS k-slabs per pass-A n-tile
+};
+
 // MULTI = false: one layer (`single`), items are independent.  MULTI = true: ALL layers of a forward in one persistent launch:
 // the global item list is layer-major and dealt round-robin to the CTA pairs, an item waits (in its producer) for the items of
 // the previous layer that wrote the frames it reads, and announces itself when its epilogues have stored -- no launch gaps and
 // no idle tail between layers.  COND: every sequence has its own filter / gate biases, read from the condition table instead of
 // bf / bg (a separate instantiation, so the unconditioned kernels carry no trace of it).  FRAMES (with COND): the table has a frame
-// axis (local conditioning), and each of a thread's two rows reads its own frame's row of it.
-template <typename C, bool MULTI, bool COND, bool FRAMES>
-__global__ void __launch_bounds__(NTHREADS, 1)
-block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_constant__ CUtensorMap mapW, const BlockParams p) {
+// axis (local conditioning), and each of a thread's two rows reads its own frame's row of it.  KS (empty, or one KslabParams):
+// after each pass-A n-tile's activation slabs the producer streams KslabParams::n_slabs more stages (the c slab at the CTA's
+// absolute frames and the two U halves) and the consumers accumulate them with the same slab_mma.  KSLAB runs as its own kernel
+// (block_fused_local_kernel), so the other kernels keep their parameter list.
+template <typename C, bool MULTI, bool COND, bool FRAMES, bool KSLAB>
+__device__ __forceinline__ void block_fused_body(const LayerDesc& single, const CUtensorMap& mapW, const BlockParams p,
+                                                 const KslabParams* kslab) {
     constexpr int CH = C::CH, NST = C::NST;
     auto LD = [&](int l) -> const LayerDesc& { return MULTI ? p.layers[l] : single; };
     extern __shared__ unsigned char smem_raw[];
@@ -200,7 +211,7 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
                     if (Ld.war_layer >= 0) wait_counter(p.layer_done + Ld.war_layer, (unsigned)LD(Ld.war_layer).n_items);
                     asm volatile("fence.proxy.async;" ::: "memory");      // generic-proxy writes of other SMs -> this thread's TMA reads
                 }
-                for (int j = 0; j < C::NT_A; ++j)
+                for (int j = 0; j < C::NT_A; ++j) {
                     for (int sl = 0; sl < C::SLABS_A; ++sl) {
                         unsigned long long* bar;
                         unsigned char* dst = acquire(bar, 3 * SLOT);
@@ -209,6 +220,18 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
                         for (int h = 0; h < 2; ++h)
                             tma_load_2d(dst + (1 + h) * SLOT, &mapW, 0, w_row0 + ((j * C::SLABS_A + sl) * 2 + h) * 8, bar);
                     }
+                    if constexpr (KSLAB) {
+                        const KslabParams& kp = *kslab;
+                        const int u_row0 = (w_row0 / C::WROWS_LAYER) * C::NT_A * kp.n_slabs * 16;
+                        for (int sl = 0; sl < kp.n_slabs; ++sl) {
+                            unsigned long long* bar;
+                            unsigned char* dst = acquire(bar, 3 * SLOT);
+                            tma_load_4d(dst, &kp.mapC, 2 * (t0 + rank * BM), sl * C::KC, 0, b, bar);
+                            for (int h = 0; h < 2; ++h)
+                                tma_load_2d(dst + (1 + h) * SLOT, &kp.mapU, 0, u_row0 + ((j * kp.n_slabs + sl) * 2 + h) * 8, bar);
+                        }
+                    }
+                }
                 for (int j = 0; j < (need_skip ? C::NT_B : C::NT_R); ++j)
                     for (int s8 = 0; s8 < C::SLABS_B; ++s8) {
                         unsigned long long* bar;
@@ -255,6 +278,14 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
                     const unsigned st = s32(ring + s * STAGE);
                     slab_mma<C>(acc, st + a_off, SLOT / 2, st + SLOT, sl == 0);
                     mbar_arrive(empty + s);
+                }
+                if constexpr (KSLAB) {
+                    for (int sl = 0; sl < kslab->n_slabs; ++sl) {
+                        const unsigned s = wait_stage();
+                        const unsigned st = s32(ring + s * STAGE);
+                        slab_mma<C>(acc, st + a_off, SLOT / 2, st + SLOT, false);
+                        mbar_arrive(empty + s);
+                    }
                 }
                 // FRAMES: the table rows of this thread's two rows' frames, derived after the n-tile's MMAs so that nothing new is
                 // live across them; rows past L (last tile) read the last frame's row
@@ -362,6 +393,18 @@ block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_consta
     }
 }
 
+template <typename C, bool MULTI, bool COND, bool FRAMES>
+__global__ void __launch_bounds__(NTHREADS, 1)
+block_fused_kernel(const __grid_constant__ LayerDesc single, const __grid_constant__ CUtensorMap mapW, const BlockParams p) {
+    block_fused_body<C, MULTI, COND, FRAMES, false>(single, mapW, p, nullptr);
+}
+template <typename C, bool MULTI, bool COND>
+__global__ void __launch_bounds__(NTHREADS, 1)
+block_fused_local_kernel(const __grid_constant__ LayerDesc single, const __grid_constant__ CUtensorMap mapW, const BlockParams p,
+                         const __grid_constant__ KslabParams kslab) {
+    block_fused_body<C, MULTI, COND, false, true>(single, mapW, p, &kslab);
+}
+
 // ---------------------------------------------------------------------------------------------- weight packing
 // Packed image of one layer (bf16): pass A blocks [n-tile j][k-slab sl][half r], pass B blocks [j][s][r]; a block is the 16 KB
 // slot image [plane][chunk KC][row 128][8].  Pass A: N row n = r*128 + row is filter (r = 0) or gate (r = 1) channel 128j + row;
@@ -402,7 +445,51 @@ __global__ void pack_block_all_kernel(const float* const* __restrict__ ptrs, __n
         }
 }
 
+// Packed [Uf; Ug] image of the audio-rate local conditioning (KslabParams::mapU), same tiling as the pass-A blocks above: blocks
+// [n-tile j][k-slab sl < Cpad / KS][half r], N row r*128 + row = filter (r = 0) / gate (r = 1) channel 128j + row, K index
+// sl*KS + ck*8 + e = condition channel (zero from C up to Cpad).  ptrs[layer] = {Uf, Ug}, each (CH, C, 1); blockIdx.y = layer.
+template <typename C>
+__global__ void pack_local_all_kernel(const float* const* __restrict__ ptrs, int Cc, int n_slabs, __nv_bfloat16* __restrict__ out_all) {
+    const float* uf = ptrs[(size_t)blockIdx.y * 2];
+    const float* ug = ptrs[(size_t)blockIdx.y * 2 + 1];
+    const int n_blocks = C::NT_A * n_slabs * 2;
+    __nv_bfloat16* out = out_all + (size_t)blockIdx.y * n_blocks * (SLOT / 2);
+    constexpr int per_plane = SLOT / 2 / C::PLANES;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (long long)n_blocks * per_plane;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int blk = (int)(i / per_plane), w = (int)(i % per_plane);
+        const int ck = w / (BM * 8), row = (w / 8) % BM, e = w % 8;
+        const int j = blk / (n_slabs * 2), sl = (blk / 2) % n_slabs, r = blk % 2;
+        const int k = sl * C::KS + ck * 8 + e, cout = j * 128 + row;
+        const float v = k < Cc ? (r == 0 ? uf : ug)[(size_t)cout * Cc + k] : 0.f;
+        const __nv_bfloat16 h = __float2bfloat16_rn(v);
+        __nv_bfloat16* o = out + (size_t)blk * (SLOT / 2) + w;
+        o[0] = h;
+        if constexpr (C::PAIR) o[per_plane] = __float2bfloat16_rn(v - __bfloat162float(h));
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- layout converters
+// channel-major fp32 (B, C, L) -> chunked pair (B, 2, Cpad/8, L, 8), channels [C, Cpad) zero
+__global__ void pair_from_channels_kernel(const float* __restrict__ x, uint4* __restrict__ out, int B, int C, int L, int c_pad) {
+    const int chunks = c_pad / 8;
+    const long long total = (long long)B * chunks * L;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int t = (int)(i % L), ck = (int)((i / L) % chunks), b = (int)(i / ((long long)L * chunks));
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const int c = ck * 8 + e;
+            v[e] = c < C ? x[((size_t)b * C + c) * L + t] : 0.f;
+        }
+        unsigned hi[4], lo[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) split2(v[2 * k], v[2 * k + 1], hi[k], lo[k]);
+        uint4* o = out + ((size_t)b * 2 * chunks + ck) * L + t;
+        o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+        o[(size_t)chunks * L] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    }
+}
 // fp32 frames (B, L, C) -> chunked pair (B, 2, C/8, L, 8) for frames [t_begin, L)
 __global__ void pair_from_frames_kernel(const float* __restrict__ x, uint4* __restrict__ out, int B, int L, int C, int t_begin) {
     const int chunks = C / 8;
@@ -598,6 +685,13 @@ static int launch_cfg(cudaLaunchConfig_t& cfg, int grid, size_t smem, cudaStream
     return 0;
 }
 
+// the fused block kernel of an instantiation; a KslabParams argument selects the K-slab (audio-rate local conditioning) kernel
+template <typename C, bool MULTI, bool COND, bool FRAMES, typename... KS>
+static auto kernel_of() {
+    if constexpr (sizeof...(KS) > 0) return tb::block_fused_local_kernel<C, MULTI, COND>;
+    else return tb::block_fused_kernel<C, MULTI, COND, FRAMES>;
+}
+
 template <typename C>
 static int fill_layer(tb::LayerDesc& d, const void* h_in, void* h_out, const float* bias4, float* fg_save, int layer, int B, int L,
                       int dilation, int in_start, int out_start, int skip_init, int item_base, const float* cond,
@@ -616,8 +710,8 @@ static int fill_layer(tb::LayerDesc& d, const void* h_in, void* h_out, const flo
     return 0;
 }
 
-template <typename C, bool COND, bool FRAMES>
-static int launch_block(const wn_tb_block_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
+template <typename C, bool COND, bool FRAMES, typename... KS>
+static int launch_block(const wn_tb_block_args* a, const float* cond, int n_frames, int hop, cudaStream_t st, const KS&... ks) {
     int dev = 0, sms = 0;
     WN_CUDA(cudaGetDevice(&dev));
     WN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -630,13 +724,14 @@ static int launch_block(const wn_tb_block_args* a, const float* cond, int n_fram
     memset(&p, 0, sizeof(p));
     p.B = a->B; p.L = a->L; p.skip_start = a->skip_start; p.n_layers = 1; p.total_items = d.n_items;
     p.skip = (float4*)a->d_skip;
-    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, false, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    const auto kern = kernel_of<C, false, COND, FRAMES, KS...>();
+    WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
     int grid = 2 * p.total_items;
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
     launch_cfg(cfg, grid, C::SMEM_BYTES, st);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, false, COND, FRAMES>, d, mW, p));
+    WN_CUDA(cudaLaunchKernelEx(&cfg, kern, d, mW, p, ks...));
     WN_CUDA(cudaGetLastError());
     return 0;
 }
@@ -686,8 +781,8 @@ extern "C" long long wn_tb_stack_items(int n_layers, int B, int L, const int* ou
     return n;
 }
 
-template <typename C, bool COND, bool FRAMES>
-static int launch_stack(const wn_tb_stack_args* a, const float* cond, int n_frames, int hop, cudaStream_t st) {
+template <typename C, bool COND, bool FRAMES, typename... KS>
+static int launch_stack(const wn_tb_stack_args* a, const float* cond, int n_frames, int hop, cudaStream_t st, const KS&... ks) {
     int dev = 0, sms = 0;
     WN_CUDA(cudaGetDevice(&dev));
     WN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -721,14 +816,15 @@ static int launch_stack(const wn_tb_stack_args* a, const float* cond, int n_fram
     p.skip = (float4*)a->d_skip;
     p.layers = (const tb::LayerDesc*)a->d_desc;
     p.item_done = a->d_flags; p.layer_done = a->d_flags + base;
-    WN_CUDA(cudaFuncSetAttribute(tb::block_fused_kernel<C, true, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    const auto kern = kernel_of<C, true, COND, FRAMES, KS...>();
+    WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
     // every CTA must be resident (items wait for items of other CTAs): one CTA per SM, at most sms/2 pairs
     int grid = 2 * base;
     const int max_grid = (sms / 2) * 2;
     if (grid > max_grid) grid = max_grid;
     cudaLaunchConfig_t cfg;
     launch_cfg(cfg, grid, C::SMEM_BYTES, st);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, tb::block_fused_kernel<C, true, COND, FRAMES>, desc[0], mW, p));
+    WN_CUDA(cudaLaunchKernelEx(&cfg, kern, desc[0], mW, p, ks...));
     WN_CUDA(cudaGetLastError());
     return 0;
 }
@@ -767,4 +863,115 @@ static int tb_stack_fwd_impl(const wn_tb_stack_args* a, const float* d_cond, int
     if (a->precision == WN_PREC_BF16_PAIRS) return launch_stack_c<tb::Cfg<256, true>>(a, d_cond, n_frames, hop, st);
     if (a->channels == 256) return launch_stack_c<tb::Cfg<256, false>>(a, d_cond, n_frames, hop, st);
     return launch_stack_c<tb::Cfg<512, false>>(a, d_cond, n_frames, hop, st);
+}
+
+// ---------------------------------------------------------------------------------------------- audio-rate local conditioning
+// The learned upsampler's output c (B, C, L) enters pass A as K-slabs (block_fused_kernel with a KslabParams): c is converted
+// once per forward to a chunked pair tensor of Cpad channels, and every layer's [Uf; Ug] is packed into its own slab image.
+template <typename C>
+static int local_slabs(int Cc) { return ceil_div(Cc, C::KS); }
+static int local_slab_width(int precision) { return precision == WN_PREC_BF16_PAIRS ? tb::Cfg<256, true>::KS : tb::Cfg<256, false>::KS; }
+
+extern "C" int wn_tb_local_padded_channels(int C, int precision) {
+    if (C < 1 || (precision != WN_PREC_BF16_PAIRS && precision != WN_PREC_BF16)) return 0;
+    return ceil_div(C, local_slab_width(precision)) * local_slab_width(precision);
+}
+extern "C" size_t wn_tb_local_weight_bytes_per_layer(int C, int channels, int precision) {
+    if (!wn_tb_precision_supported(channels, precision) || C < 1) return 0;
+    return (size_t)(2 * channels / 256) * (wn_tb_local_padded_channels(C, precision) / local_slab_width(precision)) * 2 * tb::SLOT;
+}
+
+extern "C" int wn_tb_pack_local_weights(const float* const* d_ptrs, int n_layers, int C, int channels, int precision, void* d_u_all,
+                                        void* stream) {
+    WN_REQUIRE(d_ptrs && d_u_all && n_layers > 0 && C > 0, WN_E_BADARG, "wn_tb_pack_local_weights: bad arguments");
+    WN_REQUIRE(wn_tb_precision_supported(channels, precision), WN_E_UNSUPP,
+               "wn_tb_pack_local_weights: %d channels with precision %d is not supported", channels, precision);
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid(74, n_layers);
+    __nv_bfloat16* out = (__nv_bfloat16*)d_u_all;
+    if (precision == WN_PREC_BF16_PAIRS) {
+        using Cf = tb::Cfg<256, true>;
+        tb::pack_local_all_kernel<Cf><<<grid, 256, 0, st>>>(d_ptrs, C, local_slabs<Cf>(C), out);
+    } else if (channels == 256) {
+        using Cf = tb::Cfg<256, false>;
+        tb::pack_local_all_kernel<Cf><<<grid, 256, 0, st>>>(d_ptrs, C, local_slabs<Cf>(C), out);
+    } else {
+        using Cf = tb::Cfg<512, false>;
+        tb::pack_local_all_kernel<Cf><<<grid, 256, 0, st>>>(d_ptrs, C, local_slabs<Cf>(C), out);
+    }
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int wn_tb_local_from_channels(const float* d_c, void* d_c_pair, int B, int C, int L, int precision, void* stream) {
+    const int c_pad = wn_tb_local_padded_channels(C, precision);
+    WN_REQUIRE(d_c && d_c_pair && B > 0 && C > 0 && L > 0 && c_pad > 0, WN_E_BADARG, "wn_tb_local_from_channels: bad arguments");
+    tb::pair_from_channels_kernel<<<1184, 256, 0, (cudaStream_t)stream>>>(d_c, (uint4*)d_c_pair, B, C, L, c_pad);
+    WN_CUDA(cudaGetLastError());
+    return 0;
+}
+
+template <typename C>
+static int make_kslab(tb::KslabParams& k, const void* d_c_pair, const void* d_u_all, int B, int L, int Cc, int n_layers) {
+    memset(&k, 0, sizeof(k));
+    k.n_slabs = local_slabs<C>(Cc);
+    if (int rc = tb::make_pair_map(&k.mapC, d_c_pair, B, L, k.n_slabs * C::KS, 0, tb::BM, C::KC, C::PLANES)) return rc;
+    return tb::make_wrows_map(&k.mapU, d_u_all, (long long)n_layers * C::NT_A * k.n_slabs * 16);
+}
+
+static int check_local(const void* d_c_pair, int C, const void* d_u_all, const char* who) {
+    WN_REQUIRE(d_c_pair && d_u_all && C > 0, WN_E_BADARG, "%s: null pointer or no condition channels", who);
+    WN_REQUIRE(((uintptr_t)d_c_pair | (uintptr_t)d_u_all) % 16 == 0, WN_E_BADARG, "%s: c and U must be 16-byte aligned", who);
+    return 0;
+}
+
+template <typename C>
+static int launch_block_local(const wn_tb_block_args* a, const float* cond, const void* d_c_pair, int Cc, const void* d_u_all,
+                              cudaStream_t st) {
+    tb::KslabParams k;
+    if (int rc = make_kslab<C>(k, d_c_pair, d_u_all, a->B, a->L, Cc, a->n_layers)) return rc;
+    return cond ? launch_block<C, true, false>(a, cond, 0, 0, st, k) : launch_block<C, false, false>(a, nullptr, 0, 0, st, k);
+}
+
+extern "C" int wn_tb_block_fwd_local(const wn_tb_block_args* a, const float* d_cond, const void* d_c_pair, int C, const void* d_u_all,
+                                     void* stream) {
+    if (int rc = check_local(d_c_pair, C, d_u_all, "wn_tb_block_fwd_local")) return rc;
+    WN_REQUIRE(a, WN_E_BADARG, "wn_tb_block_fwd: null args");
+    WN_REQUIRE(a->d_h_in && a->d_h_out && a->d_skip && a->d_w_all && a->d_bias4, WN_E_BADARG, "wn_tb_block_fwd: null pointer");
+    WN_REQUIRE(wn_tb_precision_supported(a->channels, a->precision), WN_E_UNSUPP, "wn_tb_block_fwd: %d channels with precision %d is not supported",
+               a->channels, a->precision);
+    WN_REQUIRE(a->B > 0 && a->L > 0 && a->dilation >= 1 && a->in_start >= 0 && a->out_start >= a->in_start && a->out_start < a->L &&
+                   a->skip_start >= a->out_start && a->skip_start < a->L && a->layer >= 0 && a->layer < a->n_layers,
+               WN_E_BADARG, "wn_tb_block_fwd: bad frame ranges or layer index");
+    WN_REQUIRE(((uintptr_t)a->d_h_in | (uintptr_t)a->d_h_out | (uintptr_t)a->d_skip | (uintptr_t)a->d_w_all | (uintptr_t)d_cond) % 16 == 0,
+               WN_E_BADARG, "wn_tb_block_fwd: buffers must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a->precision == WN_PREC_BF16_PAIRS) return launch_block_local<tb::Cfg<256, true>>(a, d_cond, d_c_pair, C, d_u_all, st);
+    if (a->channels == 256) return launch_block_local<tb::Cfg<256, false>>(a, d_cond, d_c_pair, C, d_u_all, st);
+    return launch_block_local<tb::Cfg<512, false>>(a, d_cond, d_c_pair, C, d_u_all, st);
+}
+
+template <typename C>
+static int launch_stack_local(const wn_tb_stack_args* a, const float* cond, const void* d_c_pair, int Cc, const void* d_u_all,
+                              cudaStream_t st) {
+    tb::KslabParams k;
+    if (int rc = make_kslab<C>(k, d_c_pair, d_u_all, a->B, a->L, Cc, a->n_layers)) return rc;
+    return cond ? launch_stack<C, true, false>(a, cond, 0, 0, st, k) : launch_stack<C, false, false>(a, nullptr, 0, 0, st, k);
+}
+
+extern "C" int wn_tb_stack_fwd_local(const wn_tb_stack_args* a, const float* d_cond, const void* d_c_pair, int C, const void* d_u_all,
+                                     void* stream) {
+    if (int rc = check_local(d_c_pair, C, d_u_all, "wn_tb_stack_fwd_local")) return rc;
+    WN_REQUIRE(a, WN_E_BADARG, "wn_tb_stack_fwd: null args");
+    WN_REQUIRE(a->h_ptrs && a->d_skip && a->d_w_all && a->d_bias_all && a->d_desc && a->d_flags && a->dilations && a->in_start && a->out_start,
+               WN_E_BADARG, "wn_tb_stack_fwd: null pointer");
+    WN_REQUIRE(wn_tb_precision_supported(a->channels, a->precision), WN_E_UNSUPP, "wn_tb_stack_fwd: %d channels with precision %d is not supported",
+               a->channels, a->precision);
+    WN_REQUIRE(a->B > 0 && a->L > 0 && a->n_layers > 0 && a->skip_start >= 0 && a->skip_start < a->L && (uintptr_t)a->d_desc % 128 == 0,
+               WN_E_BADARG, "wn_tb_stack_fwd: bad sizes (d_desc must be 128-byte aligned)");
+    WN_REQUIRE((uintptr_t)d_cond % 16 == 0, WN_E_BADARG, "wn_tb_stack_fwd: the condition table must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a->precision == WN_PREC_BF16_PAIRS) return launch_stack_local<tb::Cfg<256, true>>(a, d_cond, d_c_pair, C, d_u_all, st);
+    if (a->channels == 256) return launch_stack_local<tb::Cfg<256, false>>(a, d_cond, d_c_pair, C, d_u_all, st);
+    return launch_stack_local<tb::Cfg<512, false>>(a, d_cond, d_c_pair, C, d_u_all, st);
 }

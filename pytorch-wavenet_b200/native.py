@@ -170,6 +170,15 @@ SIGNATURES = {
     "wn_tb_block_fwd_cond_frames": (C.c_int, [C.POINTER(TbBlockArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "wn_tb_stack_fwd_cond_frames": (C.c_int, [C.POINTER(TbStackArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "wn_cond_segment_sums": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p] * 2),
+    "wn_tb_local_padded_channels": (C.c_int, [C.c_int] * 2),
+    "wn_tb_local_weight_bytes_per_layer": (C.c_size_t, [C.c_int] * 3),
+    "wn_tb_local_from_channels": (C.c_int, [C.c_void_p] * 2 + [C.c_int] * 4 + [C.c_void_p]),
+    "wn_tb_pack_local_weights": (C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p] * 2),
+    "wn_tb_block_fwd_local": (C.c_int, [C.POINTER(TbBlockArgs), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wn_tb_stack_fwd_local": (C.c_int, [C.POINTER(TbStackArgs), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wn_local_weight_grad_workspace_bytes": (C.c_size_t, [C.c_int] * 2),
+    "wn_local_weight_grad": (C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_int] + [C.c_void_p] * 3),
+    "wn_local_data_grad_add": (C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_int] + [C.c_void_p] * 2),
     "wn_wgrad_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "wn_wgrad": (C.c_int, [C.POINTER(WgradArgs), C.c_void_p]),
     "wn_tc_wgrad_supported": (C.c_int, [C.c_int, C.c_int]),

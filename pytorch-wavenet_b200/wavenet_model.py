@@ -65,7 +65,7 @@ class _Packs:
         self.rt, self.groups = rt, {}
 
     def __getitem__(self, name):
-        if name in ("tb", "tb_bwd") and name in self.groups and self.groups[name][-1] != self.rt.tb_precision():
+        if name in ("tb", "tb_bwd", "tb_local") and name in self.groups and self.groups[name][-1] != self.rt.tb_precision():
             del self.groups[name]                       # packed for the other operand precision
         if name not in self.groups:
             rt = self.rt
@@ -215,6 +215,17 @@ class _Packs:
                                                 stream), "pack tb")
         return tb_w, tb_b, prec
 
+    def _build_tb_local(self, stream):
+        """Every layer's [Uf; Ug] for the K-slabs of the audio-rate local conditioning (wn_tb_pack_local_weights)."""
+        rt, lib, m = self.rt, native.lib(), self.rt.model
+        R, nl, C = m.residual_channels, m.layers * m.blocks, m.local_condition_channels
+        prec, dev = rt.tb_precision(), rt.device()
+        u = torch.empty(nl, lib.wn_tb_local_weight_bytes_per_layer(C, R, prec), device=dev, dtype=torch.uint8)
+        ptrs = torch.tensor([[m.filter_local_convs[i].weight.data_ptr(), m.gate_local_convs[i].weight.data_ptr()]
+                             for i in range(nl)], dtype=torch.int64, device=dev)
+        native.check(lib.wn_tb_pack_local_weights(ptrs.data_ptr(), nl, C, R, prec, u.data_ptr(), stream), "pack tb local")
+        return u, ptrs, prec
+
     def _build_tb_bwd(self, stream):
         rt, lib = self.rt, native.lib()
         R, nl = self._dims()[0], self._dims()[6]
@@ -326,12 +337,14 @@ class _Runtime:
         return self.packed
 
     # ------------------------------------------------------------------ training-path forward
-    def stack_forward(self, x, out_len, index_input=False, save=None, cond=None, local=None):
+    def stack_forward(self, x, out_len, index_input=False, save=None, cond=None, local=None, upsampled=None):
         """x: (B, classes, L) float32 one-hot/dense, or (B, L) uint8/int64 indices when index_input.
         Returns logits (B*out_len, classes) for the last out_len frames (out_len=None: all T_final frames).
         save: optional dict; filled with what the backward needs (every layer's input, tanh/sigmoid outputs, skip).
         cond: the (B, G) fp32 condition rows of a conditioned model (WaveNetModel._condition), else None.
-        local: (y, hop) of a locally conditioned model, y the (B, C, F) fp32 series (WaveNetModel._local_condition), else None."""
+        local: (y, hop) of a locally conditioned model, y the (B, C, F) fp32 series (WaveNetModel._local_condition), else None.
+        upsampled: the (B, C, L) fp32 audio-rate features of a model with a learned upsampler (WaveNetModel._upsample), else
+        None: K-slabs of pass A on the fused tensor-core blocks, the local path at hop 1 on the FFMA blocks."""
         m, lib = self.model, native.lib()
         dev = self.device()
         if x.device != dev:
@@ -370,14 +383,19 @@ class _Runtime:
             raise RuntimeError("wavenet_b200: the fused tensor-core block needs R = D = S in (256, 512), kernel_size = 2 "
                                f"(got {R},{D},{S},{k})")
         ctab, frames = None, None
-        if cond is not None or local is not None:
+        if cond is not None or local is not None or upsampled is not None:
             if self.block_mode == "tc" or (self.fast_tf32 and not use_tb):
                 raise RuntimeError("wavenet_b200: a conditioned model runs on the fused tensor-core blocks (block_mode 'tb' / "
                                    "'auto') or the FFMA blocks ('ffma'); the two-launch 'tc' blocks have no conditioned kernel")
             if cond is not None and cond.shape[0] != B:
                 raise RuntimeError(f"wavenet_b200: {cond.shape[0]} condition rows for a batch of {B}")
-            if local is None:
-                ctab = W.cond_table(cond, stream)
+            if upsampled is not None:
+                if tuple(upsampled.shape) != (B, m.local_condition_channels, L):
+                    raise RuntimeError(f"wavenet_b200: upsampled local features of shape {tuple(upsampled.shape)} for a batch of "
+                                       f"{B} x {L} positions")
+                local = (upsampled, 1)
+            if local is None or (upsampled is not None and use_tb):
+                ctab = None if cond is None else W.cond_table(cond, stream)
             else:
                 y, hop = local
                 if y.shape[0] != B or y.shape[2] < -(-L // hop):
@@ -390,7 +408,9 @@ class _Runtime:
                 if local is not None:
                     save["local"] = local
         if use_tb:
-            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save, ctab, frames)
+            if save is not None and upsampled is not None:
+                save["kslab"] = True          # the backward reduces dU and dc on the chunked dfg (wn_local_*_grad*)
+            return self._forward_tb(x, index_input, B, L, plan, out_len, W, stream, save, ctab, frames, upsampled)
         if save is not None:
             h_all = torch.empty(n_layers + 1, B, L, R, **f32)      # h_all[i] = input of layer i
             fg_all = torch.empty(n_layers, B, L, 2 * D, **f32)     # tanh / sigmoid outputs
@@ -469,10 +489,10 @@ class _Runtime:
                         index_input=index_input, B=B, L=L)
         return logits
 
-    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None, ctab=None, frames=None):
+    def _forward_tb(self, x, index_input, B, L, plan, out_len, W, stream, save=None, ctab=None, frames=None, upsampled=None):
         """Forward on the fused tensor-core blocks (wn_tb_block_fwd): chunked bf16-pair activations, one launch per residual
         block, z resident on the SM (csrc/tc_block.cu).  With ``save`` every layer's input pair and tanh/sigmoid outputs are
-        kept for _backward_tb."""
+        kept for _backward_tb.  ``upsampled`` (B, C, L): audio-rate local features, K-slabs of pass A (wn_tb_*_fwd_local)."""
         m, lib = self.model, native.lib()
         dev = self.device()
         R, S, Cc = m.residual_channels, m.skip_channels, m.classes
@@ -504,6 +524,13 @@ class _Runtime:
             native.check(lib.wn_pair_from_frames(frames.data_ptr(), h0.data_ptr(), B, L, R, 0, stream), "pair from frames")
             del frames
         tb_w, tb_b, prec = W["tb"]
+        if upsampled is not None:
+            Cl = m.local_condition_channels
+            cpad = lib.wn_tb_local_padded_channels(Cl, prec)
+            c_pair = torch.empty(B, 2, cpad // 8, L, 8, **bf16)
+            native.check(lib.wn_tb_local_from_channels(upsampled.data_ptr(), c_pair.data_ptr(), B, Cl, L, prec, stream),
+                         "local features to pairs")
+            u_all = W["tb_local"][0]
         ev = getattr(self, "block_events", None)
         if ev is not None:
             ev[0].record(torch.cuda.current_stream(dev))
@@ -527,7 +554,10 @@ class _Runtime:
             sa.d_flags = flags.data_ptr()
             sa.n_layers, sa.channels, sa.precision, sa.B, sa.L, sa.skip_start = n_layers, R, prec, B, L, plan.skip_start
             sa.dilations, sa.in_start, sa.out_start = ints(dil), ints(plan.in_start), outs
-            if ctab is None:
+            if upsampled is not None:
+                native.check(lib.wn_tb_stack_fwd_local(ctypes.byref(sa), native.ptr(ctab), c_pair.data_ptr(), Cl, u_all.data_ptr(),
+                                                       stream), "tb stack")
+            elif ctab is None:
                 native.check(lib.wn_tb_stack_fwd(ctypes.byref(sa), stream), "tb stack")
             elif frames is not None:
                 native.check(lib.wn_tb_stack_fwd_cond_frames(ctypes.byref(sa), ctab.data_ptr(), frames[0], frames[1], stream),
@@ -546,7 +576,10 @@ class _Runtime:
                 a.dilation, a.in_start, a.out_start, a.skip_init = d, plan.in_start[i], plan.out_start[i], int(i == 0)
                 if save is not None:
                     a.d_fg_save = fg_all[i].data_ptr()
-                if ctab is None:
+                if upsampled is not None:
+                    native.check(lib.wn_tb_block_fwd_local(ctypes.byref(a), None if ctab is None else ctab[i].data_ptr(),
+                                                           c_pair.data_ptr(), Cl, u_all.data_ptr(), stream), f"tb block {i}")
+                elif ctab is None:
                     native.check(lib.wn_tb_block_fwd(ctypes.byref(a), stream), f"tb block {i}")
                 elif frames is not None:
                     native.check(lib.wn_tb_block_fwd_cond_frames(ctypes.byref(a), ctab[i].data_ptr(), frames[0], frames[1], stream),
@@ -750,6 +783,20 @@ class _Runtime:
         y, hop = local
         m = self.model
         B, L, D = saved["B"], saved["L"], m.dilation_channels
+        if saved.get("kslab"):
+            # audio-rate features c = y (B, C, L) of the K-slab forward: both contractions read the chunked dfg in place
+            lib, C = native.lib(), y.shape[1]
+            du = torch.empty(2 * D, C, device=y.device, dtype=torch.float32)
+            work = torch.empty(lib.wn_local_weight_grad_workspace_bytes(2 * D, C) // 4, device=y.device, dtype=torch.float32)
+            native.check(lib.wn_local_weight_grad(dfg.data_ptr(), B, L, 2 * D, gz, y.data_ptr(), C, work.data_ptr(),
+                                                  du.data_ptr(), stream), "local weight gradient")
+            gf, gg = du[:D].unsqueeze(-1), du[D:].unsqueeze(-1)
+            grads[f"filter_local_convs.{i}.weight"], grads[f"gate_local_convs.{i}.weight"] = gf, gg
+            if "local_dy" in saved:
+                U = torch.cat([m.filter_local_convs[i].weight.detach(), m.gate_local_convs[i].weight.detach()], 0)[:, :, 0]
+                native.check(lib.wn_local_data_grad_add(dfg.data_ptr(), B, L, 2 * D, gz, U.contiguous().data_ptr(), C,
+                                                        saved["local_dy"].data_ptr(), stream), "local data gradient")
+            return [gf, gg]
         nf = -(-L // hop)
         S = torch.empty(B, nf, 2 * D, device=y.device, dtype=torch.float32)
         native.check(native.lib().wn_cond_segment_sums(dfg.data_ptr(), pair, B, L, 2 * D, gz, hop, nf, S.data_ptr(), stream),
@@ -1106,6 +1153,13 @@ class _Runtime:
         return idx, logits, total_evals
 
 
+def _exact_convolutions():
+    """cuDNN convolutions in full fp32 and deterministic (torch lets them use TF32 by default, ~1e-3 relative): the learned
+    upsampler's output feeds every layer."""
+    return torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=False, deterministic=True,
+                                      allow_tf32=False)
+
+
 class _StackFunction(torch.autograd.Function):
     """forward()/wavenet() as one autograd node: parameters in, logits out; the input carries no gradient."""
 
@@ -1114,10 +1168,22 @@ class _StackFunction(torch.autograd.Function):
         saved = {}
         rt = model._runtime()
         local = None if local_y is None else (local_y.detach(), local_hop)
-        with torch.no_grad(), torch.cuda.device(rt.device()):
-            y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond, local=local)
-        if local is not None and ctx.needs_input_grad[5]:
-            saved["local_dy"] = torch.zeros_like(local[0])          # the backward adds every layer's share
+        ctx.upsampler = None
+        if local is not None and getattr(model, "local_upsample", None) is not None:
+            # the learned upsampler runs inside this node, so that its gradients exist while the backward still averages
+            # gradients across ranks (see backward)
+            with torch.enable_grad():
+                y_in = local[0].requires_grad_(ctx.needs_input_grad[5])
+                c = model._upsample(y_in, x.size(-1))
+            ctx.upsampler = (y_in, c)
+            with torch.no_grad(), torch.cuda.device(rt.device()):
+                y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond, upsampled=c.detach())
+            saved["local_dy"] = torch.zeros_like(c)              # gradient of c: every layer adds its share
+        else:
+            with torch.no_grad(), torch.cuda.device(rt.device()):
+                y = rt.stack_forward(x, out_len, index_input=index_input, save=saved, cond=cond, local=local)
+            if local is not None and ctx.needs_input_grad[5]:
+                saved["local_dy"] = torch.zeros_like(local[0])          # the backward adds every layer's share
         ctx.model, ctx.saved = model, saved
         ctx.names = [n for n, _ in model.named_parameters()]
         return y
@@ -1131,6 +1197,24 @@ class _StackFunction(torch.autograd.Function):
         with torch.no_grad(), torch.cuda.device(rt.device()):
             g = rt.stack_backward(ctx.saved, dlogits)
         dy = ctx.saved.get("local_dy")
+        if ctx.upsampler is not None:
+            # c = upsample(y): its gradient dy comes from dc; the upsampler's parameter gradients are averaged across ranks
+            # like every other parameter's before they reach p.grad
+            y_in, c = ctx.upsampler
+            named = [(f"local_upsample.{n}", p) for n, p in ctx.model.local_upsample.named_parameters() if p.requires_grad]
+            inputs = ([y_in] if y_in.requires_grad else []) + [p for _, p in named]
+            got = []
+            if inputs:
+                with torch.cuda.device(rt.device()), _exact_convolutions():
+                    got = torch.autograd.grad(c, inputs, dy)
+            dy = got[0] if y_in.requires_grad else None
+            ug = got[len(got) - len(named):]
+            g.update(zip([n for n, _ in named], ug))
+            reducer = getattr(rt, "grad_reducer", None)
+            if reducer is not None:
+                reducer.reduce_async(list(ug))
+                reducer.wait_all()
+            ctx.upsampler = None
         ctx.saved = None
         rt.invalidate()          # an optimizer step follows; it may write through p.data, which no version counter sees
         return (None, None, None, None, None, dy, None) + tuple(g.get(n) for n in ctx.names)
@@ -1159,6 +1243,10 @@ class WaveNetModel(nn.Module):
                                     ``local_condition_hop`` samples (repeat upsampling): position t adds Uf y[:, t // hop] /
                                     Ug y[:, t // hop] (``filter_local_convs`` / ``gate_local_convs``, 1x1, no bias)
         local_condition_hop (Int):  samples per frame of the local condition (>= 1; required when C > 0)
+        local_condition_upsample_scales (tuple of Int): a learned upsampler instead of repetition: ``local_upsample[i]`` is a
+                                    ConvTranspose1d(C, C, 2 s_i, stride=s_i) that maps F frames to F * s_i (no nonlinearity
+                                    between stages); the product of the s_i must be the hop.  Initialised to exact repetition.
+                                    Position t then adds Uf c[:, t] / Ug c[:, t], c = the upsampled series.
 
     Shape:
         - Input: (N, classes, L) float32 one-hot, L >= receptive_field + output_length - 1 recommended
@@ -1167,7 +1255,8 @@ class WaveNetModel(nn.Module):
 
     def __init__(self, layers=10, blocks=4, dilation_channels=32, residual_channels=32, skip_channels=256,
                  end_channels=256, classes=256, output_length=32, kernel_size=2, dtype=torch.FloatTensor, bias=False,
-                 condition_channels=0, local_condition_channels=0, local_condition_hop=None):
+                 condition_channels=0, local_condition_channels=0, local_condition_hop=None,
+                 local_condition_upsample_scales=None):
         super(WaveNetModel, self).__init__()
         self.layers = layers
         self.blocks = blocks
@@ -1224,6 +1313,29 @@ class WaveNetModel(nn.Module):
             for _ in range(layers * blocks):
                 self.filter_local_convs.append(nn.Conv1d(local_condition_channels, dilation_channels, 1, bias=False))
                 self.gate_local_convs.append(nn.Conv1d(local_condition_channels, dilation_channels, 1, bias=False))
+        # created after the local ones, for the same reason
+        if local_condition_upsample_scales is not None:
+            scales = local_condition_upsample_scales
+            if local_condition_channels <= 0:
+                raise ValueError("local_condition_upsample_scales needs local_condition_channels > 0")
+            try:
+                scales = tuple(scales)
+            except TypeError:
+                raise ValueError(f"local_condition_upsample_scales must be a sequence of ints >= 1, got {scales!r}") from None
+            if not scales or any(isinstance(s, bool) or not isinstance(s, int) or s < 1 for s in scales):
+                raise ValueError(f"local_condition_upsample_scales must be a sequence of ints >= 1, got {scales!r}")
+            if math.prod(scales) != local_condition_hop:
+                raise ValueError(f"the product of local_condition_upsample_scales {scales} must equal local_condition_hop "
+                                 f"{local_condition_hop}")
+            C = local_condition_channels
+            self.local_condition_upsample_scales = scales
+            self.local_upsample = nn.ModuleList(nn.ConvTranspose1d(C, C, 2 * s, stride=s) for s in scales)
+            with torch.no_grad():                   # exact repetition: stage i copies frame f to positions [f s, (f + 1) s)
+                for conv, s in zip(self.local_upsample, scales):
+                    conv.weight.zero_()
+                    conv.bias.zero_()
+                    for c in range(C):
+                        conv.weight[c, c, s // 2:s // 2 + s] = 1.0
 
         self.output_length = output_length
         self.receptive_field = receptive_field
@@ -1330,6 +1442,17 @@ class WaveNetModel(nn.Module):
             y = y.detach()
         return y.to(self._runtime().device(), torch.float32).contiguous()
 
+    def _upsample(self, y, positions):
+        """The learned upsampler: (N, C, F) frame-rate series -> (N, C, positions) contiguous audio-rate features c.  Stage i
+        maps F frames to (F + 1) s_i and keeps [s_i // 2, s_i // 2 + F s_i), so c has F * hop positions before the crop and
+        position t is still "frame t // hop"."""
+        c = y
+        with _exact_convolutions():
+            for conv in self.local_upsample:
+                s, n = conv.stride[0], c.shape[2]
+                c = conv(c)[:, :, s // 2:s // 2 + n * s]
+        return c[:, :, :positions].contiguous()
+
     def _stack(self, input, out_len, index_input=False, condition=None, local_condition=None):
         cond = self._condition(condition, input.size(0))
         y = self._local_condition(local_condition, input.size(0), input.size(-1))
@@ -1340,6 +1463,9 @@ class WaveNetModel(nn.Module):
             return _StackFunction.apply(self, input, out_len, index_input, cond, y, hop, *self.parameters())
         rt = self._runtime()
         with torch.cuda.device(rt.device()):       # native launches go to the CURRENT device: make it the model's
+            if y is not None and getattr(self, "local_upsample", None) is not None:
+                return rt.stack_forward(input, out_len, index_input=index_input, cond=cond,
+                                        upsampled=self._upsample(y, input.size(-1)))
             return rt.stack_forward(input, out_len, index_input=index_input, cond=cond,
                                     local=None if y is None else (y, hop))
 
@@ -1421,7 +1547,8 @@ class WaveNetModel(nn.Module):
                                 bias=self.start_conv.bias is not None,
                                 condition_channels=getattr(self, "condition_channels", 0),
                                 local_condition_channels=getattr(self, "local_condition_channels", 0),
-                                local_condition_hop=getattr(self, "local_condition_hop", None))
+                                local_condition_hop=getattr(self, "local_condition_hop", None),
+                                local_condition_upsample_scales=getattr(self, "local_condition_upsample_scales", None))
             twin.load_state_dict(self.state_dict())
             sh = (key, twin.cuda())
             self.__dict__["_shadow"] = sh
@@ -1457,7 +1584,8 @@ class WaveNetModel(nn.Module):
         num_given = first.shape[0]
         if local_condition is not None:
             local_condition = local_condition[None] if torch.is_tensor(local_condition) else np.asarray(local_condition)[None]
-        local = self._local_condition(local_condition, 1, num_given - 1 + num_samples)
+        local = self._sampler_local(self._local_condition(local_condition, 1, num_given - 1 + num_samples),
+                                    num_given - 1 + num_samples)
         self.eval()
         total = num_given + num_samples
         callbacks = []
@@ -1471,7 +1599,7 @@ class WaveNetModel(nn.Module):
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond,
-                                    local=None if local is None else (local.detach(), self.local_condition_hop))
+                                    local=local)
         self._export_queues()
         self.train()
         generated = (idx[0] / self.classes) * 2. - 1
@@ -1489,16 +1617,26 @@ class WaveNetModel(nn.Module):
         first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
         first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
         cond = self._condition(condition, first.shape[0])
-        local = self._local_condition(local_condition, first.shape[0], first.shape[1] - 1 + num_samples)
+        local = self._sampler_local(self._local_condition(local_condition, first.shape[0], first.shape[1] - 1 + num_samples),
+                                    first.shape[1] - 1 + num_samples)
         self.eval()
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, logits, _ = rt.generate(num_samples, first, temperature, regularize, uniforms=uniforms,
-                                         forced=forced, want_logits=return_logits, cond=cond,
-                                         local=None if local is None else (local.detach(), self.local_condition_hop))
+                                         forced=forced, want_logits=return_logits, cond=cond, local=local)
         self._export_queues()
         self.train()
         return (idx, logits) if return_logits else idx
+
+    def _sampler_local(self, y, evals):
+        """The sampler's (series, hop) for the validated frame-rate series ``y`` (None: no local conditioning).  A learned
+        upsampler runs once here, and the sampler reads its output at hop 1 (one table row per evaluation)."""
+        if y is None:
+            return None
+        if getattr(self, "local_upsample", None) is None:
+            return y.detach(), self.local_condition_hop
+        with torch.no_grad(), torch.cuda.device(self._runtime().device()):
+            return self._upsample(y.detach(), evals), 1
 
     def _export_queues(self):
         """Point ``dilated_queues[i].data`` at stream 0 of the sampler's device rings (a (C, max_length) view).
