@@ -190,7 +190,9 @@ def test_fast_kernel_equals_generic_kernel_bitwise(golden):
 def test_two_level_exchange_kernel_bitwise_and_golden(golden):
     """cfg 2 net, single stream: the two-level exchange kernel (mode 5: DSMEM inside a cluster, one L2 poller per remote
     producer) keeps kernel 3's row split and summation order -- logits and indices identical bit for bit, over warm-up
-    samples, sampling with temperature, chunked launches that continue a session, and the golden teacher-forced stream."""
+    samples, sampling with temperature, chunked launches that continue a session, and the golden teacher-forced stream.
+    The golden stream is 48 evaluations from reset rings (the receptive field is 5 116, so every layer of dilation >= 64
+    reads a zero history); runs past the receptive field against a reference are in test_gpu_generate_long.py."""
     g = golden("net_cfg2.npz")
     m = build_model(g)
     rt = m._runtime()
@@ -219,8 +221,9 @@ def test_two_level_exchange_kernel_bitwise_and_golden(golden):
 
 
 def test_cluster_kernel_cfg2(golden):
-    """The cluster (distributed shared memory) kernel is what a 256-channel net runs by default: golden parity,
-    agreement with the L2 kernels, and multi-stream == single-stream bit for bit (one cluster per stream)."""
+    """The cluster (distributed shared memory) kernel, one 16-CTA cluster per stream of a 256-channel net: golden parity
+    over 48 evaluations from reset rings (a hundredth of the receptive field; test_gpu_generate_long.py has the long
+    runs), agreement with the L2 kernels over 60, and multi-stream == single-stream bit for bit."""
     g = golden("net_cfg2.npz")
     m = build_model(g)
     rt = m._runtime()
@@ -257,8 +260,10 @@ def test_cluster_kernel_cfg2(golden):
 def test_batched_cluster_kernel_cfg2(golden):
     """The batched tensor-core cluster kernel (mode 6: 8 streams per 16-CTA cluster, bf16 hi/lo pair MMAs, bulk-copy
     exchange) is what several streams of a 256-channel net run by default.  A stream's result does not depend on its
-    slot, its cluster or its company (bitwise); logits follow the reference's golden stream and the fp32 L2 kernel;
-    launches that continue a session reproduce the single launch."""
+    slot, its cluster or its company (bitwise); logits follow the reference's golden stream (48 evaluations from reset
+    rings, a hundredth of the receptive field) and the fp32 L2 kernel (68); launches that continue a session reproduce
+    the single launch (700 evaluations, kernel against itself).  test_gpu_generate_long.py has the long runs against a
+    reference."""
     g = golden("net_cfg2.npz")
     m = build_model(g)
     rt = m._runtime()
