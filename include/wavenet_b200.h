@@ -390,7 +390,10 @@ int wn_tc_wgrad(const wn_wgrad_args* a, void* stream);
  *   x_i[target_i]), d_dlogits = (softmax(x_i) - onehot(target_i)) / N (may not alias d_logits); deterministic; *d_err
  *   (optional) is set when a target is outside [0, C).  d_work: wn_ce_workspace_bytes().  C <= 1024.
  * wn_adam_step: torch.optim.Adam's update (the reference's default optimizer, :24) of every tensor in one launch.  d_segs
- *   is a DEVICE array of segments, d_chunks a DEVICE array of (segment, chunk-of-4096) int pairs covering them.
+ *   is a DEVICE array of segments, d_chunks a DEVICE array of (segment, chunk-of-4096) int pairs covering them.  All of
+ *   them take the same `step` (1-based; each tensor's own count in torch.optim.Adam).  wn_adam_step_f64 takes the
+ *   coefficients as double, as torch does (1 - beta2 and the bias corrections are formed in double and rounded once);
+ *   wn_adam_step converts its float arguments and calls it, so 1 - 0.999f is 1.3e-5 away from 1 - 0.999.
  * wn_scatter_rows: start_conv gradient for index input: table (classes, R) = sum over frames t >= t_begin of dh[b][t][:]
  *   into row idx[b][t] (idx uint8 or int64, (B, L)), optionally also transposed into d_out_t (R, classes) = the layout of
  *   start_conv.weight; wn_colsum: out[c] = sum_r x[r][c] (bias gradients), d_work
@@ -401,6 +404,8 @@ int    wn_ce_fwd_bwd(const float* d_logits, const int64_t* d_target, float* d_dl
 typedef struct wn_adam_seg { float* p; const float* g; float* m; float* v; long long n; } wn_adam_seg;
 int    wn_adam_step(const wn_adam_seg* d_segs, const int* d_chunks, int n_chunks, float lr, float beta1, float beta2, float eps,
                     float weight_decay, int step, void* stream);
+int    wn_adam_step_f64(const wn_adam_seg* d_segs, const int* d_chunks, int n_chunks, double lr, double beta1, double beta2,
+                        double eps, double weight_decay, int step, void* stream);
 int    wn_scatter_rows(const void* d_idx, int idx_is_u8, const float* d_dh, float* d_table, float* d_out_t, int B, int L, int R,
                        int classes, int t_begin, void* stream);
 size_t wn_colsum_workspace_bytes(long long rows, int C);

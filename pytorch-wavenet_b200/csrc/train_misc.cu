@@ -57,7 +57,9 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, const long long* __restrict_
             const int c = lane + 32 * i;
             if (c < C) d[c] = (v[i] * inv - (c == (int)tg ? 1.f : 0.f)) * inv_n;
         }
-        if (lane == 0) my_loss += logf(s) + mx - x[tg];
+        // mx - x[tg] first: it is exact for logits of one sign within a factor of two of each other, where logf(s) + mx
+        // would round at the ulp of the largest logit (5e-4 at logits near 1e4)
+        if (lane == 0) my_loss += logf(s) + (mx - x[tg]);
     }
     if (lane == 0) wsum[warp] = my_loss;
     __syncthreads();
@@ -79,22 +81,22 @@ __global__ void ce_finish_kernel(const float* __restrict__ part, int n, float in
 struct AdamSeg { float* p; const float* g; float* m; float* v; long long n; };
 constexpr int ADAM_CHUNK = 4096;
 __global__ void __launch_bounds__(256)
-adam_kernel(const AdamSeg* __restrict__ segs, const int2* __restrict__ chunks, int n_chunks, float lr, float b1, float b2, float eps,
-            float wd, float bc1, float bc2_sqrt) {
+adam_kernel(const AdamSeg* __restrict__ segs, const int2* __restrict__ chunks, int n_chunks, float step_size, float omb1, float b2,
+            float omb2, float eps, float wd, float bc2_sqrt) {
+    // coefficients come rounded once from double: omb1 = 1 - beta1, omb2 = 1 - beta2, step_size = lr / (1 - beta1^step)
     const int ci = blockIdx.x;
     if (ci >= n_chunks) return;
     const int2 ck = chunks[ci];                         // (segment, first element / ADAM_CHUNK)
     const AdamSeg s = segs[ck.x];
     const long long base = (long long)ck.y * ADAM_CHUNK;
-    const float step_size = lr / bc1;
     for (int i = threadIdx.x; i < ADAM_CHUNK; i += 256) {
         const long long e = base + i;
         if (e >= s.n) break;
         float g = s.g[e];
         const float p = s.p[e];
         if (wd != 0.f) g = fmaf(wd, p, g);
-        const float m = fmaf(1.f - b1, g - s.m[e], s.m[e]);                 // m + (1 - b1)(g - m) == lerp, as torch does
-        const float v = fmaf(1.f - b2, g * g, b2 * s.v[e]);
+        const float m = fmaf(omb1, g - s.m[e], s.m[e]);                     // m + (1 - b1)(g - m) == lerp, as torch does
+        const float v = fmaf(omb2, g * g, b2 * s.v[e]);
         s.m[e] = m;
         s.v[e] = v;
         const float denom = sqrtf(v) / bc2_sqrt + eps;
@@ -189,14 +191,22 @@ extern "C" int wn_ce_fwd_bwd(const float* d_logits, const int64_t* d_target, flo
     return 0;
 }
 
-extern "C" int wn_adam_step(const wn_adam_seg* d_segs, const int* d_chunks, int n_chunks, float lr, float beta1, float beta2, float eps,
-                            float weight_decay, int step, void* stream) {
+extern "C" int wn_adam_step_f64(const wn_adam_seg* d_segs, const int* d_chunks, int n_chunks, double lr, double beta1, double beta2,
+                                double eps, double weight_decay, int step, void* stream) {
     WN_REQUIRE(d_segs && d_chunks && n_chunks > 0 && step >= 1, WN_E_BADARG, "wn_adam_step: bad arguments");
-    const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-    misc::adam_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>((const misc::AdamSeg*)d_segs, (const int2*)d_chunks, n_chunks, lr, beta1,
-                                                                   beta2, eps, weight_decay, bc1, sqrtf(bc2));
+    // torch.optim.Adam forms these in double (Python floats); 1 - beta2 from a float beta2 = 0.999f would be 1.3e-5 off
+    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+    misc::adam_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>((const misc::AdamSeg*)d_segs, (const int2*)d_chunks, n_chunks,
+                                                                   (float)(lr / bc1), (float)(1.0 - beta1), (float)beta2,
+                                                                   (float)(1.0 - beta2), (float)eps, (float)weight_decay,
+                                                                   (float)sqrt(bc2));
     WN_CUDA(cudaGetLastError());
     return 0;
+}
+
+extern "C" int wn_adam_step(const wn_adam_seg* d_segs, const int* d_chunks, int n_chunks, float lr, float beta1, float beta2, float eps,
+                            float weight_decay, int step, void* stream) {
+    return wn_adam_step_f64(d_segs, d_chunks, n_chunks, lr, beta1, beta2, eps, weight_decay, step, stream);
 }
 
 extern "C" int wn_scatter_rows(const void* d_idx, int idx_is_u8, const float* d_dh, float* d_table, float* d_out_t, int B, int L, int R,

@@ -191,6 +191,7 @@ SIGNATURES = {
     "wn_ce_workspace_bytes": (C.c_size_t, []),
     "wn_ce_fwd_bwd": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 2 + [C.c_void_p]),
     "wn_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_float] * 5 + [C.c_int, C.c_void_p]),
+    "wn_adam_step_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_double] * 5 + [C.c_int, C.c_void_p]),
     "wn_scatter_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p]),
 
     "wn_colsum_workspace_bytes": (C.c_size_t, [C.c_longlong, C.c_int]),

@@ -67,18 +67,23 @@ def fused_cross_entropy(logits, target):
 
 
 class FusedAdam(torch.optim.Optimizer):
-    """torch.optim.Adam (no amsgrad, L2 weight decay) with ONE native launch per step for all parameter tensors."""
+    """torch.optim.Adam (no amsgrad, L2 weight decay) with ONE native launch per step for all parameter tensors.
+
+    As in torch, each parameter keeps its own step count (``state[p]["step"]``), which advances only on steps where the
+    parameter has a gradient; parameters whose counts differ are updated by one launch per distinct count."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, model=None):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self._model = model              # its packed weight copies are invalidated after every step
         self._tables = {}
 
-    def _table(self, gi, params):
+    def _table(self, params):
         key = tuple((p.data_ptr(), p.grad.data_ptr(), p.numel()) for p in params)
-        t = self._tables.get(gi)
-        if t is not None and t["key"] == key:
+        t = self._tables.get(key)
+        if t is not None:
             return t
+        if len(self._tables) >= 16:      # parameter sets come and go (gradients that are None on some steps): keep a few
+            self._tables.clear()
         dev = params[0].device
         segs, chunks = np.zeros((len(params), 5), dtype=np.int64), []
         for i, p in enumerate(params):
@@ -87,9 +92,9 @@ class FusedAdam(torch.optim.Optimizer):
                 st["exp_avg"], st["exp_avg_sq"] = torch.zeros_like(p), torch.zeros_like(p)
             segs[i] = (p.data_ptr(), p.grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), p.numel())
             chunks += [(i, c) for c in range((p.numel() + 4095) // 4096)]
-        t = dict(key=key, segs=torch.from_numpy(segs).to(dev), n_chunks=len(chunks),
+        t = dict(segs=torch.from_numpy(segs).to(dev), n_chunks=len(chunks),
                  chunks=torch.tensor(chunks, dtype=torch.int32, device=dev).contiguous())
-        self._tables[gi] = t
+        self._tables[key] = t
         return t
 
     @torch.no_grad()
@@ -103,14 +108,19 @@ class FusedAdam(torch.optim.Optimizer):
             for p in params:
                 if p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous() or p.device.type != "cuda":
                     raise RuntimeError("FusedAdam handles contiguous float32 CUDA parameters")
-            group["step"] = group.get("step", 0) + 1
-            t = self._table(gi, params)
+            by_step = {}
+            for p in params:
+                st = self.state[p]
+                st["step"] = int(st.get("step", 0)) + 1
+                by_step.setdefault(st["step"], []).append(p)
             dev = params[0].device
-            with torch.cuda.device(dev):
-                native.check(lib.wn_adam_step(t["segs"].data_ptr(), t["chunks"].data_ptr(), t["n_chunks"], float(group["lr"]),
-                                              float(group["betas"][0]), float(group["betas"][1]), float(group["eps"]),
-                                              float(group["weight_decay"]), int(group["step"]),
-                                              torch.cuda.current_stream(dev).cuda_stream), "adam step")
+            for step, ps in by_step.items():
+                t = self._table(ps)
+                with torch.cuda.device(dev):
+                    native.check(lib.wn_adam_step_f64(t["segs"].data_ptr(), t["chunks"].data_ptr(), t["n_chunks"],
+                                                      float(group["lr"]), float(group["betas"][0]), float(group["betas"][1]),
+                                                      float(group["eps"]), float(group["weight_decay"]), step,
+                                                      torch.cuda.current_stream(dev).cuda_stream), "adam step")
         if self._model is not None:
             self._model.invalidate_packed_weights()        # the kernel wrote the parameters behind autograd's version counters
         return loss

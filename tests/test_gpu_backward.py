@@ -56,6 +56,47 @@ def test_gradients_match_oracle_autograd(golden, name, out_len):
     assert rel_err(m.end_conv_2.weight.grad.cpu().numpy(), 2 * want["end_conv_2.weight"].numpy()) < TOL
 
 
+@pytest.mark.parametrize("classes", [100, 257, 1000])
+@pytest.mark.parametrize("mode", ["ffma", "tb"])
+def test_gradients_at_other_class_counts(classes, mode):
+    """Class counts other than 256 through the whole training path -- index start conv (uint8 up to 256 classes, int64
+    above), the head's ragged logits and dlogits, fused_cross_entropy and the start-conv scatter -- on the FFMA blocks and
+    on the fused 256-wide tensor-core blocks, against float64 autograd over the oracle."""
+    import wavenet_model as wmod
+    import wavenet_training as wt
+    from helpers import separate_head_relu_ties
+    C = 256 if mode == "tb" else 24
+    kw = dict(layers=3, blocks=1, dilation_channels=C, residual_channels=C, skip_channels=C, end_channels=72, classes=classes,
+              output_length=40, kernel_size=2, bias=True)
+    spec = O.NetSpec(**kw)
+    torch.manual_seed(classes)
+    m = wmod.WaveNetModel(**kw)
+    B, L = 2, spec.receptive_field + spec.output_length - 1 + 30
+    g = torch.Generator().manual_seed(classes + 1)
+    idx = torch.randint(0, classes, (B, L), generator=g)
+    idx[0, -1], idx[1, -2] = classes - 1, 0
+    target = torch.randint(0, classes, (B * spec.output_length,), generator=g)
+    x = O.one_hot(idx, classes)
+    p = separate_head_relu_ties({k: v.detach() for k, v in m.state_dict().items()}, spec, x, spec.output_length)
+    m.load_state_dict(p)
+    pd = {k: v.double().requires_grad_(True) for k, v in p.items()}
+    want_loss = F.cross_entropy(O.forward_direct(pd, spec, x.double()), target)
+    want_loss.backward()
+    m = m.cuda()
+    rt = m._runtime()
+    rt.block_mode = "ffma" if mode == "ffma" else "auto"
+    xi = idx.to(torch.uint8 if classes <= 256 else torch.int64).cuda()
+    loss = wt.fused_cross_entropy(m.forward_indices(xi), target.cuda())
+    loss.backward()
+    assert rt.last_block_mode == mode
+    assert abs(float(loss) - float(want_loss)) < 1e-5 * float(want_loss)
+    for k, v in m.named_parameters():
+        if pd[k].grad is None:              # the last block's residual conv does not reach the loss
+            assert float(v.grad.abs().max()) == 0.0, k
+            continue
+        assert rel_err(v.grad.cpu().numpy(), pd[k].grad.numpy()) < TOL, k
+
+
 def test_training_step_reduces_loss(golden):
     """A few SGD steps on a fixed batch through the CUDA forward+backward lower the loss (wavenet_training.py:64-76)."""
     g = golden("net_deep.npz")

@@ -55,15 +55,22 @@ def test_forward_snapshot_real_audio(golden):
                  kernel_size=3, bias=True, output_length=9)),
     (2, 140, dict(layers=2, blocks=2, dilation_channels=130, residual_channels=4, skip_channels=260, end_channels=132,
                   kernel_size=2, bias=True, output_length=64)),
+    (2, 150, dict(layers=3, blocks=2, dilation_channels=24, residual_channels=20, skip_channels=36, end_channels=28,
+                  classes=11, kernel_size=2, bias=True, output_length=33)),
+    (1, 200, dict(layers=4, blocks=1, dilation_channels=32, residual_channels=32, skip_channels=64, end_channels=48,
+                  classes=257, kernel_size=3, bias=True, output_length=129)),
+    (3, 100, dict(layers=3, blocks=1, dilation_channels=16, residual_channels=16, skip_channels=40, end_channels=1000,
+                  classes=1000, kernel_size=2, bias=False, output_length=50)),
 ])
 def test_forward_matches_oracle_random_nets(B, L, kw):
-    """Seeded random nets incl. ragged channel counts, k=3, dense (non one-hot) input."""
+    """Seeded random nets incl. ragged channel and class counts, k=3, dense (non one-hot) input."""
     import wavenet_model as wmod
     torch.manual_seed(3)
     m = wmod.WaveNetModel(**kw)
     spec = O.NetSpec(**kw)
     p = {k: v.detach().clone() for k, v in m.state_dict().items()}
-    x = torch.rand(B, 256, L) * (torch.rand(B, 256, L) < 0.05)       # sparse dense input, not one-hot
+    C = spec.classes
+    x = torch.rand(B, C, L) * (torch.rand(B, C, L) < 0.05)           # sparse dense input, not one-hot
     with torch.no_grad():
         want = O.forward(p, spec, x).numpy()
         want_direct = O.forward_direct(p, spec, x).numpy()

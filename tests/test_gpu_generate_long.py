@@ -168,20 +168,38 @@ def test_many_streams_two_laps_deep(golden, ns):
 
 
 # ---------------------------------------------------------------------------------------------- e. generic kernels, odd shapes
-@pytest.mark.parametrize("name", ["k3", "odd_bias", "deep"])
+_class_models = {}
+
+
+def _class_model(name):
+    """seeded nets with class counts other than 256 ("c100", "c257", "c1000"): ragged channels, biases everywhere"""
+    if name not in _class_models:
+        import wavenet_model as wmod
+        with torch.random.fork_rng(devices=[]):
+            torch.manual_seed(int(name[1:]))
+            _class_models[name] = wmod.WaveNetModel(layers=4, blocks=2, dilation_channels=24, residual_channels=20,
+                                                    skip_channels=40, end_channels=72, classes=int(name[1:]),
+                                                    output_length=8, kernel_size=2, bias=True).cuda()
+    return _class_models[name]
+
+
+@pytest.mark.parametrize("name", ["k3", "odd_bias", "deep", "c100", "c257", "c1000"])
 def test_generic_kernels_on_odd_shapes(golden, name):
     """kernel_size 3 (rings of 2 dil + 1 slots, two history taps), biases on every convolution with ragged channel
-    counts, and a deeper net: 3 streams, three receptive fields from one given sample.  With biases a reset queue (zeros)
-    is not the layers' response to silence; the reference models the queue."""
-    g = golden(f"net_{name}.npz")
-    m = build_model(g)
+    counts, a deeper net, and class counts other than 256 (the selection step with idle lanes and with more than 8
+    classes per lane): 3 streams, three receptive fields from one given sample.  With biases a reset queue (zeros) is not
+    the layers' response to silence; the reference models the queue.  On the class-count nets each of modes 1 to 4 either
+    runs its kernel or refuses the shape, and kernels 1 and 2 must run."""
+    m = _class_model(name) if name[0] == "c" else build_model(golden(f"net_{name}.npz"))
+    C = m.classes
     dil = [d for d, _ in m.dilations]
     n = 3 * m.receptive_field
     rng = np.random.RandomState(105)
-    first, forced = rng.randint(0, 256, (3, 1)), rng.randint(0, 256, (3, n))
+    first, forced = rng.randint(0, C, (3, 1)), rng.randint(0, C, (3, n))
+    forced[:, 7], forced[:, 8] = 0, C - 1
     want = np.stack([_ref(name, m, dil, R.inputs(first[s], forced[s])) for s in range(3)])
     ran = []
-    for mode in (None, 1, 2, 4):
+    for mode in ((1, 2, 3, 4) if name[0] == "c" else (None, 1, 2, 4)):
         for ns in (1, 3):
             m._runtime().gen_mode = mode
             try:
@@ -196,6 +214,8 @@ def test_generic_kernels_on_odd_shapes(golden, name):
             assert np.array_equal(idx, lg.argmax(axis=2))
     m._runtime().gen_mode = None
     assert 1 in ran and len(set(ran)) >= 2, ran
+    if name[0] == "c":
+        assert {1, 2} <= set(ran), ran
 
 
 # ---------------------------------------------------------------------------------------------- f. conditioned
@@ -279,7 +299,7 @@ def _selection(tag, m, name, dil, mode, ns, n, ref_streams):
     rt = m._runtime()
     rt.gen_mode = mode
     rng = np.random.RandomState(107)
-    first = rng.randint(0, 256, (ns, 1))
+    first = rng.randint(0, m.classes, (ns, 1))
     for temperature, regularize in SETTINGS:
         uni = _uniforms(rng, ns, n)
         idx, lg = m.generate_fast_batch(n, first, temperature=temperature, regularize=regularize, uniforms=uni,
@@ -294,7 +314,7 @@ def _selection(tag, m, name, dil, mode, ns, n, ref_streams):
             bad += int(((got != idx[s]) & ~near).sum())
             close += int(((got != idx[s]) & near).sum())
         assert bad == 0 and close < 0.01 * ns * n, (tag, temperature, regularize, bad, close)
-        reg = R.regularizer(256, regularize).astype(np.float64)
+        reg = R.regularizer(m.classes, regularize).astype(np.float64)
         want = np.stack([_ref(name, m, dil, R.inputs(first[s], idx[s])) for s in ref_streams])
         whole, last = _errs(f"g {tag} T={temperature} reg={regularize}", kid, cs, ns, n, lg[ref_streams] + reg, want)
         print(f"    {ns * n} selections, {close} within rounding of an edge, {len(np.unique(idx))} distinct classes chosen")
@@ -310,3 +330,11 @@ def test_selection_thousands_of_times_cfg2(golden, mode, ns):
 def test_selection_thousands_of_times_odd_bias(golden):
     m = build_model(golden("net_odd_bias.npz"))
     _selection("odd_bias mode 2", m, "odd_bias", [d for d, _ in m.dilations], 2, 1, 4000, [0])
+
+
+@pytest.mark.parametrize("name", ["c100", "c1000"])
+def test_selection_at_other_class_counts(name):
+    """the selection step with idle lanes (100 classes) and with more than 8 classes per lane (1 000), free running at
+    every setting (temperature 1 included) with uniforms at 0 and at 1 - 2^-53"""
+    m = _class_model(name)
+    _selection(f"{name} mode 2", m, name, [d for d, _ in m.dilations], 2, 1, 3000, [0])

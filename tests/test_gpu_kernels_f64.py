@@ -10,7 +10,7 @@ Bars follow from the operand widths (block_ref's emulation of exactly these inpu
     single-pass bf16 also   rel_err(kernel, emulated) <= 0.25 e_emu   (a wrong operand plane or a dropped term fails this)
     FFMA kernels            rel_err(kernel, exact) <= 1e-5;   single TF32 pass: <= 2e-2 (hardware truncation not emulated)
 acc(K) = 2^-16 sqrt(K / 256) allows for the tensor cores' fp32 accumulation over a contraction of length K, which the
-emulation (float64 sums) leaves out; see _acc.
+emulation (float64 sums) leaves out; see helpers.tc_acc.
 rel_err is max|a - b| / max|b| per output tensor (per tap for weight gradients).  Every measured value is printed (-s)."""
 import ctypes
 import functools
@@ -19,63 +19,10 @@ import pytest
 import torch
 
 import block_ref as BR
+from helpers import kernel_rel as _rel, kernel_check as _check, kernel_miss as _miss
 
 pytestmark = pytest.mark.gpu
 TB_PRECS = [("pairs", 256), ("bf16", 256), ("bf16", 512)]
-
-
-def _rel(a, b):
-    a, b = torch.as_tensor(a).double(), torch.as_tensor(b).double()
-    return float((a - b).abs().max() / max(float(b.abs().max()), 1e-30))
-
-
-def _acc(K):
-    """Allowance for the fp32 accumulation of a K-long contraction on the tensor cores, which the float64 emulation does not
-    model: measured on an H100 it reaches ~1e-5 (max-relative) at K = 512 and grows with K, also where the operand error
-    is tiny (3xTF32: e_emu ~ 1e-7), while spread over all frames and channels rather than on a range boundary.
-
-    What the bar then still catches, per output tensor (~4e-5 to 7e-5 for the K of these tests): any frame-range, tap,
-    tile, plane or bias error (the controls miss by 10^3 or more); for bf16 pairs, a dropped lo-plane product of either
-    operand (the operand-term controls of test_two_launch_and_ffma_block_fwd); single-pass bf16 against its own emulation
-    at 0.25 e_emu.  What it cannot catch: an error below about 2^-16 of the output scale -- one missing lo-plane product on
-    a single k-slab, or for 3xTF32 a dropped tf32 lo plane altogether (~2^-12 per operand); the 50-layer model tests of
-    test_gpu_tc.py carry that case."""
-    return 2.0 ** -16 * (max(K, 256) / 256) ** 0.5
-
-
-def _worst(got, exact):
-    """(index, |error|) of the worst element, to localize a failure (frame axis = dim 1 of the frames layouts)"""
-    diff = (torch.as_tensor(got).double() - torch.as_tensor(exact).double()).abs()
-    i = int(diff.argmax())
-    return tuple(int(v) for v in torch.unravel_index(torch.tensor(i), diff.shape)), float(diff.flatten()[i])
-
-
-def _check(what, got, exact, emu=None, kind="emu", K=256):
-    """Assert the bar of `kind` ("emu": operand-split kernels, "bf16": single pass, "ffma", "tf32x1"); returns the bar.
-    K: the longest contraction feeding the output (sets the accumulation allowance of the tensor-core kernels)."""
-    e = _rel(got, exact)
-    if kind == "ffma":
-        bar, msg = 1e-5, ""
-    elif kind == "tf32x1":
-        bar, msg = 2e-2, ""
-    else:
-        e_emu = _rel(emu, exact)
-        bar, msg = 2 * e_emu + _acc(K), f" e_emu {e_emu:.2e}"
-        if kind == "bf16":
-            e_ke = _rel(got, emu)
-            msg += f" vs-emulation {e_ke:.2e} (bar {0.25 * e_emu:.2e})"
-            assert e_ke <= 0.25 * e_emu, f"{what}: kernel vs emulated operands {e_ke:.3e} > {0.25 * e_emu:.3e}"
-    idx, ad = _worst(got, exact)
-    print(f"  {what}: rel_err {e:.2e} bar {bar:.2e}{msg} worst at {idx}")
-    assert e <= bar, f"{what}: rel_err {e:.3e} > bar {bar:.3e} (worst element {idx}, |error| {ad:.3e})"
-    return bar
-
-
-def _miss(what, got, wrong, bar, factor=10):
-    """negative control: a reference with one deliberate mistake must be missed by >= factor x the bar"""
-    e = _rel(got, wrong)
-    print(f"  control {what}: rel_err {e:.2e} = {e / bar:.1f}x bar")
-    assert e >= factor * bar, f"control {what}: only {e:.3e} from a wrong reference (bar {bar:.3e})"
 
 
 def _sentinel_kept(what, t, lo):
