@@ -167,6 +167,26 @@ def block_forward(h, W, d, in_start, out_start, skip_start, skip=None, mode="exa
                 z=value(store(z, mode, False)), skip=value(store(sk, mode, False)))
 
 
+def expand_table(table, L, hop=None):
+    """A condition table on the positions [0, L), float64 (B, L, 2D): a global table (B, 2D) gives every position its
+    sequence's row; a frames table (B, F, 2D) gives position t frame t // hop."""
+    t = table.double()
+    if t.dim() == 2:
+        return t[:, None].expand(-1, L, -1)
+    return t[:, torch.arange(L) // hop]
+
+
+def with_position_biases(W, pre, out_start, keep_bias=False):
+    """W with per-position filter / gate biases on the block's output frames [out_start, L): pre (B, L, 2D) on the absolute
+    axis, [filter | gate].  They replace bf / bg (a condition table already holds the biases) or, with keep_bias, add to them."""
+    D = W["wf"].shape[0]
+    p = pre[:, out_start:].double()
+    Wm = dict(W)
+    Wm["bf"] = p[..., :D] + (_b(W, "bf") if keep_bias else 0.0)
+    Wm["bg"] = p[..., D:] + (_b(W, "bg") if keep_bias else 0.0)
+    return Wm
+
+
 def backward_ranges(L, k, d, in_start, out_start, gs_out, ds_start):
     """gz, id_start, gs_in of one block as the runtime derives them (wavenet_model._Runtime._backward_tb)"""
     gz = max(out_start, min(gs_out, ds_start))

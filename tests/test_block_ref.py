@@ -129,6 +129,62 @@ def test_block_reference_range_rules_are_tight():
     assert _rel(BR.block_forward(garbage, W, d, in_s - 1, out_s, out_s)["h_out"], ok) > 1e-3
 
 
+@pytest.mark.parametrize("term", ["global", "frames", "frames+global", "kslab", "kslab+global"])
+def test_position_biases_compose_to_the_conditioned_references(term):
+    """The whole-stack kernel tests (test_gpu_stack_kernels_f64.py) give block_forward each conditioned layer's term as
+    per-position filter / gate biases: a global or frames condition table replacing bf / bg (expand_table), or the K-slab
+    product U c[t] on top of the biases or of the global table.  Composed over a small net, that must reproduce the skip
+    sum of local_ref.stack_direct / upsample_ref.stack_direct."""
+    import local_ref
+    import upsample_ref
+    torch.set_num_threads(min(8, torch.get_num_threads()))
+    spec = O.NetSpec(layers=3, blocks=2, dilation_channels=6, residual_channels=6, skip_channels=6, end_channels=9,
+                     classes=11, output_length=9, kernel_size=2, bias=True)
+    p = {n: v.double() for n, v in O.init_params(spec, seed=9).items()}
+    g = torch.Generator().manual_seed(10)
+    rnd = lambda *s: torch.randn(*s, generator=g, dtype=torch.float64) * 0.5
+    B, L, G, C, hop, D = 2, 70, 3, 4, 5, spec.dilation_channels
+    dil = [d for d, _ in spec.dilation_schedule()]
+    for i in range(len(dil)):
+        for n in ("filter", "gate"):
+            p[f"{n}_cond_convs.{i}.weight"], p[f"{n}_local_convs.{i}.weight"] = rnd(D, G, 1), rnd(D, C, 1)
+    p["local_upsample.0.weight"], p["local_upsample.0.bias"] = rnd(C, C, 2 * hop), rnd(C)
+    x = torch.randn(B, spec.classes, L, generator=g, dtype=torch.float64)
+    h = rnd(B, G) if "global" in term else None
+    y = rnd(B, C, -(-L // hop) + 2)
+    taps = {}
+    if term.startswith("kslab"):
+        upsample_ref.stack_direct(p, spec, x, y, (hop,), h, taps)
+        c = upsample_ref.upsample(p, (hop,), y)[:, :, :L].transpose(1, 2)
+    else:
+        local_ref.stack_direct(p, spec, x, y if term.startswith("frames") else None, hop, h, taps)
+    want = taps["skip"].transpose(1, 2)
+    T, in_s, out_s = L, [], []
+    for d in dil:
+        t_out = -(-T // d) * d - d
+        in_s.append(L - T)
+        out_s.append(L - t_out)
+        T = t_out
+    hs = F.conv1d(x, p["start_conv.weight"], p["start_conv.bias"]).transpose(1, 2)
+    skip = None
+    for i, d in enumerate(dil):
+        W = BR.layer_weights(p, i)
+        u = lambda n: torch.cat([p[f"filter_{n}_convs.{i}.weight"], p[f"gate_{n}_convs.{i}.weight"]], 0)[:, :, 0]
+        table = torch.cat([W["bf"], W["bg"]]).double().expand(B, -1)                 # (B, 2D): the biases
+        if h is not None:
+            table = table + h @ u("cond").T
+        if term.startswith("frames"):
+            table = table[:, None] + (y.transpose(1, 2) @ u("local").T)              # (B, F, 2D): + U y_f per frame
+        pre = BR.expand_table(table, L, hop)
+        if term.startswith("kslab"):
+            pre = pre + BR.mm(c, u("local"), "exact")
+        o = BR.block_forward(hs, BR.with_position_biases(W, pre, out_s[i]), d, in_s[i], out_s[i], L - T, skip)
+        skip = o["skip"]
+        hs = torch.zeros_like(hs)
+        hs[:, out_s[i]:] = o["h_out"]
+    assert _rel(skip, want) < 1e-12
+
+
 def test_layout_converters_round_trip():
     x = torch.randn(2, 37, 24, generator=torch.Generator().manual_seed(7)) * 3
     p = BR.pair_from_frames(x)
