@@ -503,6 +503,23 @@ int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond);
  * launch falls outside the window, so a long run is sampled window by window, each launch continuing through t0.  The same
  * lifetime rules as wn_gen_set_condition apply; NULL clears the table, and the last wn_gen_set_condition* call wins. */
 int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond, int frame0, int n_frames, int hop);
+/* Top-k and nucleus (top-p) truncation of the temperature draw, for every stream and every kernel.  Off is top_k = 0,
+ * top_p = 1, which wn_gen_create starts with; the values stay on the handle until the next call.  WN_E_BADARG for
+ * top_k < 0 or top_p outside (0, 1] (NaN included).  The rule, per stream and selection, on the fp32 logits l that
+ * d_out_logits reports (the regularizer already subtracted):
+ *   - it applies only when temperature > 0 and 0 < top_k < classes or top_p < 1; otherwise the selection is the
+ *     untruncated one above, bit for bit (at temperature <= 0 the argmax is always kept, so truncation is a no-op);
+ *   - p_c is the kernel's own fp32 softmax of l / temperature;
+ *   - the classes are ranked by l descending, equal logits by lower class index (on l, not on p: exact and reproducible
+ *     from the reported logits);
+ *   - K1 is the first top_k classes of that ranking (all of them when top_k is 0 or >= classes);
+ *   - K is the shortest prefix of K1, in rank order, whose float64 sum of p reaches top_p times the float64 sum of p
+ *     over K1 (at least one class; decisions within float64 rounding of the threshold may go either way);
+ *   - the draw is the untruncated inverse CDF restricted to K: the float64 cumulative sum of p over K in ascending index
+ *     order, normalised by its last element, the number of edges <= u (searchsorted side 'right') mapped back to the
+ *     kept class of that rank; a count past the end gives the largest kept index, never a dropped class.
+ * Kernel 1 then needs 4 * 8 * classes more bytes of shared memory per CTA (WN_E_UNSUPP if they do not fit). */
+int wn_gen_set_truncation(wn_gen_handle* h, int top_k, double top_p);
 /* Synchronise the stream and report whether a launch aborted (a CTA waited > ~3 s for a tag): 0 = fine. */
 int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer

@@ -62,6 +62,10 @@ struct GenParams {
     // local conditioning (cond_hop > 0): cond is a window [n_layers][NS][cond_frames][2D] of frames [cond_frame0, +cond_frames);
     // evaluation t reads row t / cond_hop - cond_frame0.  cond_sstride = floats per stream (2D for a global table).
     int cond_hop, cond_frame0, cond_frames, cond_sstride;
+    // top-k / nucleus truncation (wn_gen_set_truncation): trunc = 1 when the rule applies to this launch (temperature > 0
+    // and a bound that drops classes); the kernels branch to choose_truncated on it and run their own selection otherwise
+    int top_k, trunc;
+    double top_p;
 };
 
 // This evaluation's condition table: the window row of t's frame under local conditioning (once per evaluation).
@@ -136,6 +140,130 @@ __device__ __forceinline__ void row_dot(const float* __restrict__ w, const float
 // reference's CPU math, at a fraction of the instructions on the latency-critical path.
 __device__ __forceinline__ float sigmoid_(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 __device__ __forceinline__ float tanh_(float x) { return 2.f * sigmoid_(2.f * x) - 1.f; }
+
+// ---- top-k / nucleus (top-p) selection, shared by all six kernels (wn_gen_set_truncation states the rule)
+// Order-preserving key of a logit: a larger float gets a larger key; -0 is folded onto +0 so that the two tie, as numbers.
+__device__ __forceinline__ unsigned logit_key(float v) {
+    const unsigned b = __float_as_uint(v + 0.f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+// Rank key: the logit key above the class index reversed, so that of equal logits the lower index ranks higher.  All
+// rank keys of a row are distinct, and none equals ~0 (that would need a NaN logit).
+__device__ __forceinline__ unsigned long long rank_key(const unsigned* key_s, int c, int C) {
+    return ((unsigned long long)key_s[c] << 32) | (unsigned)(C - 1 - c);
+}
+__device__ __forceinline__ double warp_sum_d(double v) {   // xor butterfly: every lane ends with the same bits
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// One warp draws from the C logits lg (shared memory) with only the top_k highest-ranked classes (0: all) and, of those,
+// the shortest rank-ordered prefix holding top_p of their probability mass.  key_s and p_s are C-entry scratch of the
+// warp; key_s may be lg itself (each lane reads lg[c] before it writes key_s[c]), p_s must not overlap either.
+//   1. p_c: the kernels' fp32 softmax of lg / temperature, bit for bit (same divisions, expf, and summation order).
+//   2. K1 = the top_k largest rank keys: bisection for the largest bound with at least top_k keys at or above it, which
+//      stops as soon as exactly top_k are (the keys are distinct, so it always gets there).
+//   3. K = the largest bound >= K1's whose keys carry >= top_p * (float64 mass of K1), bisected until one key separates
+//      the bounds that pass and fail: K is then exactly the shortest prefix that reaches the threshold.
+//   4. The kernels' inverse CDF over the classes of K in index order (per-lane chunks + a warp scan in float64), edges
+//      <= u counted over K only, the count mapped to the kept class of that rank and clamped to the last kept class.
+// Out of line, as choose_sample is, so that none of it enters the register allocation of the per-layer loops.
+__device__ __noinline__ int choose_truncated(const float* lg, unsigned* key_s, float* p_s, int C, int lane,
+                                             float temperature, int top_k, double top_p, const double* u_ptr) {
+    float m = -INFINITY;
+    for (int c = lane; c < C; c += 32) {
+        const float l = lg[c];
+        const float x = l / temperature;
+        key_s[c] = logit_key(l);
+        p_s[c] = x;
+        m = fmaxf(m, x);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float sum = 0.f;
+    for (int c = lane; c < C; c += 32) {
+        const float e = expf(p_s[c] - m);
+        p_s[c] = e;
+        sum += e;
+    }
+    sum = warp_sum(sum);
+    for (int c = lane; c < C; c += 32) p_s[c] = p_s[c] / sum;
+    __syncwarp();
+
+    unsigned long long lo = 0ull;                           // kept: rank key >= lo
+    if (top_k > 0 && top_k < C) {
+        unsigned long long hi = ~0ull;                      // fewer than top_k keys >= hi
+        int n_lo = C;
+        while (n_lo != top_k) {
+            const unsigned long long mid = lo + ((hi - lo) >> 1);
+            int n = 0;
+            for (int c = lane; c < C; c += 32) n += rank_key(key_s, c, C) >= mid ? 1 : 0;
+            n = __reduce_add_sync(0xffffffffu, n);
+            if (n >= top_k) { lo = mid; n_lo = n; } else hi = mid;
+        }
+    }
+    if (top_p < 1.0) {
+        int n_lo = 0;
+        double s_lo = 0.0;
+        for (int c = lane; c < C; c += 32)
+            if (rank_key(key_s, c, C) >= lo) { ++n_lo; s_lo += (double)p_s[c]; }
+        n_lo = __reduce_add_sync(0xffffffffu, n_lo);
+        const double thr = top_p * warp_sum_d(s_lo);
+        unsigned long long hi = ~0ull;                      // the keys >= hi carry less than thr
+        int n_hi = 0;
+        while (n_lo - n_hi > 1) {
+            const unsigned long long mid = lo + ((hi - lo) >> 1);
+            int n = 0;
+            double s = 0.0;
+            for (int c = lane; c < C; c += 32)
+                if (rank_key(key_s, c, C) >= mid) { ++n; s += (double)p_s[c]; }
+            n = __reduce_add_sync(0xffffffffu, n);
+            if (warp_sum_d(s) >= thr) { lo = mid; n_lo = n; } else { hi = mid; n_hi = n; }
+        }
+    }
+
+    const int per = (C + 31) / 32;
+    const int c_lo = lane * per, c_hi = min(C, c_lo + per);
+    double run = 0.0;
+    int nk = 0;
+    for (int c = c_lo; c < c_hi; ++c)
+        if (rank_key(key_s, c, C) >= lo) { run += (double)p_s[c]; ++nk; }
+    double incl = run;
+    int kincl = nk;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const double up = __shfl_up_sync(0xffffffffu, incl, o);
+        const int kup = __shfl_up_sync(0xffffffffu, kincl, o);
+        if (lane >= o) { incl += up; kincl += kup; }
+    }
+    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl = 0.0;
+    const int kexcl = kincl - nk;
+    const double total = __shfl_sync(0xffffffffu, incl, 31);
+    const int n_kept = __shfl_sync(0xffffffffu, kincl, 31);
+    const double u = *u_ptr;
+    const double ut = u * total;
+    int cnt = 0;
+    run = 0.0;
+    for (int c = c_lo; c < c_hi; ++c) {
+        if (rank_key(key_s, c, C) < lo) continue;
+        run += (double)p_s[c];
+        const double v = run + excl;
+        bool le = v <= ut;
+        if (fabs(v - ut) <= 1e-9 * total) le = (v / total) <= u;           // exact rule only where it can matter
+        cnt += le ? 1 : 0;
+    }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    const int r = cnt < n_kept ? cnt : n_kept - 1;                          // rank among the kept classes, ascending index
+    int choice = -1;
+    if (r >= kexcl && r < kexcl + nk) {
+        int seen = kexcl;
+        for (int c = c_lo; c < c_hi; ++c)
+            if (rank_key(key_s, c, C) >= lo && seen++ == r) { choice = c; break; }
+    }
+    return __reduce_max_sync(0xffffffffu, choice);
+}
 
 template <int SB>
 __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
@@ -313,7 +441,14 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
         for (int s = warp; s < NS; s += GEN_WARPS) {
             const float* lg = p.logitbuf + (size_t)s * C;
             int choice;
-            if (p.temperature > 0.f) {
+            if (p.trunc) {
+                // the logits into the warp's scratch (they become its rank keys); probabilities in the truncation
+                // scratch that the host adds past prob only for such launches
+                for (int c = lane; c < C; c += 32) pw[c] = __ldcg(lg + c);
+                __syncwarp();
+                choice = choose_truncated(pw, reinterpret_cast<unsigned*>(pw), prob + (GEN_WARPS + warp) * C, C, lane,
+                                          p.temperature, p.top_k, p.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
+            } else if (p.temperature > 0.f) {
                 float m = -INFINITY;
                 for (int c = lane; c < C; c += 32) {
                     const float x = __ldcg(lg + c) / p.temperature;
@@ -721,7 +856,10 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         for (int s = warp; s < NS; s += GEN_WARPS) {
             const float* lg = regA + (size_t)s * C;
             int choice;
-            if (p.temperature > 0.f) {
+            if (p.trunc) {
+                choice = choose_truncated(lg, reinterpret_cast<unsigned*>(pw), reinterpret_cast<float*>(cw), C, lane,
+                                          p.temperature, p.top_k, p.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
+            } else if (p.temperature > 0.f) {
                 float m = -INFINITY;
                 for (int c = lane; c < C; c += 32) {
                     const float x = lg[c] / p.temperature;
@@ -1332,7 +1470,10 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_fast(const GenParam
         WORKER_SYNC();
         if (*abort_s) return;
         if (warp == 0) {
-            const int choice = choose_sample(logit_s, cdf, C, lane, p.temperature, p.uniforms ? p.uniforms + samp : nullptr);
+            const int choice = p.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
+                                                          reinterpret_cast<float*>(cdf) + C, C, lane, p.temperature,
+                                                          p.top_k, p.top_p, p.uniforms + samp)
+                                       : choose_sample(logit_s, cdf, C, lane, p.temperature, p.uniforms ? p.uniforms + samp : nullptr);
             if (lane == 0) {
                 misc[0] = choice;
                 if (cta == 0) p.out_idx[samp] = choice;
@@ -1703,8 +1844,11 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
         for (int c = tid; c < C; c += GEN_NT) logit_s[c] = wait_local(xl + c, tag_l, abort_s);
         WORKER_SYNC();
         if (warp == 0) {
-            const int choice = choose_sample(logit_s, cdf, C, lane, p.temperature,
-                                             p.uniforms ? p.uniforms + (size_t)stream * p.n_samples + samp : nullptr);
+            const int choice = p.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
+                                                          reinterpret_cast<float*>(cdf) + C, C, lane, p.temperature, p.top_k,
+                                                          p.top_p, p.uniforms + (size_t)stream * p.n_samples + samp)
+                                       : choose_sample(logit_s, cdf, C, lane, p.temperature,
+                                                       p.uniforms ? p.uniforms + (size_t)stream * p.n_samples + samp : nullptr);
             if (lane == 0) {
                 misc[0] = choice;
                 if (rank == 0) p.out_idx[(size_t)stream * p.n_samples + samp] = choice;
@@ -2119,7 +2263,10 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams 
         for (int c = tid; c < C; c += GEN_NT) logit_s[c] = wait_local(xl + c, tag_l, misc + 1);
         WORKER_SYNC();
         if (warp == 0) {
-            const int choice = choose_sample(logit_s, cdf, C, lane, p.temperature, p.uniforms ? p.uniforms + samp : nullptr);
+            const int choice = p.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
+                                                          reinterpret_cast<float*>(cdf) + C, C, lane, p.temperature,
+                                                          p.top_k, p.top_p, p.uniforms + samp)
+                                       : choose_sample(logit_s, cdf, C, lane, p.temperature, p.uniforms ? p.uniforms + samp : nullptr);
             if (lane == 0) {
                 misc[0] = choice;
                 if (cta == 0) p.out_idx[samp] = choice;
@@ -2738,8 +2885,11 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             const float* xl = reinterpret_cast<const float*>(Xl);
             for (int c = lane; c < W; c += 32) lg[c] = xl[(c >> 4) * (BLK / 4) + warp * NV + (c & 15)];
             __syncwarp();
-            const int choice = choose_sample(lg, cdf + warp * W, W, lane, p.temperature,
-                                             p.uniforms ? p.uniforms + (size_t)hs_g * p.n_samples + samp : nullptr);
+            const int choice = p.trunc ? choose_truncated(lg, reinterpret_cast<unsigned*>(cdf + warp * W),
+                                                          reinterpret_cast<float*>(cdf + warp * W) + W, W, lane, p.temperature,
+                                                          p.top_k, p.top_p, p.uniforms + (size_t)hs_g * p.n_samples + samp)
+                                       : choose_sample(lg, cdf + warp * W, W, lane, p.temperature,
+                                                       p.uniforms ? p.uniforms + (size_t)hs_g * p.n_samples + samp : nullptr);
             if (lane == 0) {
                 idx_s[warp] = choice;
                 if (rank == 0) p.out_idx[(size_t)hs_g * p.n_samples + samp] = choice;
@@ -2828,6 +2978,8 @@ struct wn_gen_handle {
     bool x2_ok;             // fast_ok on a 64-CTA grid with 4 rows per stage vector per CTA: gen_kernel_x2 applies
     size_t smem_x2;
     int n_wslots_x2;
+    int top_k;              // wn_gen_set_truncation (0, 1.0: off)
+    double top_p;
 };
 
 static int validate_shape(const wn_gen_shape* s) {
@@ -2861,6 +3013,8 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     wn_gen_handle* h = new (std::nothrow) wn_gen_handle();
     WN_REQUIRE(h, WN_E_BADARG, "wn_gen_create: out of host memory");
     h->shape = *s;
+    h->top_k = 0;
+    h->top_p = 1.0;
     h->dil.assign(s->dilations, s->dilations + s->n_layers);
     h->shape.dilations = h->dil.data();
     h->lay = scratch_layout(h->shape);
@@ -3117,12 +3271,21 @@ extern "C" int wn_gen_reset(wn_gen_handle* h, void* stream) {
 
 template <int SB>
 static int launch_gen(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel<SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+    // a truncated draw needs a second C-float scratch per warp (the other kernels have a float64 one already)
+    const size_t smem = h->smem + (p.trunc ? sizeof(float) * GEN_WARPS * (size_t)p.C : 0);
+    if (p.trunc) {
+        int optin = 0, dev = 0;
+        WN_CUDA(cudaGetDevice(&dev));
+        WN_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        WN_REQUIRE(smem <= (size_t)optin, WN_E_UNSUPP,
+                   "wn_gen_run: kernel 1 needs %zu bytes of shared memory with truncation, %d available", smem, optin);
+    }
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel<SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    WN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gen_kernel<SB>, GEN_NT, h->smem));
+    WN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gen_kernel<SB>, GEN_NT, smem));
     WN_REQUIRE(per_sm * h->sm_count >= h->grid, WN_E_UNSUPP, "wn_gen_run: %d CTAs cannot be co-resident", h->grid);
     void* args[] = {(void*)&p};
-    WN_CUDA(cudaLaunchCooperativeKernel((const void*)gen_kernel<SB>, dim3(h->grid), dim3(GEN_NT), args, h->smem, st));
+    WN_CUDA(cudaLaunchCooperativeKernel((const void*)gen_kernel<SB>, dim3(h->grid), dim3(GEN_NT), args, smem, st));
     return 0;
 }
 
@@ -3293,6 +3456,16 @@ extern "C" int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond
     return 0;
 }
 
+extern "C" int wn_gen_set_truncation(wn_gen_handle* h, int top_k, double top_p) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_truncation: null handle");
+    WN_REQUIRE(top_k >= 0, WN_E_BADARG, "wn_gen_set_truncation: top_k must be >= 0 (0: off), got %d", top_k);
+    WN_REQUIRE(top_p > 0.0 && top_p <= 1.0, WN_E_BADARG, "wn_gen_set_truncation: top_p must lie in (0, 1] (1: off), got %g",
+               top_p);                                      // NaN fails both comparisons
+    h->top_k = top_k;
+    h->top_p = top_p;
+    return 0;
+}
+
 extern "C" int wn_gen_check(wn_gen_handle* h, void* stream) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_check: null handle");
     int flag = 0;
@@ -3332,6 +3505,8 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         p.first = a->d_first; p.n_given = a->n_given; p.forced = a->d_forced; p.uniforms = a->d_uniforms;
         p.out_idx = a->d_out_idx; p.out_logits = a->d_out_logits; p.n_samples = a->n_samples;
         p.t0 = a->t0 + done; p.n_evals = n; p.temperature = a->temperature; p.regularize = a->regularize;
+        p.top_k = h->top_k; p.top_p = h->top_p;
+        p.trunc = a->temperature > 0.f && ((h->top_k > 0 && h->top_k < h->shape.classes) || h->top_p < 1.0);
         WN_CUDA(cudaMemsetAsync(p.bar, 0, sizeof(unsigned), st));
         int rc;
         const bool auto_cluster = h->mode == 0 && h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok);

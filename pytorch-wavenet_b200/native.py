@@ -208,6 +208,7 @@ SIGNATURES = {
     "wn_gen_weights_changed": (C.c_int, [C.c_void_p]),
     "wn_gen_set_condition": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_set_condition_frames": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3),
+    "wn_gen_set_truncation": (C.c_int, [C.c_void_p, C.c_int, C.c_double]),
     "wn_gen_kernel_id": (C.c_int, [C.c_void_p]),
     "wn_gen_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_read_trace": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_void_p]),

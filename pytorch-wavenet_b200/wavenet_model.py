@@ -1071,12 +1071,14 @@ class _Runtime:
         return t0 + args.n_evals
 
     def generate(self, num_samples, first, temperature, regularize, uniforms=None, forced=None,
-                 want_logits=False, callbacks=None, cond=None, local=None):
+                 want_logits=False, callbacks=None, cond=None, local=None, top_k=0, top_p=1.0):
         """first: (NS, n_given) int array.  Returns (indices (NS, num_samples) int64 ndarray, logits or None, t_end).
+        top_k, top_p: the truncation of the temperature draw (wn_gen_set_truncation), set on the handle by every call.
         callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done.
         cond: the (NS, G) fp32 condition rows of a conditioned model, else None.
         local: (y, hop) of a locally conditioned model, y the (NS, C, F) fp32 series, else None.  The condition table is
         built window by window (at most ``local_table_bytes`` each), and launches are split at the window boundaries."""
+        top_k, top_p = _truncation(top_k, top_p)
         m = self.model
         dev = self.device()
         self.step_session = None             # a generate_fast run restarts the device queues (wavenet_model.py:250)
@@ -1085,6 +1087,8 @@ class _Runtime:
         if n_given < 1:
             raise RuntimeError("first_samples must hold at least one sample")
         s = self.sampler(NS)
+        # on every call, so that one call's setting never reaches the next
+        native.check(native.lib().wn_gen_set_truncation(s["handle"], top_k, top_p), "gen truncation")
         stream = torch.cuda.current_stream(dev).cuda_stream
         # the condition table is read by every launch of this run: the sampler entry keeps it alive
         if local is None:
@@ -1151,6 +1155,20 @@ class _Runtime:
             (forced.nbytes if d_forced is not None else 0)
         self.d2h_bytes_last = NS * num_samples * 4 + (logits.nbytes if want_logits else 0)
         return idx, logits, total_evals
+
+
+def _truncation(top_k, top_p):
+    """Checked (top_k, top_p) of the sampler's truncated draw: top_k an integer >= 0 (0: off), top_p a real number in
+    (0, 1] (1: off).  Raises ValueError otherwise, bools included."""
+    if isinstance(top_k, (bool, np.bool_)) or not isinstance(top_k, (int, np.integer)):
+        raise ValueError(f"top_k must be an integer >= 0 (0: off), got {top_k!r}")
+    if isinstance(top_p, (bool, np.bool_)) or not isinstance(top_p, (int, float, np.integer, np.floating)):
+        raise ValueError(f"top_p must be a number in (0, 1] (1: off), got {top_p!r}")
+    if top_k < 0:
+        raise ValueError(f"top_k must be >= 0 (0: off), got {top_k}")
+    if not 0.0 < float(top_p) <= 1.0:
+        raise ValueError(f"top_p must lie in (0, 1] (1: off), got {top_p}")
+    return int(top_k), float(top_p)
 
 
 def _exact_convolutions():
@@ -1557,24 +1575,30 @@ class WaveNetModel(nn.Module):
         return sh[1]
 
     def generate_fast(self, num_samples, first_samples=None, temperature=1., regularize=0.,
-                      progress_callback=None, progress_interval=100, condition=None, local_condition=None):
+                      progress_callback=None, progress_interval=100, condition=None, local_condition=None,
+                      top_k=0, top_p=1.0):
         """Fast-WaveNet sampling; returns the mu-law expanded waveform, float64 ndarray of ``num_samples`` values.
 
         Same schedule as the reference (wavenet_model.py:237-315): the queues are reset, the given samples warm
         them up, then every step feeds the chosen sample back.  ``temperature > 0`` draws from the softmax with
         numpy's GLOBAL RNG (one ``random_sample()`` per sample, which is what ``np.random.choice`` consumes), so
         ``np.random.seed(s)`` reproduces the reference's stream; ``temperature == 0`` takes the argmax.
+        ``top_k`` / ``top_p`` truncate the draw (0 / 1.0: off): the classes are ranked by logit (ties: lower index), the
+        first ``top_k`` are kept, of those the shortest ranked prefix holding ``top_p`` of their probability, and the
+        draw is the same inverse CDF over the kept classes only.  No effect at ``temperature == 0``; ValueError for a
+        negative or non-integer ``top_k`` or a ``top_p`` outside (0, 1].
         ``condition``: a conditioned model's label or (G,) vector for this stream.
         ``local_condition``: a locally conditioned model's (C, F) series for this stream; evaluation e (which reads sample
         e, the given samples first, and predicts sample e + 1) takes frame e // hop, so F >= ceil((n_given - 1 +
         num_samples) / hop).
         """
+        top_k, top_p = _truncation(top_k, top_p)
         if self.start_conv.weight.device.type != "cuda":
             twin = self._cuda_shadow()
             audio = twin.generate_fast(num_samples, first_samples=first_samples, temperature=temperature,
                                        regularize=regularize, progress_callback=progress_callback,
                                        progress_interval=progress_interval, condition=condition,
-                                       local_condition=local_condition)
+                                       local_condition=local_condition, top_k=top_k, top_p=top_p)
             for q, tq in zip(self.dilated_queues, twin.dilated_queues):
                 q.data, q.in_pos, q.out_pos = tq.data, tq.in_pos, tq.out_pos
             self.train()
@@ -1599,21 +1623,23 @@ class WaveNetModel(nn.Module):
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond,
-                                    local=local)
+                                    local=local, top_k=top_k, top_p=top_p)
         self._export_queues()
         self.train()
         generated = (idx[0] / self.classes) * 2. - 1
         return mu_law_expansion(generated, self.classes)
 
     def generate_fast_batch(self, num_samples, first_samples, temperature=1., regularize=0., uniforms=None,
-                            forced=None, return_logits=False, condition=None, local_condition=None):
+                            forced=None, return_logits=False, condition=None, local_condition=None, top_k=0, top_p=1.0):
         """``n_streams`` independent generate_fast runs batched in one kernel (the reference has a single stream,
         wavenet_model.py:179).  first_samples: (n_streams, n_given) ints.  Returns int64 indices
         (n_streams, num_samples) [and the per-step logits].  Run through the same sampler kernel, stream s equals a
         single-stream run bit for bit (256-wide nets run the tensor-core cluster kernel for any number of streams; other
         nets a latency kernel for one stream and one thread-block cluster per stream otherwise, which differ at rounding
         level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream.
-        local_condition: a locally conditioned model's (n_streams, C, F) series, one per stream (see generate_fast)."""
+        local_condition: a locally conditioned model's (n_streams, C, F) series, one per stream (see generate_fast).
+        top_k, top_p: the truncated draw of generate_fast, the same values for every stream."""
+        top_k, top_p = _truncation(top_k, top_p)
         first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
         first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
         cond = self._condition(condition, first.shape[0])
@@ -1623,7 +1649,8 @@ class WaveNetModel(nn.Module):
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, logits, _ = rt.generate(num_samples, first, temperature, regularize, uniforms=uniforms,
-                                         forced=forced, want_logits=return_logits, cond=cond, local=local)
+                                         forced=forced, want_logits=return_logits, cond=cond, local=local,
+                                         top_k=top_k, top_p=top_p)
         self._export_queues()
         self.train()
         return (idx, logits) if return_logits else idx
