@@ -520,6 +520,28 @@ int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond, int frame
  *     kept class of that rank; a count past the end gives the largest kept index, never a dropped class.
  * Kernel 1 then needs 4 * 8 * classes more bytes of shared memory per CTA (WN_E_UNSUPP if they do not fit). */
 int wn_gen_set_truncation(wn_gen_handle* h, int top_k, double top_p);
+/* Per-stream sampling settings: stream s's prompt length, truncation, temperature and regularizer. */
+typedef struct wn_gen_stream_params {
+    int n_given, top_k;
+    float temperature, regularize;
+    double top_p;
+} wn_gen_stream_params;
+/* Give every stream its own settings: params is a HOST array [n_streams], copied before the call returns; NULL returns to
+ * the scalar path (wn_gen_create starts there).  The setting stays on the handle until the next call.  WN_E_BADARG, and
+ * nothing changes, for n_given < 1, top_k < 0, top_p outside (0, 1] or a non-finite temperature or regularize.  The
+ * schedule of wn_gen_run then becomes, per stream s (evaluation e is still position e of every stream):
+ *   - input of evaluation e: d_first[s*pitch + e] if e < n_given[s], else d_forced[s*n_samples + e - n_given[s]] when
+ *     teacher forcing, else the stream's own last choice; pitch = a->n_given, which must equal the largest n_given[s];
+ *   - at e >= n_given[s] - 1 the stream chooses sample i = e - (n_given[s] - 1) with its own temperature, regularize,
+ *     top_k and top_p, by the rules of wn_gen_run and wn_gen_set_truncation;
+ *   - the head runs at every evaluation e >= head_from = min_s n_given[s] - 1; a stream still inside its prompt there
+ *     makes no selection: it reads no uniform and writes no index or logits;
+ *   - n_samples stays the row pitch of forced / uniforms / out_idx / out_logits, and t0 + n_evals <= head_from + n_samples.
+ * A stream that needs fewer samples than the launch runs keeps evaluating; its extra outputs land in its row's padding.
+ * While records are set, a->temperature and a->regularize must be 0 and the handle's truncation off (WN_E_BADARG
+ * otherwise), and d_uniforms is required when any stream has temperature > 0.  The library keeps a device copy of the
+ * records (allocated at the first call, freed by wn_gen_destroy) and uploads it in stream order before the next launch. */
+int wn_gen_set_stream_params(wn_gen_handle* h, const wn_gen_stream_params* params);
 /* Synchronise the stream and report whether a launch aborted (a CTA waited > ~3 s for a tag): 0 = fine. */
 int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer

@@ -18,6 +18,8 @@
 #include "common.cuh"
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
+#include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <new>
@@ -32,6 +34,14 @@ struct GenLayer {
     const float *wf, *wg, *wr, *ws, *bf, *bg, *br, *bs;
     long long ring_off;     // in floats, from rings base
     int dil, ring_len;
+};
+
+// One stream's sampling settings: the library's device copy of a wn_gen_stream_params record; trunc = 1 when the truncation
+// rule applies to the stream (temperature > 0 and a bound that drops classes).
+struct GenStream {
+    int n_given, top_k, trunc;
+    float temperature, regularize;
+    double top_p;
 };
 
 struct GenParams {
@@ -66,7 +76,47 @@ struct GenParams {
     // and a bound that drops classes); the kernels branch to choose_truncated on it and run their own selection otherwise
     int top_k, trunc;
     double top_p;
+    // per-stream settings (wn_gen_set_stream_params; null: every stream uses the scalars above).  The head runs at every
+    // evaluation t >= head_from (min over streams of n_given - 1, n_given - 1 on the scalar path); n_given is then the
+    // pitch of `first`, and trunc is set when any stream truncates (it only sizes kernel 1's scratch)
+    const GenStream* ps;
+    int head_from;
 };
+
+// Every role of every multi-stream kernel (workers, weight producers, pusher) decides whether evaluation t runs the head
+// with this one predicate, so that they all schedule the same stages.
+__device__ __forceinline__ bool head_at(const GenParams& p, int t) { return t >= p.head_from; }
+
+// Stream s's settings: its record under per-stream parameters, the launch's scalars otherwise.  Read where the stream is
+// known (input select, regularizer, selection), never held across the per-layer loops.  PS: PS_ANY tests p.ps; a kernel
+// with an instantiation per path passes PS_OFF (p.ps is null: it then carries no trace of the records) or PS_ON (set).
+enum { PS_OFF = 0, PS_ON = 1, PS_ANY = 2 };
+template <int PS = PS_ANY>
+__device__ __forceinline__ bool has_records(const GenParams& p) { return PS == PS_ANY ? p.ps != nullptr : PS == PS_ON; }
+template <int PS = PS_ANY>
+__device__ __forceinline__ GenStream stream_set(const GenParams& p, int s) {
+    if (has_records<PS>(p)) return p.ps[s];
+    GenStream g;
+    g.n_given = p.n_given; g.top_k = p.top_k; g.trunc = p.trunc;
+    g.temperature = p.temperature; g.regularize = p.regularize; g.top_p = p.top_p;
+    return g;
+}
+
+// The given input of evaluation t of stream s: its prompt sample (first has pitch p.n_given), else its forced sample when
+// teacher forcing.  false: the stream feeds back its own last choice.
+template <int PS = PS_ANY>
+__device__ __forceinline__ bool given_input(const GenParams& p, int s, int t, int& v) {
+    const int ng = has_records<PS>(p) ? p.ps[s].n_given : p.n_given;
+    if (t < ng) { v = p.first[(size_t)s * p.n_given + t]; return true; }
+    if (p.forced != nullptr) { v = p.forced[(size_t)s * p.n_samples + (t - ng)]; return true; }
+    return false;
+}
+
+// The sample stream s chooses at evaluation t (negative while t is still inside its prompt: no selection then).
+template <int PS = PS_ANY>
+__device__ __forceinline__ int sample_of(const GenParams& p, int s, int t) {
+    return t - ((has_records<PS>(p) ? p.ps[s].n_given : p.n_given) - 1);
+}
 
 // This evaluation's condition table: the window row of t's frame under local conditioning (once per evaluation).
 __device__ __forceinline__ const float* cond_at(const GenParams& p, int t, int D) {
@@ -295,13 +345,11 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;                           // absolute evaluation counter == time
         const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
-        const bool want_head = (t >= p.n_given - 1);
-        const int samp = t - (p.n_given - 1);              // sample number this evaluation chooses
+        const bool want_head = head_at(p, t);
         // ---- input index of this evaluation
-        if (t < p.n_given) {
-            for (int s = tid; s < NS; s += GEN_NT) idx_s[s] = p.first[(size_t)s * p.n_given + t];
-        } else if (p.forced != nullptr) {
-            for (int s = tid; s < NS; s += GEN_NT) idx_s[s] = p.forced[(size_t)s * p.n_samples + (t - p.n_given)];
+        for (int s = tid; s < NS; s += GEN_NT) {
+            int v;
+            if (given_input(p, s, t, v)) idx_s[s] = v;
         }
         for (int i = tid; i < nS * NS; i += GEN_NT) skacc[i] = 0.f;
         __syncthreads();
@@ -428,9 +476,10 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
                     for (int j = 0; j < SB; ++j) {
                         const int s = s0 + j;
                         if (s >= NS) break;
-                        const float v = (acc[j] + bias) - reg;
+                        const float v = (acc[j] + bias) - (p.ps ? __fmul_rn(dc * dc, p.ps[s].regularize) : reg);
                         p.logitbuf[(size_t)s * C + row] = v;
-                        if (p.out_logits) p.out_logits[((size_t)s * p.n_samples + samp) * C + row] = v;
+                        const int samp = sample_of(p, s, t);
+                        if (p.out_logits && samp >= 0) p.out_logits[((size_t)s * p.n_samples + samp) * C + row] = v;
                     }
                 }
             }
@@ -439,19 +488,22 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
         // ---- choose (every CTA redundantly, so no broadcast barrier is needed): warp per stream
         float* pw = prob + warp * C;
         for (int s = warp; s < NS; s += GEN_WARPS) {
+            const GenStream ss = stream_set(p, s);
+            const int samp = t - (ss.n_given - 1);         // sample number this evaluation chooses
+            if (samp < 0) continue;                        // still inside its prompt
             const float* lg = p.logitbuf + (size_t)s * C;
             int choice;
-            if (p.trunc) {
+            if (ss.trunc) {
                 // the logits into the warp's scratch (they become its rank keys); probabilities in the truncation
                 // scratch that the host adds past prob only for such launches
                 for (int c = lane; c < C; c += 32) pw[c] = __ldcg(lg + c);
                 __syncwarp();
                 choice = choose_truncated(pw, reinterpret_cast<unsigned*>(pw), prob + (GEN_WARPS + warp) * C, C, lane,
-                                          p.temperature, p.top_k, p.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
-            } else if (p.temperature > 0.f) {
+                                          ss.temperature, ss.top_k, ss.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
+            } else if (ss.temperature > 0.f) {
                 float m = -INFINITY;
                 for (int c = lane; c < C; c += 32) {
-                    const float x = __ldcg(lg + c) / p.temperature;
+                    const float x = __ldcg(lg + c) / ss.temperature;
                     pw[c] = x;
                     m = fmaxf(m, x);
                 }
@@ -679,10 +731,10 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
     // ---- weight prefetch pipeline (thread 0 produces): stage q of the launch lives in slot q % NSLOT
     int pf_ev = 0, pf_st = 0;                 // producer cursor
     long long pf_q = 0, cons_q = 0;
-    auto stages_in_eval = [&](int ev) { return (p.t0 + ev >= p.n_given - 1) ? 2 * NL + 2 : 2 * NL; };
+    auto stages_in_eval = [&](int ev) { return head_at(p, p.t0 + ev) ? 2 * NL + 2 : 2 * NL; };
     auto produce_one = [&]() {                // the last thread only (it has no epilogue work)
         if (pf_ev >= p.n_evals) return;
-        const bool wh = (p.t0 + pf_ev >= p.n_given - 1);
+        const bool wh = head_at(p, p.t0 + pf_ev);
         const StageDesc d = stage_desc(p, pf_st, wh, nD, nR, nS, nE, nC);
         const int slot = (int)(pf_q % NSLOT);
         mbar_expect_tx(fullb + slot, (unsigned)(d.n * d.K * 4));
@@ -735,12 +787,10 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         const unsigned tag = (unsigned)t + 1u;
         const int par = t & 1;
         const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
-        const bool want_head = (t >= p.n_given - 1);
-        const int samp = t - (p.n_given - 1);
-        if (t < p.n_given) {
-            for (int s = tid; s < NS; s += GEN_NT) idx_s[s] = p.first[(size_t)s * p.n_given + t];
-        } else if (p.forced != nullptr) {
-            for (int s = tid; s < NS; s += GEN_NT) idx_s[s] = p.forced[(size_t)s * p.n_samples + (t - p.n_given)];
+        const bool want_head = head_at(p, t);
+        for (int s = tid; s < NS; s += GEN_NT) {
+            int v;
+            if (given_input(p, s, t, v)) idx_s[s] = v;
         }
         for (int i = tid; i < nS * NS; i += GEN_NT) skacc[i] = 0.f;
         __syncthreads();
@@ -843,9 +893,10 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         for (int i = tid; i < nC * NS; i += GEN_NT) {
             const int it = i / NS, s = i - it * NS, row = oC + it;
             const float dc = (float)row - (float)C / 2.f;
-            const float v = (sum_parts(it, nw, s) + __ldg(p.e2b + row)) - (dc * dc) * p.regularize;
+            const float v = (sum_parts(it, nw, s) + __ldg(p.e2b + row)) - (dc * dc) * (p.ps ? p.ps[s].regularize : p.regularize);
             st_pair(lgl + (size_t)s * C + row, v, tag);
-            if (p.out_logits) p.out_logits[((size_t)s * p.n_samples + samp) * C + row] = v;
+            const int samp = sample_of(p, s, t);
+            if (p.out_logits && samp >= 0) p.out_logits[((size_t)s * p.n_samples + samp) * C + row] = v;
         }
         // ---- every CTA collects all logits and picks the next sample itself (no broadcast needed)
         for (int i = tid; i < NS * C; i += GEN_NT) regA[i] = poll_pair(lgl + i, tag, p.err, abort_s);
@@ -854,15 +905,18 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         float* pw = prob + warp * C;
         double* cw = cdf + warp * C;
         for (int s = warp; s < NS; s += GEN_WARPS) {
+            const GenStream ss = stream_set(p, s);
+            const int samp = t - (ss.n_given - 1);
+            if (samp < 0) continue;                        // still inside its prompt
             const float* lg = regA + (size_t)s * C;
             int choice;
-            if (p.trunc) {
+            if (ss.trunc) {
                 choice = choose_truncated(lg, reinterpret_cast<unsigned*>(pw), reinterpret_cast<float*>(cw), C, lane,
-                                          p.temperature, p.top_k, p.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
-            } else if (p.temperature > 0.f) {
+                                          ss.temperature, ss.top_k, ss.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
+            } else if (ss.temperature > 0.f) {
                 float m = -INFINITY;
                 for (int c = lane; c < C; c += 32) {
-                    const float x = lg[c] / p.temperature;
+                    const float x = lg[c] / ss.temperature;
                     pw[c] = x;
                     m = fmaxf(m, x);
                 }
@@ -1590,7 +1644,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
         if (lane == 0) {
             unsigned q = 0;
             for (int ev = 0; ev < p.n_evals; ++ev) {
-                const bool wh = (p.t0 + ev >= p.n_given - 1);
+                const bool wh = head_at(p, p.t0 + ev);
                 const int n_st = wh ? 2 * NL + 2 : 2 * NL;
                 for (int st = 0; st < n_st; ++st, ++q) {
                     StageDesc d = stage_desc(p, st, true, nD, nR, nS, nE, nC);
@@ -1646,11 +1700,10 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
         const int t = p.t0 + ev;
         const unsigned rtag = (unsigned)t + 1u;                  // ring tag of time t
         const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
-        const bool want_head = (t >= p.n_given - 1);
-        const int samp = t - (p.n_given - 1);
+        const bool want_head = head_at(p, t);
         if (tid == 0) {
-            if (t < p.n_given) misc[0] = p.first[(size_t)stream * p.n_given + t];
-            else if (p.forced != nullptr) misc[0] = p.forced[(size_t)stream * p.n_samples + (t - p.n_given)];
+            int v;
+            if (given_input(p, stream, t, v)) misc[0] = v;
         }
         for (int l = tid; l < NL; l += GEN_NT) {
             const int s1 = slot_s[l] + 1;
@@ -1835,23 +1888,28 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
                 acc = warp_sum(acc);
                 const int row = oC + it;
                 const float dc = (float)row - (float)C / 2.f;
-                const float v = (acc + __ldg(p.e2b + row)) - (dc * dc) * p.regularize;
+                const float v = (acc + __ldg(p.e2b + row)) - (dc * dc) * (p.ps ? p.ps[stream].regularize : p.regularize);
                 if (lane < CL) st_remote_pair(xl + row, (unsigned)lane, v, tag_l);
-                if (lane == 0 && p.out_logits) p.out_logits[((size_t)stream * p.n_samples + samp) * C + row] = v;
+                const int samp = sample_of(p, stream, t);
+                if (lane == 0 && p.out_logits && samp >= 0) p.out_logits[((size_t)stream * p.n_samples + samp) * C + row] = v;
             }
             release_slot();
         }
         for (int c = tid; c < C; c += GEN_NT) logit_s[c] = wait_local(xl + c, tag_l, abort_s);
         WORKER_SYNC();
         if (warp == 0) {
-            const int choice = p.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
-                                                          reinterpret_cast<float*>(cdf) + C, C, lane, p.temperature, p.top_k,
-                                                          p.top_p, p.uniforms + (size_t)stream * p.n_samples + samp)
-                                       : choose_sample(logit_s, cdf, C, lane, p.temperature,
-                                                       p.uniforms ? p.uniforms + (size_t)stream * p.n_samples + samp : nullptr);
-            if (lane == 0) {
-                misc[0] = choice;
-                if (rank == 0) p.out_idx[(size_t)stream * p.n_samples + samp] = choice;
+            const GenStream ss = stream_set(p, stream);
+            const int samp = t - (ss.n_given - 1);
+            if (samp >= 0) {                                     // no selection while the stream is inside its prompt
+                const int choice = ss.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
+                                                               reinterpret_cast<float*>(cdf) + C, C, lane, ss.temperature,
+                                                               ss.top_k, ss.top_p, p.uniforms + (size_t)stream * p.n_samples + samp)
+                                            : choose_sample(logit_s, cdf, C, lane, ss.temperature,
+                                                            p.uniforms ? p.uniforms + (size_t)stream * p.n_samples + samp : nullptr);
+                if (lane == 0) {
+                    misc[0] = choice;
+                    if (rank == 0) p.out_idx[(size_t)stream * p.n_samples + samp] = choice;
+                }
             }
         }
     }
@@ -2404,7 +2462,8 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
 // COND: the filter / gate biases come from the condition table (a separate instantiation: the per-layer branch costs the
 // unconditioned single-stream kernel ~6 % of its time per sample).  FRAMES (with COND): the table is a local-conditioning
 // window, and each evaluation reads its frame's rows (a third instantiation, so the other two carry no trace of it).
-template <int CS, bool COND, bool FRAMES>
+// PS: per-stream settings (p.ps set); the scalar path runs the PS = false instantiations, which read only the scalars.
+template <int CS, bool COND, bool FRAMES, bool PS>
 __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
     extern __shared__ __align__(128) unsigned char smb[];
     constexpr int W = CL8_W, SB = CL8_SB, NV = 16, BLK = CL8_BLK, VEC = CL8_VEC, VR = CL / CS, NVC = NV * VR;
@@ -2501,7 +2560,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     if (warp == GEN_WARPS + 1) {
         int sb = 0;
         for (int ev = 0; ev < p.n_evals; ++ev) {
-            const bool wh = (p.t0 + ev >= p.n_given - 1);
+            const bool wh = head_at(p, p.t0 + ev);
             for (int l = 0; l < NL; ++l) {
                 CL8_STAGED_SYNC();
                 push(sb, Xz + (l & 1) * VEC, 2 + (l & 1));
@@ -2529,7 +2588,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         if (lane == 0) {
             unsigned q = 0;
             for (int ev = 0; ev < p.n_evals; ++ev) {
-                const bool wh = (p.t0 + ev >= p.n_given - 1);
+                const bool wh = head_at(p, p.t0 + ev);
                 const int n_st = wh ? 3 * NL + 2 : 3 * NL;      // per layer: old taps, current input, stage 2; then the two head stages
                 for (int st = 0; st < n_st; ++st, ++q) {
                     const unsigned char* src;
@@ -2566,7 +2625,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     if (VR == 2 && warp == GEN_WARPS + 2) {
         unsigned q = 0;
         for (int ev = 0; ev < p.n_evals; ++ev) {
-            const bool wh = (p.t0 + ev >= p.n_given - 1);
+            const bool wh = head_at(p, p.t0 + ev);
             const int n_st = wh ? 3 * NL + 2 : 3 * NL;
             for (int st = 0; st < n_st; ++st, ++q) {
                 const unsigned half = (st < 3 * NL) ? CL8_IMG2 : CL8_IMGH;
@@ -2697,8 +2756,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;
         const unsigned rtag = (unsigned)t + 1u;          // ring tag of time t
-        const bool want_head = (t >= p.n_given - 1);
-        const int samp = t - (p.n_given - 1);
+        const bool want_head = head_at(p, t);
         const bool tr_on = p.trace != nullptr && blockIdx.x == 0 && tid == 0 && ev == p.n_evals - 1;
         // FRAMES: this stream's rows of evaluation t's frame; layer l's row is l * NS * cond_sstride further
         const float* cs_t = nullptr;
@@ -2707,9 +2765,8 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
 #define TR8() do { if (tr_on && tr_n < 2040) p.trace[tr_n++] = clock64(); } while (0)
         if (tr_on) p.trace[2040] = clock64();             // whole-evaluation stamps live at [2040..2047]
         if (tid < SB && cl * SB + tid < NS) {
-            const int g = cl * SB + tid;
-            if (t < p.n_given) idx_s[tid] = p.first[(size_t)g * p.n_given + t];
-            else if (p.forced != nullptr) idx_s[tid] = p.forced[(size_t)g * p.n_samples + (t - p.n_given)];
+            int v;
+            if (given_input<PS ? PS_ON : PS_OFF>(p, cl * SB + tid, t, v)) idx_s[tid] = v;
         }
         for (int l = tid; l < NL; l += GEN_NT) {
             const int s1 = slot_s[l] + 1;
@@ -2870,8 +2927,12 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         WORKER_SYNC();
         if (fin_a) {
             const float dc = (float)fch - (float)W / 2.f;
-            const float v = (head_sum(part_of(pb_i, fvr), fc, fs) + __ldg(p.e2b + fch)) - (dc * dc) * p.regularize;
-            if (fs_on && p.out_logits) p.out_logits[((size_t)fsg * p.n_samples + samp) * W + fch] = v;
+            const float v = (head_sum(part_of(pb_i, fvr), fc, fs) + __ldg(p.e2b + fch)) -
+                            (dc * dc) * ((PS && fs_on) ? p.ps[fsg].regularize : p.regularize);
+            if (fs_on && p.out_logits) {
+                const int samp = sample_of<PS ? PS_ON : PS_OFF>(p, fsg, t);
+                if (samp >= 0) p.out_logits[((size_t)fsg * p.n_samples + samp) * W + fch] = v;
+            }
             reinterpret_cast<float*>(stg_of(sb_i, fvr))[fs * NV + fc] = v;               // logits travel as fp32: [stream][16]
         }
         pb_i ^= 1;
@@ -2881,18 +2942,23 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         if (tr_on) p.trace[2042] = clock64();             // head done, logits everywhere
         // every CTA holds all logits of its 8 streams: warp = stream draws the next index (all CTAs agree)
         if (hs_g < NS) {
-            float* lg = logit_s + warp * W;
-            const float* xl = reinterpret_cast<const float*>(Xl);
-            for (int c = lane; c < W; c += 32) lg[c] = xl[(c >> 4) * (BLK / 4) + warp * NV + (c & 15)];
-            __syncwarp();
-            const int choice = p.trunc ? choose_truncated(lg, reinterpret_cast<unsigned*>(cdf + warp * W),
-                                                          reinterpret_cast<float*>(cdf + warp * W) + W, W, lane, p.temperature,
-                                                          p.top_k, p.top_p, p.uniforms + (size_t)hs_g * p.n_samples + samp)
-                                       : choose_sample(lg, cdf + warp * W, W, lane, p.temperature,
-                                                       p.uniforms ? p.uniforms + (size_t)hs_g * p.n_samples + samp : nullptr);
-            if (lane == 0) {
-                idx_s[warp] = choice;
-                if (rank == 0) p.out_idx[(size_t)hs_g * p.n_samples + samp] = choice;
+            const GenStream ss = stream_set<PS ? PS_ON : PS_OFF>(p, hs_g);
+            const int samp = t - (ss.n_given - 1);
+            if (samp >= 0) {                              // no selection while the stream is inside its prompt
+                float* lg = logit_s + warp * W;
+                const float* xl = reinterpret_cast<const float*>(Xl);
+                for (int c = lane; c < W; c += 32) lg[c] = xl[(c >> 4) * (BLK / 4) + warp * NV + (c & 15)];
+                __syncwarp();
+                const int choice = ss.trunc ? choose_truncated(lg, reinterpret_cast<unsigned*>(cdf + warp * W),
+                                                               reinterpret_cast<float*>(cdf + warp * W) + W, W, lane,
+                                                               ss.temperature, ss.top_k, ss.top_p,
+                                                               p.uniforms + (size_t)hs_g * p.n_samples + samp)
+                                            : choose_sample(lg, cdf + warp * W, W, lane, ss.temperature,
+                                                            p.uniforms ? p.uniforms + (size_t)hs_g * p.n_samples + samp : nullptr);
+                if (lane == 0) {
+                    idx_s[warp] = choice;
+                    if (rank == 0) p.out_idx[(size_t)hs_g * p.n_samples + samp] = choice;
+                }
             }
         }
         if (tr_on) p.trace[2043] = clock64();             // sampled
@@ -2980,6 +3046,12 @@ struct wn_gen_handle {
     int n_wslots_x2;
     int top_k;              // wn_gen_set_truncation (0, 1.0: off)
     double top_p;
+    // wn_gen_set_stream_params: the host records (empty: the scalar path), their device copy (allocated at the first call,
+    // outside the workspace), whether it still has to be uploaded, and what wn_gen_run checks and derives from them
+    std::vector<wn_gen_stream_params> sp;
+    GenStream* d_sp;
+    bool sp_dirty, sp_any_trunc, sp_any_temp;
+    int sp_max_given, sp_head_from;
 };
 
 static int validate_shape(const wn_gen_shape* s) {
@@ -3015,6 +3087,8 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     h->shape = *s;
     h->top_k = 0;
     h->top_p = 1.0;
+    h->d_sp = nullptr;
+    h->sp_dirty = false;
     h->dil.assign(s->dilations, s->dilations + s->n_layers);
     h->shape.dilations = h->dil.data();
     h->lay = scratch_layout(h->shape);
@@ -3322,11 +3396,11 @@ static int launch_gen_cluster(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     return 0;
 }
 
-template <int CS, bool COND, bool FRAMES>
+template <int CS, bool COND, bool FRAMES, bool PS>
 static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, int* max_clusters_out, bool launch) {
     const size_t smem = (CS == 16) ? h->smem_cl8 : h->smem_cl8_8;
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * CS));
     cfg.blockDim = dim3(GEN_NT + 64 + (CS == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
@@ -3340,18 +3414,29 @@ static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, in
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND, FRAMES>, &cfg));
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND, FRAMES, PS>, &cfg));
     if (max_clusters_out) *max_clusters_out = max_clusters;
     if (!launch) return 0;
     WN_REQUIRE(max_clusters >= 1, WN_E_UNSUPP, "wn_gen_run: a %d-CTA cluster cannot be scheduled on this device", CS);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND, FRAMES>, p));   // clusters are independent: more than fit run in waves
+    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND, FRAMES, PS>, p));   // clusters are independent: more than fit run in waves
     return 0;
+}
+template <bool PS>
+static int launch_gen_cl8_cond(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
+    if (p.cond && p.cond_hop)
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true, PS>(h, p, st, nullptr, true)
+                               : launch_gen_cl8_cs<8, true, true, PS>(h, p, st, nullptr, true);
+    if (p.cond)
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false, PS>(h, p, st, nullptr, true)
+                               : launch_gen_cl8_cs<8, true, false, PS>(h, p, st, nullptr, true);
+    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false, PS>(h, p, st, nullptr, true)
+                           : launch_gen_cl8_cs<8, false, false, PS>(h, p, st, nullptr, true);
 }
 // Cluster size: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8 (15 clusters fit instead of 7).
 static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     if (h->cl8_cs == 0) {
         int fit16 = 0;
-        const int rc = launch_gen_cl8_cs<16, false, false>(h, p, st, &fit16, false);
+        const int rc = launch_gen_cl8_cs<16, false, false, false>(h, p, st, &fit16, false);
         if (rc) return rc;
         const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
         h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
@@ -3360,14 +3445,7 @@ static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
             if (v == 16 || (v == 8 && h->cl8_8_ok)) h->cl8_cs = v;
         }
     }
-    if (p.cond && p.cond_hop)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true>(h, p, st, nullptr, true)
-                               : launch_gen_cl8_cs<8, true, true>(h, p, st, nullptr, true);
-    if (p.cond)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false>(h, p, st, nullptr, true)
-                               : launch_gen_cl8_cs<8, true, false>(h, p, st, nullptr, true);
-    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false>(h, p, st, nullptr, true)
-                           : launch_gen_cl8_cs<8, false, false>(h, p, st, nullptr, true);
+    return p.ps ? launch_gen_cl8_cond<true>(h, p, st) : launch_gen_cl8_cond<false>(h, p, st);
 }
 
 // 64 CTAs as 4 clusters of 16, all co-resident (the clusters exchange through the L2 while they run): launched with the
@@ -3466,6 +3544,44 @@ extern "C" int wn_gen_set_truncation(wn_gen_handle* h, int top_k, double top_p) 
     return 0;
 }
 
+static bool stream_truncates(const wn_gen_stream_params& q, int classes) {
+    return q.temperature > 0.f && ((q.top_k > 0 && q.top_k < classes) || q.top_p < 1.0);
+}
+
+extern "C" int wn_gen_set_stream_params(wn_gen_handle* h, const wn_gen_stream_params* params) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_stream_params: null handle");
+    if (params == nullptr) {
+        h->sp.clear();
+        return 0;
+    }
+    const int NS = h->shape.n_streams;
+    for (int s = 0; s < NS; ++s) {                          // all records are checked before any is taken
+        const wn_gen_stream_params& q = params[s];
+        WN_REQUIRE(q.n_given >= 1, WN_E_BADARG, "wn_gen_set_stream_params: stream %d: n_given must be >= 1, got %d", s, q.n_given);
+        WN_REQUIRE(q.top_k >= 0, WN_E_BADARG, "wn_gen_set_stream_params: stream %d: top_k must be >= 0 (0: off), got %d", s, q.top_k);
+        WN_REQUIRE(q.top_p > 0.0 && q.top_p <= 1.0, WN_E_BADARG,
+                   "wn_gen_set_stream_params: stream %d: top_p must lie in (0, 1] (1: off), got %g", s, q.top_p);
+        WN_REQUIRE(std::isfinite(q.temperature) && std::isfinite(q.regularize), WN_E_BADARG,
+                   "wn_gen_set_stream_params: stream %d: temperature %g and regularize %g must be finite", s,
+                   (double)q.temperature, (double)q.regularize);
+    }
+    h->sp.assign(params, params + NS);
+    h->sp_max_given = 0;
+    h->sp_head_from = 0x7fffffff;
+    h->sp_any_trunc = h->sp_any_temp = false;
+    for (const wn_gen_stream_params& q : h->sp) {
+        h->sp_max_given = std::max(h->sp_max_given, q.n_given);
+        h->sp_head_from = std::min(h->sp_head_from, q.n_given - 1);
+        h->sp_any_trunc = h->sp_any_trunc || stream_truncates(q, h->shape.classes);
+        h->sp_any_temp = h->sp_any_temp || q.temperature > 0.f;
+    }
+    if (NS > 1) {                                           // one stream: wn_gen_run folds the record into the scalars
+        if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, sizeof(GenStream) * (size_t)NS));
+        h->sp_dirty = true;
+    }
+    return 0;
+}
+
 extern "C" int wn_gen_check(wn_gen_handle* h, void* stream) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_check: null handle");
     int flag = 0;
@@ -3482,9 +3598,20 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
     WN_REQUIRE(a->n_given >= 1 && a->n_samples >= 0 && a->n_evals >= 0 && a->t0 >= 0, WN_E_BADARG, "wn_gen_run: bad counts");
     WN_REQUIRE(a->t0 == h->cur_t, WN_E_STATE, "wn_gen_run: t0=%d does not continue the previous call (expected %d)", a->t0,
                h->cur_t);
-    WN_REQUIRE(a->t0 + a->n_evals <= a->n_given - 1 + a->n_samples, WN_E_BADARG,
-               "wn_gen_run: evaluations [%d,%d) exceed the schedule of %d given + %d samples", a->t0, a->t0 + a->n_evals,
-               a->n_given, a->n_samples);
+    const bool per_stream = !h->sp.empty();
+    if (per_stream) {
+        WN_REQUIRE(a->n_given == h->sp_max_given, WN_E_BADARG,
+                   "wn_gen_run: with per-stream parameters n_given is the pitch of d_first and must equal the longest prompt "
+                   "(%d), got %d", h->sp_max_given, a->n_given);
+        WN_REQUIRE(a->temperature == 0.f && a->regularize == 0.f && h->top_k == 0 && h->top_p == 1.0, WN_E_BADARG,
+                   "wn_gen_run: with per-stream parameters the scalar temperature and regularize must be 0 and the "
+                   "handle's truncation off (the records hold them)");
+        WN_REQUIRE(!h->sp_any_temp || a->d_uniforms, WN_E_BADARG, "wn_gen_run: a stream with temperature > 0 needs d_uniforms");
+    }
+    const int head_from = per_stream ? h->sp_head_from : a->n_given - 1;
+    WN_REQUIRE(a->t0 + a->n_evals <= head_from + a->n_samples, WN_E_BADARG,
+               "wn_gen_run: evaluations [%d,%d) exceed the schedule of %d samples from evaluation %d", a->t0,
+               a->t0 + a->n_evals, a->n_samples, head_from);
     WN_REQUIRE(!(a->temperature > 0.f) || a->d_uniforms, WN_E_BADARG, "wn_gen_run: temperature > 0 needs d_uniforms");
     if (a->n_evals == 0) return 0;
     if (h->base.cond && h->base.cond_hop) {
@@ -3494,6 +3621,18 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                    a->t0 + a->n_evals, f_lo, f_hi, h->base.cond_frame0, h->base.cond_frame0 + h->base.cond_frames);
     }
     cudaStream_t st = (cudaStream_t)stream;
+    if (per_stream && h->shape.n_streams > 1 && h->sp_dirty) {
+        // in stream order, so that a launch still reading the previous records finishes first
+        std::vector<GenStream> recs(h->sp.size());
+        for (size_t s = 0; s < recs.size(); ++s) {
+            const wn_gen_stream_params& q = h->sp[s];
+            recs[s].n_given = q.n_given; recs[s].top_k = q.top_k; recs[s].trunc = stream_truncates(q, h->shape.classes);
+            recs[s].temperature = q.temperature; recs[s].regularize = q.regularize; recs[s].top_p = q.top_p;
+        }
+        WN_CUDA(cudaMemcpyAsync(h->d_sp, recs.data(), sizeof(GenStream) * recs.size(), cudaMemcpyHostToDevice, st));
+        WN_CUDA(cudaStreamSynchronize(st));                   // recs is pageable host memory that dies with this scope
+        h->sp_dirty = false;
+    }
     const int bars_per_eval = 2 * h->shape.n_layers + 2;
     int done = 0;
     while (done < a->n_evals) {
@@ -3507,6 +3646,16 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         p.t0 = a->t0 + done; p.n_evals = n; p.temperature = a->temperature; p.regularize = a->regularize;
         p.top_k = h->top_k; p.top_p = h->top_p;
         p.trunc = a->temperature > 0.f && ((h->top_k > 0 && h->top_k < h->shape.classes) || h->top_p < 1.0);
+        p.ps = nullptr;
+        p.head_from = head_from;
+        if (per_stream && h->shape.n_streams == 1) {           // the single record becomes the scalars (kernels 3, 5 read only those)
+            const wn_gen_stream_params& q = h->sp[0];
+            p.temperature = q.temperature; p.regularize = q.regularize; p.top_k = q.top_k; p.top_p = q.top_p;
+            p.trunc = stream_truncates(q, h->shape.classes);
+        } else if (per_stream) {
+            p.ps = h->d_sp;
+            p.trunc = h->sp_any_trunc;                          // sizes kernel 1's truncation scratch; the records decide
+        }
         WN_CUDA(cudaMemsetAsync(p.bar, 0, sizeof(unsigned), st));
         int rc;
         const bool auto_cluster = h->mode == 0 && h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok);
@@ -3550,6 +3699,7 @@ extern "C" int wn_gen_read_trace(wn_gen_handle* h, long long* host_out, int n, v
 }
 
 extern "C" int wn_gen_destroy(wn_gen_handle* h) {
+    if (h && h->d_sp) cudaFree(h->d_sp);
     delete h;
     return 0;
 }

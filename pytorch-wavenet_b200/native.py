@@ -112,6 +112,11 @@ class GenShape(C.Structure):
                 ("E", C.c_int), ("classes", C.c_int), ("n_streams", C.c_int), ("dilations", C.POINTER(C.c_int))]
 
 
+class GenStreamParams(C.Structure):
+    _fields_ = [("n_given", C.c_int), ("top_k", C.c_int), ("temperature", C.c_float), ("regularize", C.c_float),
+                ("top_p", C.c_double)]
+
+
 class GenRunArgs(C.Structure):
     _fields_ = [("d_first", C.c_void_p), ("n_given", C.c_int),
                 ("d_forced", C.c_void_p), ("d_uniforms", C.c_void_p),
@@ -209,6 +214,7 @@ SIGNATURES = {
     "wn_gen_set_condition": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_set_condition_frames": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3),
     "wn_gen_set_truncation": (C.c_int, [C.c_void_p, C.c_int, C.c_double]),
+    "wn_gen_set_stream_params": (C.c_int, [C.c_void_p, C.POINTER(GenStreamParams)]),
     "wn_gen_kernel_id": (C.c_int, [C.c_void_p]),
     "wn_gen_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_read_trace": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_void_p]),

@@ -1074,41 +1074,62 @@ class _Runtime:
                  want_logits=False, callbacks=None, cond=None, local=None, top_k=0, top_p=1.0):
         """first: (NS, n_given) int array.  Returns (indices (NS, num_samples) int64 ndarray, logits or None, t_end).
         top_k, top_p: the truncation of the temperature draw (wn_gen_set_truncation), set on the handle by every call.
+        Per-stream form (see _stream_plan): first a list of NS 1-D prompts of any lengths, num_samples and the four settings
+        scalars or NS values each, uniforms / forced (NS, >= n_s) matrices or lists.  The prompts are padded into a matrix
+        whose pitch is the longest prompt, the records go to wn_gen_set_stream_params, and the rows of the returned arrays
+        have the launch's pitch (t_end - head_from): row s holds stream s's samples first, then padding.
         callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done.
         cond: the (NS, G) fp32 condition rows of a conditioned model, else None.
         local: (y, hop) of a locally conditioned model, y the (NS, C, F) fp32 series, else None.  The condition table is
         built window by window (at most ``local_table_bytes`` each), and launches are split at the window boundaries."""
-        top_k, top_p = _truncation(top_k, top_p)
+        plan = _stream_plan(first, num_samples, temperature, regularize, top_k, top_p)
         m = self.model
         dev = self.device()
         self.step_session = None             # a generate_fast run restarts the device queues (wavenet_model.py:250)
-        first = np.ascontiguousarray(first, dtype=np.int32)
-        NS, n_given = first.shape
-        if n_given < 1:
-            raise RuntimeError("first_samples must hold at least one sample")
+        first, NS = plan.first, plan.n_streams
+        if plan.per_stream:
+            # the launch's scalars: the pitch of first, the row pitch, no scalar settings (the records hold them)
+            n_given, num_samples, temperature, regularize, top_k, top_p = plan.pitch, plan.n_samples, 0.0, 0.0, 0, 1.0
+        else:
+            n_given, temperature, regularize, top_k, top_p = first.shape[1], plan.temperature[0], plan.regularize[0], \
+                plan.top_k[0], plan.top_p[0]
         s = self.sampler(NS)
         # on every call, so that one call's setting never reaches the next
         native.check(native.lib().wn_gen_set_truncation(s["handle"], top_k, top_p), "gen truncation")
+        native.check(native.lib().wn_gen_set_stream_params(s["handle"], plan.records() if plan.per_stream else None),
+                     "gen stream params")
         stream = torch.cuda.current_stream(dev).cuda_stream
         # the condition table is read by every launch of this run: the sampler entry keeps it alive
         if local is None:
             s["cond"] = None if cond is None else self.packed_weights(stream).cond_table(cond, stream)
             native.check(native.lib().wn_gen_set_condition(s["handle"], native.ptr(s["cond"])), "gen condition")
-        d_first = torch.from_numpy(first).to(dev, non_blocking=True)
         d_out = torch.zeros(NS, max(num_samples, 1), device=dev, dtype=torch.int32)
         d_uni = d_forced = d_logits = None
-        if temperature > 0:
-            if uniforms is None:
-                # exactly the draws np.random.choice would make: one random_sample() per drawn sample
-                uniforms = np.stack([np.random.random_sample(num_samples) for _ in range(NS)])
-            uniforms = np.ascontiguousarray(np.asarray(uniforms, dtype=np.float64).reshape(NS, num_samples))
-            d_uni = torch.from_numpy(uniforms).to(dev, non_blocking=True)
-        if forced is not None:
-            forced = np.ascontiguousarray(np.asarray(forced, dtype=np.int32).reshape(NS, num_samples))
-            d_forced = torch.from_numpy(forced).to(dev, non_blocking=True)
+        if plan.per_stream:
+            if any(t > 0 for t in plan.temperature):
+                if uniforms is None:
+                    # generate_fast's draws, stream by stream in order; a temperature-0 stream draws nothing
+                    uniforms = [np.random.random_sample(n) if t > 0 else np.zeros(0)
+                                for n, t in zip(plan.counts, plan.temperature)]
+                uniforms = plan.rows(uniforms, np.float64, "uniforms", need=[t > 0 for t in plan.temperature])
+                d_uni = torch.from_numpy(uniforms).to(dev, non_blocking=True)
+            if forced is not None:
+                forced = plan.rows(forced, np.int32, "forced")
+                d_forced = torch.from_numpy(forced).to(dev, non_blocking=True)
+        else:
+            if temperature > 0:
+                if uniforms is None:
+                    # exactly the draws np.random.choice would make: one random_sample() per drawn sample
+                    uniforms = np.stack([np.random.random_sample(num_samples) for _ in range(NS)])
+                uniforms = np.ascontiguousarray(np.asarray(uniforms, dtype=np.float64).reshape(NS, num_samples))
+                d_uni = torch.from_numpy(uniforms).to(dev, non_blocking=True)
+            if forced is not None:
+                forced = np.ascontiguousarray(np.asarray(forced, dtype=np.int32).reshape(NS, num_samples))
+                d_forced = torch.from_numpy(forced).to(dev, non_blocking=True)
+        d_first = torch.from_numpy(first).to(dev, non_blocking=True)
         if want_logits:
             d_logits = torch.zeros(NS, max(num_samples, 1), m.classes, device=dev, dtype=torch.float32)
-        total_evals = n_given - 1 + num_samples
+        total_evals = plan.n_evals
         common = dict(d_uni=d_uni, d_forced=d_forced, d_logits=d_logits)
         window = [None]                       # (first frame, frames) of the local-conditioning table the handle holds
 
@@ -1155,6 +1176,122 @@ class _Runtime:
             (forced.nbytes if d_forced is not None else 0)
         self.d2h_bytes_last = NS * num_samples * 4 + (logits.nbytes if want_logits else 0)
         return idx, logits, total_evals
+
+
+class _StreamPlan:
+    """The schedule of one sampler call (see wn_gen_set_stream_params): first the (NS, pitch) int32 prompt matrix (row s
+    holds prompt s, then padding that is never read), n_given / counts the prompt lengths and sample counts, head_from
+    the first evaluation that runs the head, n_samples the row pitch of uniforms / forced / the outputs, n_evals the
+    evaluations of the call; temperature / regularize / top_k / top_p one value per stream.  per_stream: the call needs
+    per-stream records (settings or prompt lengths that differ, or counts given per stream); otherwise it is today's
+    scalar call."""
+
+    def records(self):
+        recs = (native.GenStreamParams * self.n_streams)()
+        for s in range(self.n_streams):
+            recs[s] = native.GenStreamParams(self.n_given[s], self.top_k[s], self.temperature[s], self.regularize[s],
+                                             self.top_p[s])
+        return recs
+
+    def rows(self, v, dtype, name, need=None):
+        """v -- an (NS, >= n_s) matrix or a list of NS 1-D arrays, row s holding stream s's first n_s values -- as the
+        contiguous (NS, n_samples) matrix the kernels read; padding is zero.  need[s] False: stream s's row is not read
+        (a temperature-0 stream's uniforms) and may be short."""
+        out = np.zeros((self.n_streams, self.n_samples), dtype=dtype)
+        if isinstance(v, (list, tuple)):
+            if len(v) != self.n_streams:
+                raise ValueError(f"{name} must hold {self.n_streams} rows, got {len(v)}")
+            rows_ = [np.asarray(r.detach().cpu().numpy() if torch.is_tensor(r) else r).reshape(-1) for r in v]
+        else:
+            a = np.asarray(v.detach().cpu().numpy() if torch.is_tensor(v) else v)
+            if a.ndim != 2 or a.shape[0] != self.n_streams:
+                raise ValueError(f"{name} must be an ({self.n_streams}, >= {max(self.counts, default=0)}) array or a list "
+                                 f"of {self.n_streams} rows, got shape {a.shape}")
+            rows_ = list(a)
+        for s, (r, n) in enumerate(zip(rows_, self.counts)):
+            if need is not None and not need[s]:
+                continue
+            if r.shape[0] < n:
+                raise ValueError(f"{name} row {s} holds {r.shape[0]} values, stream {s} needs {n}")
+            out[s, :n] = r[:n]
+        return out
+
+
+def _is_seq(v):
+    """a per-stream sequence (list, tuple, or an array / tensor of at least one dimension), not a scalar"""
+    return isinstance(v, (list, tuple)) or ((isinstance(v, np.ndarray) or torch.is_tensor(v)) and v.ndim > 0)
+
+
+def _per_stream_values(name, v, n, check):
+    """(values, given per stream): a scalar repeated n times, or a length-n sequence, every value checked"""
+    if not _is_seq(v):
+        if isinstance(v, np.ndarray) or torch.is_tensor(v):
+            v = v.item()
+        return [check(v)] * n, False
+    a = v.detach().cpu().numpy() if torch.is_tensor(v) else v
+    if np.ndim(a) != 1 or len(a) != n:
+        raise ValueError(f"{name} must be a scalar or a sequence of {n} values (one per stream), got shape {np.shape(a)}")
+    return [check(x.item() if isinstance(x, np.generic) else x) for x in a], True
+
+
+def _finite(name):
+    def check(x):
+        if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)) \
+                or not np.isfinite(float(x)):
+            raise ValueError(f"{name} must be a finite real number, got {x!r}")
+        return float(x)
+    return check
+
+
+def _stream_plan(first_samples, num_samples, temperature, regularize, top_k, top_p):
+    """The checked _StreamPlan of a sampler call; ValueError before any device work.  first_samples: an (NS, n_given) int
+    array, or a list of NS 1-D int arrays of any lengths >= 1.  num_samples: an int, or a sequence of NS ints >= 0.
+    temperature, regularize (finite numbers), top_k, top_p (see _truncation): scalars or NS values each.  A scalar
+    call (rectangular prompt, every argument a scalar) keeps today's unchecked scalar temperature and regularize."""
+    plan = _StreamPlan()
+    if isinstance(first_samples, (list, tuple)) and any(
+            (torch.is_tensor(r) and r.dim() != 0) or np.ndim(r) != 0 for r in first_samples):
+        prompts = []
+        for s, r in enumerate(first_samples):
+            a = np.asarray(r.detach().cpu().numpy() if torch.is_tensor(r) else r)
+            if a.ndim != 1 or a.shape[0] < 1 or not (np.issubdtype(a.dtype, np.integer) and a.dtype != np.bool_):
+                raise ValueError(f"first_samples[{s}] must be a 1-D int array of at least one sample, got "
+                                 f"{a.dtype} {a.shape}")
+            prompts.append(a.astype(np.int64))
+    else:
+        first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
+        first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
+        if first.shape[1] < 1:
+            raise RuntimeError("first_samples must hold at least one sample")
+        prompts = list(first)
+    NS = plan.n_streams = len(prompts)
+    plan.n_given = [int(r.shape[0]) for r in prompts]
+
+    def count(x):
+        if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)) or x < 0:
+            raise ValueError(f"num_samples must hold integers >= 0, got {x!r}")
+        return int(x)
+    if _is_seq(num_samples):
+        plan.counts, counts_given = _per_stream_values("num_samples", num_samples, NS, count)
+    else:
+        plan.counts, counts_given = [int(num_samples)] * NS, False
+    plan.temperature, t_given = _per_stream_values("temperature", temperature, NS,
+                                                   _finite("temperature") if _is_seq(temperature) else float)
+    plan.regularize, r_given = _per_stream_values("regularize", regularize, NS,
+                                                  _finite("regularize") if _is_seq(regularize) else float)
+    plan.top_k, k_given = _per_stream_values("top_k", top_k, NS, lambda k: _truncation(k, 1.0)[0])
+    plan.top_p, p_given = _per_stream_values("top_p", top_p, NS, lambda q: _truncation(0, q)[1])
+    ragged = len(set(plan.n_given)) > 1
+    plan.ragged = ragged or counts_given
+    plan.per_stream = plan.ragged or t_given or r_given or k_given or p_given
+    plan.head_from = min(plan.n_given) - 1
+    plan.pitch = max(plan.n_given)
+    plan.n_evals = max(g - 1 + n for g, n in zip(plan.n_given, plan.counts))
+    plan.n_samples = plan.n_evals - plan.head_from
+    plan.first = np.zeros((NS, plan.pitch), dtype=np.int32)
+    for s, r in enumerate(prompts):
+        plan.first[s, :r.shape[0]] = r
+    return plan
 
 
 def _truncation(top_k, top_p):
@@ -1638,22 +1775,83 @@ class WaveNetModel(nn.Module):
         nets a latency kernel for one stream and one thread-block cluster per stream otherwise, which differ at rounding
         level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream.
         local_condition: a locally conditioned model's (n_streams, C, F) series, one per stream (see generate_fast).
-        top_k, top_p: the truncated draw of generate_fast, the same values for every stream."""
-        top_k, top_p = _truncation(top_k, top_p)
-        first = np.asarray(first_samples.detach().cpu().numpy() if torch.is_tensor(first_samples) else first_samples)
-        first = first.astype(np.int64).reshape(first.shape[0], -1) if first.ndim > 1 else first.astype(np.int64)[None, :]
-        cond = self._condition(condition, first.shape[0])
-        local = self._sampler_local(self._local_condition(local_condition, first.shape[0], first.shape[1] - 1 + num_samples),
-                                    first.shape[1] - 1 + num_samples)
+        top_k, top_p: the truncated draw of generate_fast.
+
+        Every stream may have its own job: ``first_samples`` may be a list of n_streams 1-D int arrays of any lengths >= 1,
+        ``num_samples`` a sequence of n_streams counts, ``temperature``, ``regularize``, ``top_k`` and ``top_p`` sequences
+        of n_streams values, ``uniforms`` / ``forced`` (n_streams, >= n_s) arrays or lists whose row s supplies the first
+        n_s entries, and ``local_condition`` a list of (C, F_s) series.  Stream s then gives what
+        ``generate_fast(n_s, first_samples[s], ...)`` with its own settings gives; with ``uniforms=None`` the streams with
+        temperature > 0 draw their n_s uniforms from numpy's global RNG in stream order, so a seeded batch equals seeded
+        generate_fast calls in order.  With a sequence of counts or prompts of different lengths the return is a list of
+        per-stream index arrays (n_s,) [and a list of (n_s, classes) logits]; otherwise it is the arrays above.  Streams
+        that finish early keep running until the longest job is done.  ValueError for a malformed argument, before any
+        device work."""
+        plan = _stream_plan(first_samples, num_samples, temperature, regularize, top_k, top_p)
+        NS = plan.n_streams
+        cond = self._condition(condition, NS)
+        positions = [g - 1 + n for g, n in zip(plan.n_given, plan.counts)]
+        if plan.per_stream:
+            local = self._per_stream_local(local_condition, positions, plan.n_evals)
+            if uniforms is not None:          # the rows are checked here, before any device work
+                plan.rows(uniforms, np.float64, "uniforms", need=[t > 0 for t in plan.temperature])
+            if forced is not None:
+                plan.rows(forced, np.int32, "forced")
+            first, counts = [r[:g] for r, g in zip(plan.first, plan.n_given)], plan.counts
+        else:
+            local = self._sampler_local(self._local_condition(local_condition, NS, plan.n_evals), plan.n_evals)
+            first, counts = plan.first.astype(np.int64), plan.counts[0]
         self.eval()
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
-            idx, logits, _ = rt.generate(num_samples, first, temperature, regularize, uniforms=uniforms,
+            idx, logits, _ = rt.generate(counts, first, temperature, regularize, uniforms=uniforms,
                                          forced=forced, want_logits=return_logits, cond=cond, local=local,
                                          top_k=top_k, top_p=top_p)
         self._export_queues()
         self.train()
+        if plan.ragged:
+            idx = [idx[s, :n] for s, n in enumerate(plan.counts)]
+            logits = [logits[s, :n] for s, n in enumerate(plan.counts)] if return_logits else None
+        elif plan.per_stream:
+            idx = idx[:, :plan.counts[0]]
+            logits = logits[:, :plan.counts[0]] if return_logits else None
         return (idx, logits) if return_logits else idx
+
+    def _per_stream_local(self, local_condition, positions, n_evals):
+        """The sampler's (series, hop) for per-stream jobs (None: no local conditioning).  local_condition: an (NS, C, F)
+        array or a list of NS (C, F_s) series, stream s needing ceil(positions[s] / hop) frames.  Each series is checked
+        and upsampled at its own length (an upsampled position near a series' end depends on the next frame, so a padded
+        batch would change it), then the frame axis is padded with zeros to cover the call's n_evals evaluations; only
+        the discarded outputs of a stream past its own job read the padding."""
+        if not getattr(self, "local_condition_channels", 0) or local_condition is None:
+            return self._sampler_local(self._local_condition(local_condition, len(positions), max(positions)), n_evals)
+        if isinstance(local_condition, (list, tuple)):
+            if len(local_condition) != len(positions):
+                raise ValueError(f"local_condition must hold {len(positions)} series (one per stream), got "
+                                 f"{len(local_condition)}")
+            series = list(local_condition)
+        else:
+            y = local_condition if torch.is_tensor(local_condition) else np.asarray(local_condition)
+            if y.ndim != 3 or y.shape[0] != len(positions):
+                raise ValueError(f"local_condition must be an ({len(positions)}, C, F) array or a list of (C, F_s) series, "
+                                 f"got shape {tuple(y.shape)}")
+            series = [y[s] for s in range(len(positions))]
+        ys = []
+        for s, (y, pos) in enumerate(zip(series, positions)):
+            y = y if torch.is_tensor(y) else np.asarray(y)
+            ys.append(self._local_condition(y[None], 1, pos))
+        upsample = getattr(self, "local_upsample", None) is not None
+        with torch.no_grad(), torch.cuda.device(self._runtime().device()):
+            if upsample:
+                ys = [self._upsample(y.detach(), pos) for y, pos in zip(ys, positions)]
+                hop, width = 1, n_evals
+            else:
+                hop = self.local_condition_hop
+                width = max(max(y.shape[2] for y in ys), -(-n_evals // hop))
+            out = torch.zeros(len(ys), ys[0].shape[1], max(width, 1), device=ys[0].device, dtype=torch.float32)
+            for s, y in enumerate(ys):
+                out[s, :, :min(y.shape[2], out.shape[2])] = y[0, :, :out.shape[2]]
+        return out, hop
 
     def _sampler_local(self, y, evals):
         """The sampler's (series, hop) for the validated frame-rate series ``y`` (None: no local conditioning).  A learned
@@ -1704,6 +1902,9 @@ class WaveNetModel(nn.Module):
                 s = rt.sampler(1)
                 native.check(native.lib().wn_gen_reset(s["handle"], torch.cuda.current_stream(dev).cuda_stream), "gen reset")
                 native.check(native.lib().wn_gen_set_condition(s["handle"], None), "gen condition")
+                # sampler handles are cached per stream count: a per-stream setting of an earlier call must not reach
+                # the queue step's scalar launches
+                native.check(native.lib().wn_gen_set_stream_params(s["handle"], None), "gen stream params")
                 s["cond"] = None
                 ses = dict(sampler=s, t=0, inp=torch.zeros(1, dtype=torch.int32, device=dev),
                            out=torch.zeros(1, dtype=torch.int32, device=dev),
