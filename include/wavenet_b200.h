@@ -474,21 +474,18 @@ int wn_gen_destroy(wn_gen_handle* h);
  *   2  generic flag-in-data exchange through L2 (any shape, any number of streams)
  *   3  single-stream L2 kernel with register-free cooperative polling (k = 2, power-of-two row split)
  *   4  cluster kernel: one 16-CTA thread-block cluster per stream, exchange through distributed shared memory
- *   5  single-stream two-level exchange: kernel 3's grid (64 CTAs x 4 rows) as 4 clusters of 16; values go to the 16 CTAs
- *      of the producer's cluster through distributed shared memory and reach the other clusters through ONE L2 poller per
- *      (cluster, producer) that forwards them by DSMEM (256-wide nets: R = D = S = E = classes = 256).  Measured slower
- *      than kernel 3 (a 16-CTA DSMEM all-to-all costs as much as the L2 one it replaces): selectable, never the default
  *   6  tensor-core cluster kernel: up to 8 streams per thread-block cluster (256-wide nets: R = D = S = E = classes = 256,
  *      k = 2).  The weights of a stage enter shared memory once per 8 streams, as bf16 hi/lo pairs pre-split into MMA
  *      fragment order at wn_gen_reset (wn_gen_workspace_bytes includes the images; wn_gen_weights_changed after in-place
  *      weight updates); dot products are mma.sync m16n8k16 with three MMAs per product (fp32-class: ~1e-6 on the
  *      logits); the exchange is one 512-byte st.async.v4 block per destination CTA, credited to an mbarrier there.
  *      Clusters of 16 CTAs while all of them are co-resident (as reported by the occupancy query), else clusters of 8
- *      CTAs that own two 16-channel slices each (more clusters per wave)
- * Kernels 2, 3 and 5 sum in the same order (bit-identical results); kernel 4 splits rows differently (rounding-level
+ *      CTAs that own two 16-channel slices each (more clusters per wave); wn_gen_create fixes the size
+ * WN_E_BADARG for any other mode (5 included), WN_E_UNSUPP for a kernel that does not apply to the shape.
+ * Kernels 2 and 3 sum in the same order (bit-identical results); kernel 4 splits rows differently (rounding-level
  * differences). */
 int wn_gen_set_mode(wn_gen_handle* h, int mode);
-/* The parameter tensors given to wn_gen_create were written in place (an optimizer step): kernels 1-5 read them on every
+/* The parameter tensors given to wn_gen_create were written in place (an optimizer step): kernels 1-4 read them on every
  * launch and need nothing; kernel 6 keeps pre-split copies, which the next wn_gen_reset rebuilds after this call. */
 int wn_gen_weights_changed(wn_gen_handle* h);
 /* Global conditioning of the sampler: d_cond is a condition table [n_layers][n_streams][2D] (see wn_cond_table); every
@@ -547,9 +544,11 @@ int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer
  * of the LAST evaluation of a launch (single-stream kernel only); this copies the first n stamps to the host. */
 int wn_gen_read_trace(wn_gen_handle* h, long long* host_out, int n, void* stream);
-/* Which kernel wn_gen_run launches in the handle's current mode: the number (1-6) documented at wn_gen_set_mode. */
+/* Which kernel wn_gen_run launches in the handle's current mode: the number (1-4, 6) documented at wn_gen_set_mode, 0 when
+ * none fits in shared memory (wn_gen_run then returns WN_E_UNSUPP). */
 int wn_gen_kernel_id(const wn_gen_handle* h);
-/* how wn_gen_run launches: grid size, block size, dependent exchange stages per evaluation */
+/* how wn_gen_run launches: grid size, block size, dependent exchange stages per evaluation (WN_E_UNSUPP when no kernel
+ * fits, as for wn_gen_run) */
 int wn_gen_launch_info(const wn_gen_handle* h, int* grid, int* block, int* barriers_per_eval);
 
 #ifdef __cplusplus

@@ -191,7 +191,79 @@ __device__ __forceinline__ void row_dot(const float* __restrict__ w, const float
 __device__ __forceinline__ float sigmoid_(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 __device__ __forceinline__ float tanh_(float x) { return 2.f * sigmoid_(2.f * x) - 1.f; }
 
-// ---- top-k / nucleus (top-p) selection, shared by all six kernels (wn_gen_set_truncation states the rule)
+// The argmax of every kernel: one warp over the C logits lg (shared memory), the lowest index wins ties.
+__device__ __forceinline__ int warp_argmax(const float* lg, int C, int lane) {
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int c = lane; c < C; c += 32) {
+        const float x = lg[c];
+        if (x > best || (x == best && c < bi)) { best = x; bi = c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+    }
+    return bi == 0x7fffffff ? 0 : bi;
+}
+
+// argmax (first index wins ties) or numpy.random.choice's inverse-CDF draw, by one warp over C logits in shared memory.
+// Kept out of line so that its fp64 code does not sit in the instruction stream of the per-layer loop.
+__device__ __noinline__ int choose_sample(float* logit_s, double* cdf, int C, int lane, float temperature, const double* u_ptr) {
+    int choice;
+    if (temperature > 0.f) {
+        float m = -INFINITY;
+        for (int c = lane; c < C; c += 32) {
+            const float x = logit_s[c] / temperature;
+            logit_s[c] = x;
+            m = fmaxf(m, x);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        float sum = 0.f;
+        for (int c = lane; c < C; c += 32) {
+            const float e = expf(logit_s[c] - m);
+            logit_s[c] = e;
+            sum += e;
+        }
+        sum = warp_sum(sum);
+        __syncwarp();
+        // numpy.random.choice: float64 cumulative sum of the float32 probabilities, normalised by its last element,
+        // searchsorted(side='right').  The running sum is taken per lane over a contiguous chunk plus a warp scan
+        // (equal to the sequential sum up to float64 rounding, i.e. ~1e-16 relative on the CDF).
+        const int per = (C + 31) / 32;
+        const int c_lo = lane * per, c_hi = min(C, c_lo + per);
+        double run = 0.0;
+        for (int c = c_lo; c < c_hi; ++c) { run += (double)(logit_s[c] / sum); cdf[c] = run; }
+        double incl = run;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const double up = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += up;
+        }
+        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0) excl = 0.0;
+        const double total = __shfl_sync(0xffffffffu, incl, 31);
+        const double u = *u_ptr;
+        const double ut = u * total;
+        int cnt = 0;
+        for (int c = c_lo; c < c_hi; ++c) {
+            const double v = cdf[c] + excl;
+            bool le = v <= ut;
+            if (fabs(v - ut) <= 1e-9 * total) le = (v / total) <= u;       // exact rule only where it can matter
+            cnt += le ? 1 : 0;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        choice = cnt < C ? cnt : C - 1;
+    } else {
+        choice = warp_argmax(logit_s, C, lane);
+    }
+    return choice;
+}
+
+// ---- top-k / nucleus (top-p) selection, shared by all five kernels (wn_gen_set_truncation states the rule)
 // Order-preserving key of a logit: a larger float gets a larger key; -0 is folded onto +0 so that the two tie, as numbers.
 __device__ __forceinline__ unsigned logit_key(float v) {
     const unsigned b = __float_as_uint(v + 0.f);
@@ -491,19 +563,20 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
             const GenStream ss = stream_set(p, s);
             const int samp = t - (ss.n_given - 1);         // sample number this evaluation chooses
             if (samp < 0) continue;                        // still inside its prompt
+            // the logits (written by other CTAs: through the L2) into the warp's scratch
             const float* lg = p.logitbuf + (size_t)s * C;
+            for (int c = lane; c < C; c += 32) pw[c] = __ldcg(lg + c);
+            __syncwarp();
             int choice;
             if (ss.trunc) {
-                // the logits into the warp's scratch (they become its rank keys); probabilities in the truncation
-                // scratch that the host adds past prob only for such launches
-                for (int c = lane; c < C; c += 32) pw[c] = __ldcg(lg + c);
-                __syncwarp();
+                // the logits become the rank keys; probabilities in the truncation scratch that the host adds past prob
+                // only for such launches
                 choice = choose_truncated(pw, reinterpret_cast<unsigned*>(pw), prob + (GEN_WARPS + warp) * C, C, lane,
                                           ss.temperature, ss.top_k, ss.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
             } else if (ss.temperature > 0.f) {
                 float m = -INFINITY;
                 for (int c = lane; c < C; c += 32) {
-                    const float x = __ldcg(lg + c) / ss.temperature;
+                    const float x = pw[c] / ss.temperature;
                     pw[c] = x;
                     m = fmaxf(m, x);
                 }
@@ -533,19 +606,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
                 }
                 choice = __shfl_sync(0xffffffffu, choice, 0);
             } else {
-                float best = -INFINITY;
-                int bi = 0x7fffffff;
-                for (int c = lane; c < C; c += 32) {
-                    const float x = __ldcg(lg + c);
-                    if (x > best || (x == best && c < bi)) { best = x; bi = c; }
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                    if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-                }
-                choice = bi == 0x7fffffff ? 0 : bi;
+                choice = warp_argmax(pw, C, lane);
             }
             if (lane == 0) {
                 idx_s[s] = choice;
@@ -913,52 +974,11 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
             if (ss.trunc) {
                 choice = choose_truncated(lg, reinterpret_cast<unsigned*>(pw), reinterpret_cast<float*>(cw), C, lane,
                                           ss.temperature, ss.top_k, ss.top_p, p.uniforms + (size_t)s * p.n_samples + samp);
-            } else if (ss.temperature > 0.f) {
-                float m = -INFINITY;
-                for (int c = lane; c < C; c += 32) {
-                    const float x = lg[c] / ss.temperature;
-                    pw[c] = x;
-                    m = fmaxf(m, x);
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                float sum = 0.f;
-                for (int c = lane; c < C; c += 32) {
-                    const float e = expf(pw[c] - m);
-                    pw[c] = e;
-                    sum += e;
-                }
-                sum = warp_sum(sum);
-                for (int c = lane; c < C; c += 32) cw[c] = (double)(pw[c] / sum);
-                __syncwarp();
-                // numpy.random.choice: sequential float64 cumulative sum, normalised by its last element,
-                // searchsorted(side='right') == number of normalised entries <= u
-                if (lane == 0) {
-                    double run = 0.0;
-                    for (int c = 0; c < C; ++c) { run += cw[c]; cw[c] = run; }
-                }
-                __syncwarp();
-                const double total = cw[C - 1];
-                const double u = p.uniforms[(size_t)s * p.n_samples + samp];
-                int cnt = 0;
-                for (int c = lane; c < C; c += 32) cnt += ((cw[c] / total) <= u) ? 1 : 0;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-                choice = cnt < C ? cnt : C - 1;
             } else {
-                float best = -INFINITY;
-                int bi = 0x7fffffff;
-                for (int c = lane; c < C; c += 32) {
-                    const float x = lg[c];
-                    if (x > best || (x == best && c < bi)) { best = x; bi = c; }
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                    if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-                }
-                choice = bi == 0x7fffffff ? 0 : bi;
+                for (int c = lane; c < C; c += 32) pw[c] = lg[c];      // choose_sample overwrites its input
+                __syncwarp();
+                choice = choose_sample(pw, cw, C, lane, ss.temperature,
+                                       p.uniforms ? p.uniforms + (size_t)s * p.n_samples + samp : nullptr);
             }
             if (lane == 0) {
                 idx_s[s] = choice;
@@ -1086,73 +1106,6 @@ __device__ __forceinline__ void poll_taps(const uint2* old_slot, unsigned tag_ol
 #define WORKER_SYNC() asm volatile("bar.sync 1, 256;" ::: "memory")
 __device__ __forceinline__ void mbar_arrive_(unsigned long long* b) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
-}
-
-// argmax (first index wins ties) or numpy.random.choice's inverse-CDF draw, by one warp over C logits in shared memory.
-// Kept out of line so that its fp64 code does not sit in the instruction stream of the per-layer loop.
-__device__ __noinline__ int choose_sample(float* logit_s, double* cdf, int C, int lane, float temperature, const double* u_ptr) {
-    int choice;
-    if (temperature > 0.f) {
-        float m = -INFINITY;
-        for (int c = lane; c < C; c += 32) {
-            const float x = logit_s[c] / temperature;
-            logit_s[c] = x;
-            m = fmaxf(m, x);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        float sum = 0.f;
-        for (int c = lane; c < C; c += 32) {
-            const float e = expf(logit_s[c] - m);
-            logit_s[c] = e;
-            sum += e;
-        }
-        sum = warp_sum(sum);
-        __syncwarp();
-        // numpy.random.choice: float64 cumulative sum of the float32 probabilities, normalised by its last element,
-        // searchsorted(side='right').  The running sum is taken per lane over a contiguous chunk plus a warp scan
-        // (equal to the sequential sum up to float64 rounding, i.e. ~1e-16 relative on the CDF).
-        const int per = (C + 31) / 32;
-        const int c_lo = lane * per, c_hi = min(C, c_lo + per);
-        double run = 0.0;
-        for (int c = c_lo; c < c_hi; ++c) { run += (double)(logit_s[c] / sum); cdf[c] = run; }
-        double incl = run;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const double up = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += up;
-        }
-        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-        if (lane == 0) excl = 0.0;
-        const double total = __shfl_sync(0xffffffffu, incl, 31);
-        const double u = *u_ptr;
-        const double ut = u * total;
-        int cnt = 0;
-        for (int c = c_lo; c < c_hi; ++c) {
-            const double v = cdf[c] + excl;
-            bool le = v <= ut;
-            if (fabs(v - ut) <= 1e-9 * total) le = (v / total) <= u;       // exact rule only where it can matter
-            cnt += le ? 1 : 0;
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        choice = cnt < C ? cnt : C - 1;
-    } else {
-        float best = -INFINITY;
-        int bi = 0x7fffffff;
-        for (int c = lane; c < C; c += 32) {
-            const float x = logit_s[c];
-            if (x > best || (x == best && c < bi)) { best = x; bi = c; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-        }
-        choice = bi == 0x7fffffff ? 0 : bi;
-    }
-    return choice;
 }
 
 template <bool PREFETCH, bool TRACE>
@@ -1918,425 +1871,6 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
     cluster_sync_all();                                          // peers may still be storing into this CTA's shared memory
 }
 
-// ================================================================================================ two-level exchange kernel
-// Single stream, the grid of gen_kernel_fast (64 CTAs x 4 rows per stage vector) organised as 4 thread-block clusters of 16.
-// gen_kernel_fast pays, per stage, for an all-to-all in which 64 CTAs poll all 256 {value, tag} pairs through the
-// L2.  Here a value travels two hops instead:
-//   * inside a cluster the producer stores it straight into the shared memory of its 16 CTAs (distributed shared memory)
-//     -- and, once, to the L2 buffer the other kernels use (the ring history needs that anyway);
-//   * between clusters ONE CTA per destination cluster polls it in the L2 -- rank r of cluster c fetches the 32-byte sector
-//     of the four values that rank r of each other cluster produced (3 sectors per stage instead of 64) -- and forwards it
-//     to its 16 cluster peers through DSMEM.
-// Every consumer then spins on its OWN shared memory (no polling storm on hot L2 lines, no staging pass and one CTA barrier
-// per stage instead of two).  Same row ownership, K split, summation order and activations as gen_kernel_fast /
-// gen_kernel_ll: logits and indices are bit-identical to theirs.
-// It measured slower than gen_kernel_fast: the all-to-all inside a 16-CTA cluster alone (tools/dsmem_probe.cu, variant A)
-// is no better than the L2 all-to-all it replaces, and the second hop is added on top.  Kept as mode 5 (selectable, tested bit-identical), never the default.
-__device__ __forceinline__ void wait_local2(const uint2* p, unsigned tag, float& a, float& b) {        // two pairs, 16-byte aligned
-    const unsigned addr = smem_u32(p);
-    unsigned x, y, z, w;
-    asm volatile("ld.volatile.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(addr) : "memory");
-    if (y != tag || w != tag) {
-        const long long t0 = clock64();
-        unsigned spins = 0;
-        do {
-            asm volatile("ld.volatile.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(addr) : "memory");
-            if ((++spins & 1023u) == 0 && clock64() - t0 > GEN_TIMEOUT_CYCLES) asm volatile("trap;");
-        } while (y != tag || w != tag);
-    }
-    a = __uint_as_float(x);
-    b = __uint_as_float(z);
-}
-
-__global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_x2(const GenParams p) {
-    extern __shared__ __align__(16) float sm[];
-    // exchange buffers first: they must sit at the same offset in every CTA (mapa keeps the offset)
-    uint2* Xcur = reinterpret_cast<uint2*>(sm);                  // [2][R]  layer input h, by layer parity
-    uint2* Xz = Xcur + 2 * p.R;                                  // [2][D]  gated activation z, by layer parity
-    uint2* Xhead = Xz + 2 * p.D;                                 // [S + E + C] skip, y1, logits of the current evaluation
-    uint2* old_s = Xhead + (p.S + p.E + p.C);                    // [2][R] prefetched old taps
-    float* part = reinterpret_cast<float*>(old_s + 2 * p.R);     // [2][GEN_WARPS] partial sums, double buffered by stage parity
-    float* skacc = part + 2 * GEN_WARPS;                         // [nS]
-    float* logit_s = skacc + 4;                                  // [C]
-    double* cdf = reinterpret_cast<double*>(logit_s + ((p.C + 3) & ~3));      // [C]
-    float* wbuf = reinterpret_cast<float*>(cdf + p.C);                        // [n_wslots][wslot_floats]
-    unsigned long long* fullb = reinterpret_cast<unsigned long long*>(wbuf + (size_t)p.n_wslots * p.wslot_floats);
-    unsigned long long* emptyb = fullb + 4;
-    GenLayer* lay_s = reinterpret_cast<GenLayer*>(fullb + 8);
-    int* slot_s = reinterpret_cast<int*>(lay_s + p.n_layers);
-    int* misc = slot_s + p.n_layers;                             // [0] current index
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int cta = blockIdx.x, G = gridDim.x;
-    const int rank = (int)cluster_rank(), cl = cta / CL, NCL = G / CL;
-    const int R = p.R, D = p.D, S = p.S, E = p.E, C = p.C, NL = p.n_layers;
-    const int K1 = 2 * R;
-    constexpr int NV = 4;                                        // values per CTA per stage vector (host checks D/G = R/G = ... = 4)
-    const int oV = cta * NV;                                     // first index this CTA owns in every stage vector
-    const int NSLOT = p.n_wslots;
-    // fixed warp -> (row, K-part) assignment per stage kind, as in gen_kernel_fast (same summation order)
-    const int HS1 = GEN_WARPS / (2 * NV), HS2 = GEN_WARPS / (2 * NV), HSA = GEN_WARPS / NV, HSB = GEN_WARPS / NV;
-    const int row1 = warp / HS1, g1 = ((warp - row1 * HS1) * (K1 / HS1) >> 2) + lane, n1 = (((K1 / HS1) >> 2) - lane + 31) / 32;
-    const int row2 = warp / HS2, g2 = ((warp - row2 * HS2) * (D / HS2) >> 2) + lane, n2 = (((D / HS2) >> 2) - lane + 31) / 32;
-    const int rowA = warp / HSA, gA = ((warp - rowA * HSA) * (S / HSA) >> 2) + lane, nA = (((S / HSA) >> 2) - lane + 31) / 32;
-    const int rowB = warp / HSB, gB = ((warp - rowB * HSB) * (E / HSB) >> 2) + lane, nB = (((E / HSB) >> 2) - lane + 31) / 32;
-
-    {   // zero the exchange buffers (tag 0 = nothing yet), copy the layer table
-        unsigned long long* z0 = reinterpret_cast<unsigned long long*>(Xcur);
-        const int n0 = 2 * R + 2 * D + S + E + C + 2 * R;
-        for (int i = tid; i < n0; i += GEN_NT + 32) z0[i] = 0ull;
-        const int* src = reinterpret_cast<const int*>(p.layers);
-        int* dst = reinterpret_cast<int*>(lay_s);
-        for (int i = tid; i < NL * (int)(sizeof(GenLayer) / sizeof(int)); i += GEN_NT + 32) dst[i] = src[i];
-    }
-    if (tid == 0) {
-        misc[0] = p.cur_idx[0];
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(fullb + i, 1); mbar_init(emptyb + i, GEN_WARPS); }
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-    for (int l = tid; l < NL; l += GEN_NT) {
-        const int len = lay_s[l].ring_len;
-        slot_s[l] = (p.t0 + len - 1) % len;
-    }
-    cluster_sync_all();                                          // nobody may store into a peer before it is zeroed
-    const unsigned smask = (unsigned)NSLOT - 1u, sshift = (NSLOT == 4) ? 2u : 1u;
-
-    // ---- producer warp: weight rows of this CTA for every stage, in order, through the TMA ring (as gen_kernel_fast)
-    if (warp == GEN_WARPS) {
-        if (lane == 0) {
-            unsigned q = 0;
-            for (int ev = 0; ev < p.n_evals; ++ev) {
-                const bool wh = (p.t0 + ev >= p.n_given - 1);
-                const int n_st = wh ? 2 * NL + 2 : 2 * NL;
-                for (int st = 0; st < n_st; ++st, ++q) {
-                    StageDesc d = stage_desc(p, st, true, NV, NV, NV, NV, NV);
-                    if (st < 2 * NL && (st & 1)) { d.n_first = NV; d.n = 2 * NV; }
-                    const int slot = (int)(q & smask);
-                    if (q >= (unsigned)NSLOT) {
-                        const unsigned par = ((q >> sshift) & 1u) ^ 1u;
-                        unsigned done = 0, spins = 0;
-                        while (!done) {
-                            asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                                         : "=r"(done) : "r"(smem_u32(emptyb + slot)), "r"(par) : "memory");
-                            if (!done && ++spins > (1u << 30)) asm volatile("trap;");
-                        }
-                    }
-                    mbar_expect_tx(fullb + slot, (unsigned)(d.n * d.K * 4));
-                    float* dst = wbuf + (size_t)slot * p.wslot_floats;
-                    for (int i = 0; i < d.n; ++i)
-                        bulk_g2s(dst + (size_t)i * d.K, stage_row(p, lay_s, st, d, i, cta, G), d.K * 4, fullb + slot);
-                }
-            }
-        }
-        cluster_sync_all();                                      // matches the workers' final cluster barrier
-        return;
-    }
-    unsigned cons_q = 0;
-    auto stage_weights = [&](int row, int K) -> const float* {
-        const int slot = (int)(cons_q & smask);
-        mbar_wait(fullb + slot, (cons_q >> sshift) & 1u);
-        return wbuf + (size_t)slot * p.wslot_floats + (size_t)row * K;
-    };
-    auto release_slot = [&]() {
-        __syncwarp();
-        if (lane == 0) mbar_arrive_(emptyb + (cons_q & smask));
-        ++cons_q;
-    };
-    auto prefetch_old = [&](int ln, int te, int slot_te) {
-        const GenLayer& Lp = lay_s[ln];
-        if (te >= Lp.dil && tid < R / 2) {
-            const int so = (slot_te + 1 == Lp.ring_len) ? 0 : slot_te + 1;
-            const uint2* src = p.ringLL + Lp.ring_off + (size_t)so * R + 2 * tid;
-            const unsigned dst = (unsigned)__cvta_generic_to_shared(old_s + (ln & 1) * R + 2 * tid);
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    // Second hop: warps 4 .. 4+NCL-2 each serve one OTHER cluster: fetch the sector (4 pairs) its rank-`rank` CTA published to
-    // the L2 vector `gvec` (tag gtag) and store it, re-tagged, into vector `xvec` of all 16 CTAs of this cluster.
-    auto forward = [&](const uint2* gvec, unsigned gtag, uint2* xvec, unsigned xtag) {
-        const int k = warp - 4;
-        if (k < 0 || k >= NCL - 1) return;
-        const int cp = (cl + 1 + k) % NCL;
-        const int idx = (cp * CL + rank) * NV + 2 * (lane >> 4);        // lanes 0-15: pairs 0,1; lanes 16-31: pairs 2,3
-        Pair2 q = ld_pair2(gvec + idx);
-        if (q.a.y != gtag || q.b.y != gtag) {
-            const long long t0 = clock64();
-            unsigned spins = 0;
-            do {
-                q = ld_pair2(gvec + idx);
-                if ((++spins & 255u) == 0 && clock64() - t0 > GEN_TIMEOUT_CYCLES) asm volatile("trap;");
-            } while (q.a.y != gtag || q.b.y != gtag);
-        }
-        st_remote_pair(xvec + idx, (unsigned)(lane & 15), __uint_as_float(q.a.x), xtag);
-        st_remote_pair(xvec + idx + 1, (unsigned)(lane & 15), __uint_as_float(q.b.x), xtag);
-    };
-    {
-        const int len0 = lay_s[0].ring_len;
-        prefetch_old(0, p.t0, p.t0 % len0);
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-    }
-    WORKER_SYNC();
-    unsigned stage_par = 0;
-    unsigned seq = (unsigned)p.t0 * (unsigned)(2 * NL + 4);      // exchange tag counter, unique per (evaluation, stage)
-
-    for (int ev = 0; ev < p.n_evals; ++ev) {
-        const int t = p.t0 + ev;
-        const unsigned rtag = (unsigned)t + 1u;                  // tag of time t in the L2 buffers (ring history, exchange vectors)
-        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
-        const int par = t & 1;
-        const bool want_head = (t >= p.n_given - 1);
-        const int samp = t - (p.n_given - 1);
-        if (tid == 0) {
-            if (t < p.n_given) misc[0] = p.first[t];
-            else if (p.forced != nullptr) misc[0] = p.forced[t - p.n_given];
-        }
-        for (int l = tid; l < NL; l += GEN_NT) {
-            const int s1 = slot_s[l] + 1;
-            slot_s[l] = (s1 == lay_s[l].ring_len) ? 0 : s1;
-        }
-        if (tid < NV) skacc[tid] = 0.f;
-        WORKER_SYNC();
-        int idx = misc[0];
-        idx = idx < 0 ? 0 : (idx >= C ? C - 1 : idx);
-        const unsigned etag = seq + 1u;                          // tags of this evaluation: etag + 2l (h of layer l), etag + 2l + 1 (z)
-        seq += (unsigned)(2 * NL + 4);
-
-        // layer 0's input: the start-conv column, computed locally by every CTA; owners also enqueue it in the L2 ring
-        {
-            const GenLayer& L0 = lay_s[0];
-            for (int r = tid; r < R; r += GEN_NT) {
-                const float v = __ldg(p.start_w + (size_t)r * C + idx) + (p.start_b ? __ldg(p.start_b + r) : 0.f);
-                reinterpret_cast<volatile unsigned long long*>(Xcur)[r] =
-                    ((unsigned long long)etag << 32) | (unsigned long long)__float_as_uint(v);
-                if (r >= oV && r < oV + NV) st_pair(p.ringLL + L0.ring_off + (size_t)slot_s[0] * R + r, v, rtag);
-            }
-        }
-
-        for (int l = 0; l < NL; ++l) {
-            const GenLayer& L = lay_s[l];
-            const int slot_t = slot_s[l];
-            const int slot_old = (slot_t + 1 == L.ring_len) ? 0 : slot_t + 1;
-            const bool have_old = (t >= L.dil);
-            const unsigned tag_old = (unsigned)(t - L.dil) + 1u, tag_cur = etag + 2u * (unsigned)l, tag_z = tag_cur + 1u;
-            const uint2* xc = Xcur + (l & 1) * R;
-            const uint2* os = old_s + (l & 1) * R;
-            uint2* zb = Xz + (l & 1) * D;
-            uint2* zl = p.zLL + (size_t)(par * NL + l) * D;
-            // ================= stage 1: filter/gate rows, K = 2R interleaved (old, cur) per channel
-            {
-                const float* w1 = stage_weights(row1, K1);
-                float acc = 0.f;
-                bool old_ok = true;
-                float cc[FAST_MAXI][2];
-#pragma unroll
-                for (int it = 0; it < FAST_MAXI; ++it)
-                    if (it < n1) wait_local2(xc + 2 * (g1 + it * 32), tag_cur, cc[it][0], cc[it][1]);
-#pragma unroll
-                for (int it = 0; it < FAST_MAXI; ++it)
-                    if (it < n1) {
-                        const int g4 = g1 + it * 32, r0 = 2 * g4;
-                        float o0 = 0.f, o1 = 0.f;
-                        if (have_old) {
-                            const uint4 q = *reinterpret_cast<const uint4*>(os + r0);
-                            old_ok = old_ok && q.y == tag_old && q.w == tag_old;
-                            o0 = __uint_as_float(q.x);
-                            o1 = __uint_as_float(q.z);
-                        }
-                        const float4 w4 = reinterpret_cast<const float4*>(w1)[g4];
-                        acc = fmaf(w4.x, o0, acc); acc = fmaf(w4.y, cc[it][0], acc); acc = fmaf(w4.z, o1, acc); acc = fmaf(w4.w, cc[it][1], acc);
-                    }
-                if (!__all_sync(0xffffffffu, old_ok)) {            // prefetched copy not there yet (rare): poll the ring itself
-                    acc = 0.f;
-                    for (int it = 0; it < n1; ++it) {
-                        const int g4 = g1 + it * 32, r0 = 2 * g4;
-                        float o0, o1;
-                        poll2(p.ringLL + L.ring_off + (size_t)slot_old * R + r0, tag_old, o0, o1, p.err, misc + 1);
-                        const float4 w4 = reinterpret_cast<const float4*>(w1)[g4];
-                        acc = fmaf(w4.x, o0, acc); acc = fmaf(w4.y, cc[it][0], acc); acc = fmaf(w4.z, o1, acc); acc = fmaf(w4.w, cc[it][1], acc);
-                    }
-                }
-                acc = warp_sum(acc);
-                if (lane == 0) part[stage_par * GEN_WARPS + warp] = acc;
-                release_slot();
-            }
-            WORKER_SYNC();
-            if (tid < CL * NV) {                                   // publish z: thread -> (value tid / 16, destination CTA tid % 16)
-                const int vi = tid >> 4, c = oV + vi;
-                const float* pf = part + stage_par * GEN_WARPS + (2 * vi) * HS1;
-                float f = pf[0], g = pf[HS1];
-                for (int q = 1; q < HS1; ++q) { f += pf[q]; g += pf[HS1 + q]; }
-                if (ct) {                                          // one stream: the table is [n_layers][1][(frames)][2D]
-                    f += __ldg(ct + (size_t)l * p.cond_sstride + c);
-                    g += __ldg(ct + (size_t)l * p.cond_sstride + D + c);
-                } else {
-                    f += L.bf ? __ldg(L.bf + c) : 0.f;
-                    g += L.bg ? __ldg(L.bg + c) : 0.f;
-                }
-                const float zv = tanh_(f) * sigmoid_(g);
-                st_remote_pair(zb + c, (unsigned)(tid & 15), zv, tag_z);
-                if ((tid & 15) == 0) st_pair(zl + c, zv, rtag);
-            }
-            forward(zl, rtag, zb, tag_z);
-            stage_par ^= 1;
-            // ================= stage 2: residual rows (first NV) and skip rows (next NV), K = D
-            if (l + 1 < NL) prefetch_old(l + 1, t, slot_s[l + 1]);
-            else if (ev + 1 < p.n_evals) prefetch_old(0, t + 1, (slot_s[0] + 1 == lay_s[0].ring_len) ? 0 : slot_s[0] + 1);
-            {
-                const bool active2 = (row2 < NV) ? (l + 1 < NL) : want_head;
-                const float* w2 = stage_weights(row2, D);
-                float acc = 0.f;
-                if (active2) {
-                    float zz[FAST_MAXI][4];
-#pragma unroll
-                    for (int it = 0; it < FAST_MAXI; ++it)
-                        if (it < n2) {
-                            wait_local2(zb + 4 * (g2 + it * 32), tag_z, zz[it][0], zz[it][1]);
-                            wait_local2(zb + 4 * (g2 + it * 32) + 2, tag_z, zz[it][2], zz[it][3]);
-                        }
-#pragma unroll
-                    for (int it = 0; it < FAST_MAXI; ++it)
-                        if (it < n2) {
-                            const float4 w4 = reinterpret_cast<const float4*>(w2)[g2 + it * 32];
-                            acc = fmaf(w4.x, zz[it][0], acc); acc = fmaf(w4.y, zz[it][1], acc); acc = fmaf(w4.z, zz[it][2], acc); acc = fmaf(w4.w, zz[it][3], acc);
-                        }
-                    acc = warp_sum(acc);
-                }
-                if (lane == 0) part[stage_par * GEN_WARPS + warp] = acc;
-                release_slot();
-                asm volatile("cp.async.wait_group 0;" ::: "memory");      // the old taps for the next stage 1 have landed
-            }
-            WORKER_SYNC();
-            if (tid < CL * NV) {
-                if (l + 1 < NL) {                                  // publish h' = Wr z + br + h
-                    const int vi = tid >> 4, row = oV + vi;
-                    const GenLayer& Ln = lay_s[l + 1];
-                    const float* ps = part + stage_par * GEN_WARPS + vi * HS2;
-                    float v = ps[0];
-                    for (int q = 1; q < HS2; ++q) v += ps[q];
-                    v += L.br ? __ldg(L.br + row) : 0.f;
-                    const float hv = v + wait_local(xc + row, tag_cur, misc + 1);
-                    st_remote_pair(Xcur + ((l + 1) & 1) * R + row, (unsigned)(tid & 15), hv, tag_cur + 2u);
-                    if ((tid & 15) == 0) st_pair(p.ringLL + Ln.ring_off + (size_t)slot_s[l + 1] * R + row, hv, rtag);
-                }
-            } else if (tid < CL * NV + NV && want_head) {          // skip rows accumulate locally
-                const int li = tid - CL * NV;
-                const float* ps = part + stage_par * GEN_WARPS + (NV + li) * HS2;
-                float v = ps[0];
-                for (int q = 1; q < HS2; ++q) v += ps[q];
-                v += L.bs ? __ldg(L.bs + oV + li) : 0.f;
-                skacc[li] = v + skacc[li];
-            }
-            if (l + 1 < NL) {
-                const GenLayer& Ln = lay_s[l + 1];
-                forward(p.ringLL + Ln.ring_off + (size_t)slot_s[l + 1] * R, rtag, Xcur + ((l + 1) & 1) * R, tag_cur + 2u);
-            }
-            stage_par ^= 1;
-        }
-        if (!want_head) continue;
-
-        // ================= head
-        const unsigned tag_s = etag + 2u * (unsigned)NL + 1u, tag_y = tag_s + 1u, tag_l = tag_s + 2u;
-        uint2* xs = Xhead, *xy = Xhead + S, *xl = Xhead + S + E;
-        uint2* skl = p.skipLL + (size_t)par * S;
-        uint2* yl = p.y1LL + (size_t)par * E;
-        uint2* lgl = p.logitLL + (size_t)par * C;
-        WORKER_SYNC();                                           // skacc complete
-        if (tid < CL * NV) {
-            const int vi = tid >> 4;
-            st_remote_pair(xs + oV + vi, (unsigned)(tid & 15), skacc[vi], tag_s);
-            if ((tid & 15) == 0) st_pair(skl + oV + vi, skacc[vi], rtag);
-        }
-        forward(skl, rtag, xs, tag_s);
-        {
-            const float* w = stage_weights(rowA, S);
-            float zz[FAST_MAXI][4];
-#pragma unroll
-            for (int it = 0; it < FAST_MAXI; ++it)
-                if (it < nA) {
-                    wait_local2(xs + 4 * (gA + it * 32), tag_s, zz[it][0], zz[it][1]);
-                    wait_local2(xs + 4 * (gA + it * 32) + 2, tag_s, zz[it][2], zz[it][3]);
-                }
-            float acc = 0.f;
-#pragma unroll
-            for (int it = 0; it < FAST_MAXI; ++it)
-                if (it < nA) {
-                    const float4 w4 = reinterpret_cast<const float4*>(w)[gA + it * 32];
-                    acc = fmaf(w4.x, fmaxf(zz[it][0], 0.f), acc); acc = fmaf(w4.y, fmaxf(zz[it][1], 0.f), acc);
-                    acc = fmaf(w4.z, fmaxf(zz[it][2], 0.f), acc); acc = fmaf(w4.w, fmaxf(zz[it][3], 0.f), acc);
-                }
-            acc = warp_sum(acc);
-            if (lane == 0) part[stage_par * GEN_WARPS + warp] = acc;
-            release_slot();
-        }
-        WORKER_SYNC();
-        if (tid < CL * NV) {
-            const int vi = tid >> 4, row = oV + vi;
-            const float* ps = part + stage_par * GEN_WARPS + vi * HSA;
-            float v = ps[0];
-            for (int q = 1; q < HSA; ++q) v += ps[q];
-            v = fmaxf(v + __ldg(p.e1b + row), 0.f);
-            st_remote_pair(xy + row, (unsigned)(tid & 15), v, tag_y);
-            if ((tid & 15) == 0) st_pair(yl + row, v, rtag);
-        }
-        forward(yl, rtag, xy, tag_y);
-        stage_par ^= 1;
-        {
-            const float* w = stage_weights(rowB, E);
-            float zz[FAST_MAXI][4];
-#pragma unroll
-            for (int it = 0; it < FAST_MAXI; ++it)
-                if (it < nB) {
-                    wait_local2(xy + 4 * (gB + it * 32), tag_y, zz[it][0], zz[it][1]);
-                    wait_local2(xy + 4 * (gB + it * 32) + 2, tag_y, zz[it][2], zz[it][3]);
-                }
-            float acc = 0.f;
-#pragma unroll
-            for (int it = 0; it < FAST_MAXI; ++it)
-                if (it < nB) {
-                    const float4 w4 = reinterpret_cast<const float4*>(w)[gB + it * 32];
-                    acc = fmaf(w4.x, zz[it][0], acc); acc = fmaf(w4.y, zz[it][1], acc); acc = fmaf(w4.z, zz[it][2], acc); acc = fmaf(w4.w, zz[it][3], acc);
-                }
-            acc = warp_sum(acc);
-            if (lane == 0) part[stage_par * GEN_WARPS + warp] = acc;
-            release_slot();
-        }
-        WORKER_SYNC();
-        if (tid < CL * NV) {
-            const int vi = tid >> 4, row = oV + vi;
-            const float* ps = part + stage_par * GEN_WARPS + vi * HSB;
-            float v = ps[0];
-            for (int q = 1; q < HSB; ++q) v += ps[q];
-            const float dc = (float)row - (float)C / 2.f;
-            v = (v + __ldg(p.e2b + row)) - (dc * dc) * p.regularize;
-            st_remote_pair(xl + row, (unsigned)(tid & 15), v, tag_l);
-            if ((tid & 15) == 0) {
-                st_pair(lgl + row, v, rtag);
-                if (p.out_logits) p.out_logits[(size_t)samp * C + row] = v;
-            }
-        }
-        forward(lgl, rtag, xl, tag_l);
-        stage_par ^= 1;
-        for (int c = tid; c < C; c += GEN_NT) logit_s[c] = wait_local(xl + c, tag_l, misc + 1);
-        WORKER_SYNC();
-        if (warp == 0) {
-            const int choice = p.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
-                                                          reinterpret_cast<float*>(cdf) + C, C, lane, p.temperature,
-                                                          p.top_k, p.top_p, p.uniforms + samp)
-                                       : choose_sample(logit_s, cdf, C, lane, p.temperature, p.uniforms ? p.uniforms + samp : nullptr);
-            if (lane == 0) {
-                misc[0] = choice;
-                if (cta == 0) p.out_idx[samp] = choice;
-            }
-        }
-        // the top-of-evaluation barrier publishes misc[0]
-    }
-    WORKER_SYNC();
-    if (cta == 0 && tid == 0) p.cur_idx[0] = misc[0];
-    cluster_sync_all();                                          // peers may still be storing into this CTA's shared memory
-}
-
 // ================================================================================================ batched cluster kernel
 // Tensor-core sampler for 256-wide nets (R = D = S = E = classes = 256, k = 2), one stream or many: a thread-block cluster
 // advances up to CL8_SB = 8 independent streams together, so the weights of a stage enter shared memory ONCE per 8 streams
@@ -3027,7 +2561,7 @@ struct wn_gen_handle {
     size_t smem;
     bool tables_uploaded;
     int cur_t;
-    int mode;               // 0 = best kernel for the shape (default), 1 = grid barrier, 2 = generic flag-in-data, 3-5 see wn_gen_set_mode
+    int mode;               // what wn_gen_set_mode stored (0 = best kernel for the shape, the default); pick_kernel decides
     size_t smem_ll;
     bool fast_ok;           // single stream, k=2, power-of-two grid, rows per stage divide 8: gen_kernel_fast applies
     size_t smem_fast;
@@ -3039,11 +2573,8 @@ struct wn_gen_handle {
     bool cl8_ok, cl8_packed;   // gen_kernel_cl8 applies (cl8_shape_ok and the shared memory fits); its weight images are built
     bool generic_ok, ll_ok;    // the grid-barrier / the generic flag-exchange kernel fit in shared memory for this stream count
     bool cl8_8_ok;             // ... and so does its 8-CTA-cluster instantiation
-    int cl8_cs;                // cluster size picked at the first launch (0 = not yet)
+    int cl8_cs;                // its cluster size, 16 or 8 (wn_gen_create)
     size_t smem_cl8, smem_cl8_8;
-    bool x2_ok;             // fast_ok on a 64-CTA grid with 4 rows per stage vector per CTA: gen_kernel_x2 applies
-    size_t smem_x2;
-    int n_wslots_x2;
     int top_k;              // wn_gen_set_truncation (0, 1.0: off)
     double top_p;
     // wn_gen_set_stream_params: the host records (empty: the scalar path), their device copy (allocated at the first call,
@@ -3070,6 +2601,56 @@ extern "C" int wn_gen_workspace_bytes(const wn_gen_shape* s, size_t* ring_bytes,
     return 0;
 }
 
+// The batched cluster kernel's launch at cluster size cs; attr holds the cluster dimension that cfg points to.
+static cudaLaunchConfig_t cl8_config(const wn_gen_handle* h, int cs, cudaStream_t st, cudaLaunchAttribute* attr) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * cs));
+    cfg.blockDim = dim3(GEN_NT + 64 + (cs == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
+    cfg.dynamicSmemBytes = cs == 16 ? h->smem_cl8 : h->smem_cl8_8;
+    cfg.stream = st;
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = cs;
+    attr->val.clusterDim.y = 1;
+    attr->val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cfg;
+}
+
+// Cluster size of the batched cluster kernel: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8
+// (15 clusters fit instead of 7).  WN_GEN_CL8_CS=16|8 forces one (8 only where it fits).
+static int choose_cl8_cs(wn_gen_handle* h) {
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cl8_config(h, 16, nullptr, &attr);
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<16, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)cfg.dynamicSmemBytes));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<16, false, false, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    int fit16 = 0;
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&fit16, gen_kernel_cl8<16, false, false, false>, &cfg));
+    const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
+    h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
+    if (const char* e = getenv("WN_GEN_CL8_CS")) {
+        const int v = atoi(e);
+        if (v == 16 || (v == 8 && h->cl8_8_ok)) h->cl8_cs = v;
+    }
+    return 0;
+}
+
+// The kernel wn_gen_run launches in the handle's mode (the mode number of wn_gen_set_mode), 0 when none fits.
+static int pick_kernel(const wn_gen_handle* h) {
+    const int m = h->mode;
+    if (m == 3 || m == 4 || m == 6) return m;               // wn_gen_set_mode accepts these only where they apply
+    if (m == 0) {
+        if (h->cl8_ok) return 6;                            // any number of streams of a 256-wide net
+        if (h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok)) return 4;
+        // kernel 3 only where kernel 2 or 4 fits too: a net too deep for kernel 2's shared memory (on an H100 from ~2 240
+        // layers of 256 channels with 512 end channels and classes) keeps kernel 1, which auto has always run there
+        if (h->fast_ok && (h->ll_ok || h->cluster_ok)) return 3;
+    }
+    if (m != 1 && h->ll_ok) return 2;                       // modes 0 and 2
+    return h->generic_ok ? 1 : 0;
+}
+
 extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, float* d_rings, void* d_scratch,
                              wn_gen_handle** out) {
     if (int rc = validate_shape(s)) return rc;
@@ -3085,6 +2666,7 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     wn_gen_handle* h = new (std::nothrow) wn_gen_handle();
     WN_REQUIRE(h, WN_E_BADARG, "wn_gen_create: out of host memory");
     h->shape = *s;
+    h->mode = 0;
     h->top_k = 0;
     h->top_p = 1.0;
     h->d_sp = nullptr;
@@ -3155,10 +2737,9 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     p.skacc_n = (p.skacc_n + 3) / 4 * 4;
     h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + NS + (size_t)GEN_WARPS * s->classes);
     // the grid-barrier / generic kernels stage all streams' vectors in every CTA; the cluster kernels do not
-    h->generic_ok = h->smem <= (size_t)smem_optin;
     const bool cluster_shape = s->k == 2 && s->n_layers >= 2 && s->D % CL == 0 && s->R % CL == 0 && s->S % CL == 0 &&
                                s->E % CL == 0 && s->classes % CL == 0;
-    if (!h->generic_ok && !cluster_shape) {
+    if (h->smem > (size_t)smem_optin && !cluster_shape) {
         const size_t need = h->smem;
         delete h;
         return set_err(WN_E_UNSUPP, "wn_gen_create: %zu bytes of shared memory needed for %d streams, %d available", need,
@@ -3204,7 +2785,6 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
             p.regA = regA_ll;
             h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + NS + (size_t)GEN_WARPS * s->classes);
         }
-        h->mode = (s->n_layers >= 2 && h->smem_ll <= (size_t)smem_optin) ? 0 : 1;
         // ---- fast kernel eligibility (same K split as the generic kernel so both sum in the same order)
         auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
         auto split_ok = [&](int rows, int K) {
@@ -3238,23 +2818,6 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
             h->n_wslots_fast = fs;
             h->smem_fast = fbase + (size_t)fs * slot * 4;
             h->fast_ok = h->smem_fast <= (size_t)smem_optin;
-        }
-        // ---- two-level exchange kernel: the fast kernel's grid as clusters of 16, exactly 4 values per CTA per stage vector
-        h->x2_ok = false;
-        if (ok && G % CL == 0 && G / CL >= 1 && G / CL <= 5 && s->D / G == 4 && s->R / G == 4 && s->S / G == 4 &&
-            s->E / G == 4 && s->classes / G == 4 && !getenv("WN_GEN_NOX2")) {
-            const size_t xbase = sizeof(uint2) * (size_t)(2 * s->R + 2 * s->D + s->S + s->E + s->classes + 2 * s->R) +
-                                 sizeof(float) * (size_t)(2 * GEN_WARPS + 4 + ((s->classes + 3) & ~3)) +
-                                 sizeof(double) * s->classes + 64 + sizeof(GenLayer) * (size_t)s->n_layers +
-                                 sizeof(int) * (size_t)(s->n_layers + 4);
-            int xs = 0;
-            if (xbase < (size_t)smem_optin) {
-                long long fit = ((long long)smem_optin - (long long)xbase) / (slot * 4);
-                xs = fit >= 4 ? 4 : (fit >= 2 ? 2 : 0);
-            }
-            h->n_wslots_x2 = xs;
-            h->smem_x2 = xbase + (size_t)xs * slot * 4;
-            h->x2_ok = xs >= 2 && h->smem_x2 <= (size_t)smem_optin;
         }
     }
     // ---- cluster kernel eligibility: rows of every stage split evenly over 16 CTAs x 8 warps, <= 4 rows per warp
@@ -3302,18 +2865,20 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
         h->smem_cl8_8 = smem_for(2);
         h->cl8_ok = cl8_shape_ok(*s) && h->smem_cl8 <= (size_t)smem_optin && !getenv("WN_GEN_NOCL8");
         h->cl8_8_ok = h->cl8_ok && h->smem_cl8_8 <= (size_t)smem_optin;
-        h->cl8_cs = 0;
         h->cl8_packed = false;
         p.cl8_img = reinterpret_cast<const unsigned char*>(h->scratch + h->lay.cl8_img);
     }
     h->generic_ok = h->smem <= (size_t)smem_optin;
     h->ll_ok = h->smem_ll <= (size_t)smem_optin && s->n_layers >= 2;
-    if (h->mode == 1 && (h->cl8_ok || h->cluster_ok)) h->mode = 0;       // many streams: only the cluster kernels fit
     if (!h->generic_ok && !h->cl8_ok && !h->cluster_ok) {
         const size_t need = h->smem > h->smem_ll ? h->smem : h->smem_ll;
         delete h;
         return set_err(WN_E_UNSUPP, "wn_gen_create: %zu bytes of shared memory needed for %d streams, %d available", need,
                        s->n_streams, smem_optin);
+    }
+    if (int rc = h->cl8_ok ? choose_cl8_cs(h) : 0) {
+        delete h;
+        return rc;
     }
     h->tables_uploaded = false;
     h->cur_t = 0;
@@ -3397,26 +2962,14 @@ static int launch_gen_cluster(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
 }
 
 template <int CS, bool COND, bool FRAMES, bool PS>
-static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, int* max_clusters_out, bool launch) {
-    const size_t smem = (CS == 16) ? h->smem_cl8 : h->smem_cl8_8;
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cl8_config(h, CS, st, &attr);
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)cfg.dynamicSmemBytes));
     WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * CS));
-    cfg.blockDim = dim3(GEN_NT + 64 + (CS == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     int max_clusters = 0;
     WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND, FRAMES, PS>, &cfg));
-    if (max_clusters_out) *max_clusters_out = max_clusters;
-    if (!launch) return 0;
     WN_REQUIRE(max_clusters >= 1, WN_E_UNSUPP, "wn_gen_run: a %d-CTA cluster cannot be scheduled on this device", CS);
     WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND, FRAMES, PS>, p));   // clusters are independent: more than fit run in waves
     return 0;
@@ -3424,56 +2977,13 @@ static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st, in
 template <bool PS>
 static int launch_gen_cl8_cond(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     if (p.cond && p.cond_hop)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true, PS>(h, p, st, nullptr, true)
-                               : launch_gen_cl8_cs<8, true, true, PS>(h, p, st, nullptr, true);
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true, PS>(h, p, st) : launch_gen_cl8_cs<8, true, true, PS>(h, p, st);
     if (p.cond)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false, PS>(h, p, st, nullptr, true)
-                               : launch_gen_cl8_cs<8, true, false, PS>(h, p, st, nullptr, true);
-    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false, PS>(h, p, st, nullptr, true)
-                           : launch_gen_cl8_cs<8, false, false, PS>(h, p, st, nullptr, true);
+        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false, PS>(h, p, st) : launch_gen_cl8_cs<8, true, false, PS>(h, p, st);
+    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false, PS>(h, p, st) : launch_gen_cl8_cs<8, false, false, PS>(h, p, st);
 }
-// Cluster size: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8 (15 clusters fit instead of 7).
 static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
-    if (h->cl8_cs == 0) {
-        int fit16 = 0;
-        const int rc = launch_gen_cl8_cs<16, false, false, false>(h, p, st, &fit16, false);
-        if (rc) return rc;
-        const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
-        h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
-        if (const char* e = getenv("WN_GEN_CL8_CS")) {
-            const int v = atoi(e);
-            if (v == 16 || (v == 8 && h->cl8_8_ok)) h->cl8_cs = v;
-        }
-    }
     return p.ps ? launch_gen_cl8_cond<true>(h, p, st) : launch_gen_cl8_cond<false>(h, p, st);
-}
-
-// 64 CTAs as 4 clusters of 16, all co-resident (the clusters exchange through the L2 while they run): launched with the
-// cluster dimension AND the cooperative attribute, which makes the driver refuse the launch unless every CTA fits at once.
-static int launch_gen_x2(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_x2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_x2));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_x2, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)h->grid);
-    cfg.blockDim = dim3(GEN_NT + 32);
-    cfg.dynamicSmemBytes = h->smem_x2;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeCooperative;
-    attr[1].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int max_clusters = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_x2, &cfg));
-    WN_REQUIRE(max_clusters >= h->grid / CL, WN_E_UNSUPP, "wn_gen_run: %d clusters of %d CTAs cannot be co-resident (%d fit)",
-               h->grid / CL, CL, max_clusters);
-    cfg.numAttrs = 2;
-    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_x2, p));
-    return 0;
 }
 
 template <bool PF, bool TRACE>
@@ -3495,12 +3005,11 @@ static int launch_gen_fast(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
 
 extern "C" int wn_gen_set_mode(wn_gen_handle* h, int mode) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_mode: null handle");
-    WN_REQUIRE(mode >= 0 && mode <= 6, WN_E_BADARG,
+    WN_REQUIRE(mode >= 0 && mode <= 6 && mode != 5, WN_E_BADARG,
                "wn_gen_set_mode: mode must be 0 (auto), 1 (grid barrier), 2 (generic flag exchange), 3 (single-stream L2 kernel), "
-               "4 (cluster / DSMEM kernel), 5 (single-stream two-level exchange kernel) or 6 (batched tensor-core cluster kernel)");
+               "4 (cluster / DSMEM kernel) or 6 (batched tensor-core cluster kernel), got %d", mode);
     if (mode == 3) WN_REQUIRE(h->fast_ok, WN_E_UNSUPP, "wn_gen_set_mode: the single-stream L2 kernel does not apply to this shape");
     if (mode == 4) WN_REQUIRE(h->cluster_ok, WN_E_UNSUPP, "wn_gen_set_mode: the cluster kernel does not apply to this shape");
-    if (mode == 5) WN_REQUIRE(h->x2_ok, WN_E_UNSUPP, "wn_gen_set_mode: the two-level exchange kernel does not apply to this shape");
     if (mode == 6) WN_REQUIRE(h->cl8_ok, WN_E_UNSUPP, "wn_gen_set_mode: the batched cluster kernel does not apply to this shape");
     WN_REQUIRE(h->cur_t == 0, WN_E_STATE, "wn_gen_set_mode: switch kernels only right after wn_gen_reset");
     if (mode != 1) WN_REQUIRE(h->shape.n_layers >= 2, WN_E_UNSUPP, "wn_gen_set_mode: flag exchange needs >= 2 layers");
@@ -3620,6 +3129,10 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                    "wn_gen_run: evaluations [%d,%d) read frames [%d,%d], outside the condition window [%d,%d)", a->t0,
                    a->t0 + a->n_evals, f_lo, f_hi, h->base.cond_frame0, h->base.cond_frame0 + h->base.cond_frames);
     }
+    const int kid = pick_kernel(h);
+    WN_REQUIRE(kid != 0, WN_E_UNSUPP,
+               "wn_gen_run: %d streams need a cluster kernel (modes 4, 6) for this net; mode %d does not fit in shared memory",
+               h->shape.n_streams, h->mode);
     cudaStream_t st = (cudaStream_t)stream;
     if (per_stream && h->shape.n_streams > 1 && h->sp_dirty) {
         // in stream order, so that a launch still reading the previous records finishes first
@@ -3648,7 +3161,7 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         p.trunc = a->temperature > 0.f && ((h->top_k > 0 && h->top_k < h->shape.classes) || h->top_p < 1.0);
         p.ps = nullptr;
         p.head_from = head_from;
-        if (per_stream && h->shape.n_streams == 1) {           // the single record becomes the scalars (kernels 3, 5 read only those)
+        if (per_stream && h->shape.n_streams == 1) {           // the single record becomes the scalars (kernel 3 reads only those)
             const wn_gen_stream_params& q = h->sp[0];
             p.temperature = q.temperature; p.regularize = q.regularize; p.top_k = q.top_k; p.top_p = q.top_p;
             p.trunc = stream_truncates(q, h->shape.classes);
@@ -3658,29 +3171,27 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         }
         WN_CUDA(cudaMemsetAsync(p.bar, 0, sizeof(unsigned), st));
         int rc;
-        const bool auto_cluster = h->mode == 0 && h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok);
-        if ((h->mode == 0 || h->mode == 6) && h->cl8_ok) {       // several streams of a 256-wide net: 8 streams per cluster
+        switch (kid) {
+        case 6:                                              // several streams of a 256-wide net: 8 streams per cluster
             rc = launch_gen_cl8(h, p, st);
-        } else if ((auto_cluster || h->mode == 4) && h->cluster_ok) {
+            break;
+        case 4:
             p.n_wslots = h->n_wslots_cluster;
             p.wslot_floats = h->wslot_cluster;
             rc = launch_gen_cluster(h, p, st);
-        } else if (h->mode == 5 && h->x2_ok) {                // never picked automatically: measured slower than kernel 3
-            p.n_wslots = h->n_wslots_x2;
-            rc = launch_gen_x2(h, p, st);
-        } else if ((h->mode == 0 || h->mode == 3) && h->fast_ok) {
+            break;
+        case 3:
             p.n_wslots = h->n_wslots_fast;
             p.regA = h->xn_fast;                    // the fast kernel reads its input-vector pitch from regA
             rc = p.n_wslots ? launch_gen_fast<true>(h, p, st) : launch_gen_fast<false>(h, p, st);
-        } else if (!(((h->mode == 0 || h->mode == 2) && h->ll_ok) || h->generic_ok)) {
-            return set_err(WN_E_UNSUPP, "wn_gen_run: %d streams need a cluster kernel (modes 4, 6) for this net; mode %d does not fit in "
-                           "shared memory", h->shape.n_streams, h->mode);
-        } else if ((h->mode == 0 || h->mode == 2) && h->ll_ok) {
+            break;
+        case 2:
             if (h->shape.n_streams == 1)
                 rc = p.n_wslots ? launch_gen_ll<1, true>(h, p, st) : launch_gen_ll<1, false>(h, p, st);
             else
                 rc = p.n_wslots ? launch_gen_ll<8, true>(h, p, st) : launch_gen_ll<8, false>(h, p, st);
-        } else {
+            break;
+        default:
             rc = (h->shape.n_streams == 1) ? launch_gen<1>(h, p, st) : launch_gen<8>(h, p, st);
         }
         if (rc) return rc;
@@ -3704,27 +3215,23 @@ extern "C" int wn_gen_destroy(wn_gen_handle* h) {
     return 0;
 }
 
-/* the kernel wn_gen_run picks in the handle's current mode: the mode number (1-6) of wn_gen_set_mode */
-extern "C" int wn_gen_kernel_id(const wn_gen_handle* h) {
-    if (!h) return 0;
-    const bool auto_cluster = h->mode == 0 && h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok);
-    if ((h->mode == 0 || h->mode == 6) && h->cl8_ok) return 6;
-    if ((auto_cluster || h->mode == 4) && h->cluster_ok) return 4;
-    if (h->mode == 5 && h->x2_ok) return 5;
-    if ((h->mode == 0 || h->mode == 3) && h->fast_ok) return 3;
-    if ((h->mode == 0 || h->mode == 2) && h->ll_ok) return 2;
-    return 1;
-}
+/* the kernel wn_gen_run picks in the handle's current mode: the mode number (1-4, 6) of wn_gen_set_mode, 0 when none fits */
+extern "C" int wn_gen_kernel_id(const wn_gen_handle* h) { return h ? pick_kernel(h) : 0; }
 
 extern "C" int wn_gen_launch_info(const wn_gen_handle* h, int* grid, int* block, int* barriers_per_eval) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_launch_info: null handle");
-    // the kernel wn_gen_run would pick in the handle's current mode (same selection as in wn_gen_run)
-    const bool auto_cluster = h->mode == 0 && h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok);
-    const bool cl8 = (h->mode == 0 || h->mode == 6) && h->cl8_ok;
-    const bool cluster = !cl8 && (auto_cluster || h->mode == 4) && h->cluster_ok;
-    const bool fast = !cluster && ((h->mode == 5 && h->x2_ok) || ((h->mode == 0 || h->mode == 3) && h->fast_ok));
-    if (grid) *grid = cl8 ? (h->shape.n_streams + CL8_SB - 1) / CL8_SB * (h->cl8_cs ? h->cl8_cs : CL) : cluster ? h->shape.n_streams * CL : h->grid;
-    if (block) *block = cl8 ? GEN_NT + 64 + (h->cl8_cs == 8 ? 32 : 0) : (cluster || fast) ? GEN_NT + 32 : GEN_NT;   // + helper warps
+    const int kid = pick_kernel(h);
+    WN_REQUIRE(kid != 0, WN_E_UNSUPP, "wn_gen_launch_info: no sampler kernel fits this net in mode %d", h->mode);
+    int g = kid == 4 ? h->shape.n_streams * CL : h->grid;
+    int b = (kid == 4 || kid == 3) ? GEN_NT + 32 : GEN_NT;                      // + the helper warp
+    if (kid == 6) {
+        cudaLaunchAttribute attr;
+        const cudaLaunchConfig_t cfg = cl8_config(h, h->cl8_cs, nullptr, &attr);
+        g = (int)cfg.gridDim.x;
+        b = (int)cfg.blockDim.x;
+    }
+    if (grid) *grid = g;
+    if (block) *block = b;
     if (barriers_per_eval) *barriers_per_eval = 2 * h->shape.n_layers + 2;      // exchange stages per evaluation
     return 0;
 }

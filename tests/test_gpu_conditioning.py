@@ -105,7 +105,7 @@ def test_zero_condition_is_identity_in_every_sampler(cs, monkeypatch):
                 v.zero_()
     first = np.random.RandomState(0).randint(0, 256, (3, 20))
     for ns in (1, 3):
-        for mode in range(1, 7):
+        for mode in (1, 2, 3, 4, 6):
             res = []
             for m, cond in ((m0, None), (m1, [2, 0, 1][:ns])):
                 m._runtime().gen_mode = mode
@@ -323,7 +323,7 @@ def test_batched_streams_equal_single_stream_runs(mode, cs, monkeypatch):
     assert len({tuple(r) for r in idx}) > 1                # distinct conditions give distinct streams
 
 
-@pytest.mark.parametrize("mode", [1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("mode", [1, 2, 3, 4, 6])
 def test_sampler_matches_folded_oracle(mode):
     G, NS = 4, 3
     kw = _kw(256, 3, 1, 16)
@@ -340,7 +340,7 @@ def test_sampler_matches_folded_oracle(mode):
     cond = np.random.RandomState(4).randn(NS, G).astype(np.float32)
     refs = [O.generate_fast({k: v.float() for k, v in _folded(p, spec, _h(cond, G)[s]).items()}, spec, 24,
                             first_samples=first[s], temperature=0.0, keep_logits=True) for s in range(NS)]
-    ns = 1 if mode in (3, 5) else NS
+    ns = 1 if mode == 3 else NS
     forced = np.stack([r.indices for r in refs[:ns]])
     try:
         _, logits = m.generate_fast_batch(24, first[:ns], temperature=0.0, forced=forced, return_logits=True,

@@ -24,7 +24,7 @@ def _runs(rt, m, first, uni, forced):
 
 @pytest.mark.parametrize("cs", [16, 8])
 def test_live_streams_bitwise_vs_full_cluster(golden, monkeypatch, cs):
-    monkeypatch.setenv("WN_GEN_CL8_CS", str(cs))      # read at a sampler handle's first launch: a fresh model per setting
+    monkeypatch.setenv("WN_GEN_CL8_CS", str(cs))      # read when a sampler handle is created: a fresh model per setting
     m = build_model(golden("net_cfg2.npz"))
     rt = m._runtime()
     rt.gen_mode = 6

@@ -187,37 +187,25 @@ def test_fast_kernel_equals_generic_kernel_bitwise(golden):
     assert np.array_equal(a, b) and len(calls) > 3
 
 
-def test_two_level_exchange_kernel_bitwise_and_golden(golden):
-    """cfg 2 net, single stream: the two-level exchange kernel (mode 5: DSMEM inside a cluster, one L2 poller per remote
-    producer) keeps kernel 3's row split and summation order -- logits and indices identical bit for bit, over warm-up
-    samples, sampling with temperature, chunked launches that continue a session, and the golden teacher-forced stream.
-    The golden stream is 48 evaluations from reset rings (the receptive field is 5 116, so every layer of dilation >= 64
-    reads a zero history); runs past the receptive field against a reference are in test_gpu_generate_long.py."""
+def test_fast_kernel_long_chunked(golden):
+    """cfg 2 net, single stream, kernel 3: the golden teacher-forced stream, and a 700-sample argmax run in chunked
+    launches that continue a session equal to one launch.  The golden stream is 48 evaluations from reset rings (the
+    receptive field is 5 116, so every layer of dilation >= 64 reads a zero history); runs past the receptive field against
+    a reference are in test_gpu_generate_long.py."""
     g = golden("net_cfg2.npz")
     m = build_model(g)
     rt = m._runtime()
-    rng = np.random.RandomState(5)
-    first = rng.randint(0, 256, size=(2, 11))
-    uni = rng.random_sample((2, 300))
-    out = {}
-    for mode in (5, 3):
-        rt.gen_mode = mode
-        out[mode] = [m.generate_fast_batch(300, first[s:s + 1], temperature=1.0, uniforms=uni[s:s + 1], return_logits=True)
-                     for s in range(2)]
-        _, lg = m.generate_fast_batch(48, np.array([[128]]), temperature=0.0, forced=g["gen_argmax_idx"][None, :],
-                                      return_logits=True)
-        assert rel_err(lg[0], g["gen_argmax_logits"]) < TOL
-    for s in range(2):
-        assert np.array_equal(out[5][s][0], out[3][s][0]) and np.array_equal(out[5][s][1], out[3][s][1])
-    rt.gen_mode = 5
+    first = np.random.RandomState(5).randint(0, 256, size=(2, 11))
+    rt.gen_mode = 3
+    _, lg = m.generate_fast_batch(48, np.array([[128]]), temperature=0.0, forced=g["gen_argmax_idx"][None, :],
+                                  return_logits=True)
+    assert rel_err(lg[0], g["gen_argmax_logits"]) < TOL
     calls = []
     a = m.generate_fast(700, first_samples=first[0], temperature=0.0, progress_callback=lambda i, n: calls.append(i),
                         progress_interval=64)
     b = m.generate_fast(700, first_samples=first[0], temperature=0.0)
-    rt.gen_mode = 3
-    c = m.generate_fast(700, first_samples=first[0], temperature=0.0)
     rt.gen_mode = None
-    assert np.array_equal(a, b) and np.array_equal(b, c) and len(calls) > 3
+    assert np.array_equal(a, b) and len(calls) > 3
 
 
 def test_cluster_kernel_cfg2(golden):

@@ -30,7 +30,7 @@ from test_gpu_generate_truncated import _selections, _uniforms
 pytestmark = pytest.mark.gpu
 
 # kernels 1, 2, 4 and 6 at clusters of 16 and of 8
-PS_CASES = [K256[i] for i in (7, 6, 2, 4, 5)]
+PS_CASES = [K256[i] for i in (6, 5, 2, 3, 4)]
 # (temperature, regularize, top_k, top_p, prompt length, samples) of the 11 streams of the mixed launch
 MIXED = [(0.0, 0.0, 0, 1.0, 1, 1000), (1.0, 0.0, 0, 1.0, 2, 700), (0.8, 1e-4, 50, 1.0, 5, 400),
          (1.2, 0.0, 0, 0.9, 600, 300), (1.0, 1e-4, 40, 0.95, 5200, 5), (0.0, 1e-4, 0, 1.0, 5, 0),

@@ -254,7 +254,7 @@ def test_sampler_kernels_match_reference(cs, monkeypatch):
     want = _ref_logits(m, spec, first, forced, y, hop, h, n)
     free = [_ref_free(m, spec, first[s:s + 1], y[s:s + 1], hop, h[s:s + 1], n) for s in range(3)]
     ran = []
-    for mode in range(1, 7):
+    for mode in (1, 2, 3, 4, 6):
         for ns in (1, 3):
             m._runtime().gen_mode = mode
             try:
@@ -533,7 +533,7 @@ def test_ffma_block_fwd_cond_frames_kernel(shape, case):
 def _gen_all_modes(m, first, n, **cond):
     """{(mode, ns): (indices, logits)} over every sampler kernel that applies, for 1 and all streams"""
     out = {}
-    for mode in range(1, 7):
+    for mode in (1, 2, 3, 4, 6):
         for ns in (1, first.shape[0]):
             m._runtime().gen_mode = mode
             kw = {k: v[:ns] for k, v in cond.items()}

@@ -13,7 +13,7 @@ import torch
 import bench
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 4000
-modes = [int(a) for a in sys.argv[2:]] or [3, 5]
+modes = [int(a) for a in sys.argv[2:]] or [3, 2]
 model = bench.build_model(bench.GEN_KW).cuda()
 rt = model._runtime()
 ref = None
