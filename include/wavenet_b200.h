@@ -447,6 +447,23 @@ int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, float* d_rings
                   wn_gen_handle** out);
 /* zero the rings and the time counter (DilatedQueue.reset, wavenet_modules.py:74-77) */
 int wn_gen_reset(wn_gen_handle* h, void* stream);
+/* Prefill: start a run at t0 = t_end > 0 from rings written by a forward pass over the prompt instead of by evaluations
+ * [0, t_end).  Layer l's input at time t (what evaluation t enqueues in ring l) is read from d_src at frame
+ * frame_of_t_end - (t_end - t), stream s = sequence s of the buffer (B = n_streams, L frames), in either layout
+ *     WN_GEN_SRC_FRAMES  fp32 frames (B, L, R)                   (wn_start_fwd_index_*, wn_block_fwd*)
+ *     WN_GEN_SRC_PAIRS   chunked bf16 pairs (B, 2, R/8, L, 8)    (wn_tb_block_fwd*; the value is float(hi) + float(lo))
+ * for the times [max(0, t_end - ring_len_l), t_end) the ring holds; slots of times < 0 keep wn_gen_reset's zeros.  The
+ * rings are written in the layout of the kernel wn_gen_run would launch now (wn_gen_kernel_id): plain floats for kernel 1,
+ * {value, tag = t + 1} pairs otherwise.  wn_gen_prefill_layer works only right after wn_gen_reset (WN_E_STATE otherwise);
+ * wn_gen_prefill_commit(h, t_end) returns WN_E_STATE unless every layer was filled for that t_end, then moves the handle to
+ * t = t_end, so the next wn_gen_run starts at t0 = t_end (evaluation t_end must read a given sample: t_end < n_given).
+ * wn_gen_run returns WN_E_STATE after a prefill that was not committed, or when the kernel it would launch keeps another
+ * ring layout than the one the prefill wrote. */
+#define WN_GEN_SRC_FRAMES 0
+#define WN_GEN_SRC_PAIRS  1
+int wn_gen_prefill_layer(wn_gen_handle* h, int layer, const void* d_src, int layout, int L, int frame_of_t_end, int t_end,
+                         void* stream);
+int wn_gen_prefill_commit(wn_gen_handle* h, int t_end);
 /* Run evaluations [t0, t0+n_evals) of a schedule with n_given given samples per stream:
  *   evaluation e takes as input  d_first[s*n_given + e]            if e <  n_given
  *                                d_forced[s*n_samples + e-n_given] if d_forced != NULL   (teacher forcing)

@@ -2503,6 +2503,32 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     cluster_sync_all();                                  // peers may still be storing into this CTA's shared memory
 }
 
+// ------------------------------------------------------------------------------------------------ ring prefill
+// One layer's input at times [t_lo, t_end), computed by a forward pass, into the ring slots t % ring_len: frame
+// f_end - (t_end - t) of stream s in src, fp32 frames (B, L, R) or chunked bf16 pairs (B, 2, R/8, L, 8) (value hi + lo).
+// plain: kernel 1's ring of floats; otherwise the {value, tag = t + 1} pairs the flag-exchange kernels poll for.
+__global__ void gen_prefill_kernel(const void* __restrict__ src, int pairs, int L, int f_end, int t_lo, int t_end, int NS,
+                                   int R, int ring_len, float* __restrict__ rings, long long ring_off, int plain) {
+    const long long n = (long long)(t_end - t_lo) * NS * R;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int r = (int)(i % R);
+        const long long q = i / R;
+        const int s = (int)(q % NS), t = t_lo + (int)(q / NS);
+        const long long f = f_end - (t_end - t);
+        float v;
+        if (pairs) {
+            const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(src);
+            const size_t hi = ((((size_t)s * 2) * (R / 8) + r / 8) * L + f) * 8 + (r & 7);
+            v = __bfloat162float(b[hi]) + __bfloat162float(b[hi + (size_t)(R / 8) * L * 8]);
+        } else {
+            v = reinterpret_cast<const float*>(src)[((size_t)s * L + f) * R + r];
+        }
+        const size_t e = ((size_t)(t % ring_len) * NS + s) * R + r;
+        if (plain) rings[ring_off + e] = v;                          // ring_off counts elements of either kind
+        else reinterpret_cast<uint2*>(rings)[ring_off + e] = make_uint2(__float_as_uint(v), (unsigned)t + 1u);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 struct ScratchLayout {
     size_t bar, cur_idx, layers, zbuf, skipbuf, y1buf, logitbuf, err, zLL, skipLL, y1LL, logitLL, ll_end, trace, cl8_img, cl8_bytes, total;
@@ -2583,6 +2609,10 @@ struct wn_gen_handle {
     GenStream* d_sp;
     bool sp_dirty, sp_any_trunc, sp_any_temp;
     int sp_max_given, sp_head_from;
+    // wn_gen_prefill_*: the t_end each layer's ring was filled for (-1: not filled since wn_gen_reset), and the ring layout
+    // the fill wrote (-1: none; 1: plain floats of kernel 1, 0: {value, tag} pairs of every other kernel)
+    std::vector<int> pf_t_end;
+    int pf_plain;
 };
 
 static int validate_shape(const wn_gen_shape* s) {
@@ -2882,6 +2912,8 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     }
     h->tables_uploaded = false;
     h->cur_t = 0;
+    h->pf_t_end.assign(s->n_layers, -1);
+    h->pf_plain = -1;
     *out = h;
     return 0;
 }
@@ -2905,6 +2937,54 @@ extern "C" int wn_gen_reset(wn_gen_handle* h, void* stream) {
         h->cl8_packed = true;
     }
     h->cur_t = 0;
+    h->pf_t_end.assign(h->shape.n_layers, -1);
+    h->pf_plain = -1;
+    return 0;
+}
+
+// Nothing but the rings carries state into a launch at t0 > 0 when evaluation t0 reads a given sample: cur_idx is read only
+// when it does not, and every exchange tag is either in shared memory (kernels 4, 6: zeroed at launch; kernel 4's `seq`
+// starts from t0) or tagged t + 1 in the scratch wn_gen_reset zeroes (kernels 2, 3), and kernel 1's barrier counter is
+// cleared before every launch.  So rings written here continue exactly like rings written by evaluations [0, t_end).
+extern "C" int wn_gen_prefill_layer(wn_gen_handle* h, int layer, const void* d_src, int layout, int L, int frame_of_t_end,
+                                    int t_end, void* stream) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_prefill_layer: null handle");
+    WN_REQUIRE(h->tables_uploaded && h->cur_t == 0, WN_E_STATE,
+               "wn_gen_prefill_layer: prefill only right after wn_gen_reset (the handle is at t = %d)", h->cur_t);
+    WN_REQUIRE(layer >= 0 && layer < h->shape.n_layers && d_src && (layout == WN_GEN_SRC_FRAMES || layout == WN_GEN_SRC_PAIRS) &&
+                   t_end >= 1 && L >= 1 && frame_of_t_end <= L,
+               WN_E_BADARG, "wn_gen_prefill_layer: bad arguments (layer %d, layout %d, L %d, frame %d, t_end %d)", layer, layout,
+               L, frame_of_t_end, t_end);
+    const int R = h->shape.R, NS = h->shape.n_streams;
+    WN_REQUIRE(layout == WN_GEN_SRC_FRAMES || R % 8 == 0, WN_E_BADARG, "wn_gen_prefill_layer: chunked pairs need R %% 8 == 0");
+    const GenLayer& Lr = h->layers[layer];
+    const int n_t = std::min(t_end, Lr.ring_len);
+    WN_REQUIRE(frame_of_t_end - n_t >= 0, WN_E_BADARG,
+               "wn_gen_prefill_layer: layer %d needs frames [%d, %d), the buffer starts at 0", layer, frame_of_t_end - n_t,
+               frame_of_t_end);
+    const int kid = pick_kernel(h);
+    WN_REQUIRE(kid != 0, WN_E_UNSUPP, "wn_gen_prefill_layer: no sampler kernel fits this net in mode %d", h->mode);
+    const int plain = kid == 1;
+    WN_REQUIRE(h->pf_plain < 0 || h->pf_plain == plain, WN_E_STATE,
+               "wn_gen_prefill_layer: the sampler kernel changed between layers (ring layout differs)");
+    const long long n = (long long)n_t * NS * R;
+    const int grid = (int)std::min<long long>((n + 255) / 256, 4LL * h->sm_count);
+    gen_prefill_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(d_src, layout == WN_GEN_SRC_PAIRS, L, frame_of_t_end, t_end - n_t,
+                                                               t_end, NS, R, Lr.ring_len, h->base.rings, Lr.ring_off, plain);
+    WN_CUDA(cudaGetLastError());
+    h->pf_plain = plain;
+    h->pf_t_end[layer] = t_end;
+    return 0;
+}
+
+extern "C" int wn_gen_prefill_commit(wn_gen_handle* h, int t_end) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_prefill_commit: null handle");
+    WN_REQUIRE(h->cur_t == 0, WN_E_STATE, "wn_gen_prefill_commit: the handle is at t = %d, not right after wn_gen_reset",
+               h->cur_t);
+    for (int l = 0; l < h->shape.n_layers; ++l)
+        WN_REQUIRE(h->pf_t_end[l] == t_end, WN_E_STATE, "wn_gen_prefill_commit: layer %d was filled for t_end %d, not %d", l,
+                   h->pf_t_end[l], t_end);
+    h->cur_t = t_end;
     return 0;
 }
 
@@ -3133,6 +3213,16 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
     WN_REQUIRE(kid != 0, WN_E_UNSUPP,
                "wn_gen_run: %d streams need a cluster kernel (modes 4, 6) for this net; mode %d does not fit in shared memory",
                h->shape.n_streams, h->mode);
+    if (h->pf_plain >= 0) {
+        WN_REQUIRE(h->cur_t > 0, WN_E_STATE, "wn_gen_run: rings were prefilled but not committed (wn_gen_prefill_commit)");
+        WN_REQUIRE(h->pf_plain == (kid == 1), WN_E_STATE,
+                   "wn_gen_run: the rings were prefilled for kernel %s, kernel %d keeps another ring layout",
+                   h->pf_plain ? "1" : "2, 3, 4 or 6", kid);
+        // the first evaluation after the prefill must read a given sample: no evaluation chose the one before it
+        WN_REQUIRE(a->t0 != h->pf_t_end[0] || a->t0 <= head_from, WN_E_BADARG,
+                   "wn_gen_run: evaluation %d after a prefill must read a prompt sample (prompts of %d samples)", a->t0,
+                   head_from + 1);
+    }
     cudaStream_t st = (cudaStream_t)stream;
     if (per_stream && h->shape.n_streams > 1 && h->sp_dirty) {
         // in stream order, so that a launch still reading the previous records finishes first

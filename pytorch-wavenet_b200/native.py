@@ -57,6 +57,7 @@ class TcBlockArgs(C.Structure):
 
 
 PREC_BF16, PREC_BF16_PAIRS = 1, 2        # WN_PREC_* of include/wavenet_b200.h
+GEN_SRC_FRAMES, GEN_SRC_PAIRS = 0, 1     # WN_GEN_SRC_* (wn_gen_prefill_layer)
 
 
 class TbBlockArgs(C.Structure):
@@ -207,6 +208,8 @@ SIGNATURES = {
     "wn_gen_create": (C.c_int, [C.POINTER(GenShape), C.POINTER(GenWeights), C.c_void_p, C.c_void_p,
                                 C.POINTER(C.c_void_p)]),
     "wn_gen_reset": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "wn_gen_prefill_layer": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p]),
+    "wn_gen_prefill_commit": (C.c_int, [C.c_void_p, C.c_int]),
     "wn_gen_run": (C.c_int, [C.c_void_p, C.POINTER(GenRunArgs), C.c_void_p]),
     "wn_gen_destroy": (C.c_int, [C.c_void_p]),
     "wn_gen_set_mode": (C.c_int, [C.c_void_p, C.c_int]),

@@ -52,6 +52,23 @@ class StackPlan:
         self.skip_start = L - T
 
 
+def prefill_window(T, dilations, kernel_size, hop=1):
+    """(P0, S, W) of the sampler's ring prefill to T evaluations (_Runtime.prefill): one forward over prompt positions
+    [P0, T), W = T - P0 of them, placed at buffer frames [S, S + W) with every layer's history before frame S zero.
+
+    Ring l holds x_l[t] for t in [T - ring_len_l, T), ring_len_l = (k-1) d_l + 1, and x_l[t] depends on positions
+    [t - rf_l + 1, t] (rf_0 = 1, rf_{l+1} = rf_l + (k-1) d_l), so the ring needs positions >= T - rf_{l+1} >= T - rf.
+    From P0 = max(0, T - rf) the window's zero history reaches no needed value (P0 > 0), or is the reset queues' own zero
+    history (P0 = 0): the forward costs at most one receptive field per stream, however long the prompt.  With local
+    conditioning at `hop`, P0 is rounded down and S up to multiples of hop so that window frame f reads condition frame
+    (P0 - S) / hop + f // hop.  S >= the largest (k-1) d keeps every tap inside the buffer."""
+    rf = 1 + (kernel_size - 1) * sum(dilations)
+    P0 = max(0, T - rf) // hop * hop
+    unit = math.lcm(8, hop)
+    S = max(-(-(kernel_size - 1) * max(dilations) // unit) * unit, unit)
+    return P0, S, T - P0
+
+
 class _Packs:
     """Lazily built packed weight groups of one model state (see _Runtime.packed_weights):
       layers              K-outer fp32 copies for the SIMT block kernels
@@ -205,26 +222,34 @@ class _Packs:
                      "local condition table")
         return out
 
-    def _build_tb(self, stream):
+    def _build_tb(self, stream, prec=None):
         rt, lib = self.rt, native.lib()
         R, nl = self._dims()[0], self._dims()[6]
-        prec, dev = rt.tb_precision(), rt.device()
+        prec, dev = prec or rt.tb_precision(), rt.device()
         tb_w = torch.empty(nl, lib.wn_tb_weight_bytes_per_layer(R, prec), device=dev, dtype=torch.uint8)
         tb_b = torch.empty(nl, 4 * R, device=dev, dtype=torch.float32)
         native.check(lib.wn_tb_pack_all_weights(self._ptr_table().data_ptr(), nl, R, prec, tb_w.data_ptr(), tb_b.data_ptr(),
                                                 stream), "pack tb")
         return tb_w, tb_b, prec
 
-    def _build_tb_local(self, stream):
+    def _build_tb_local(self, stream, prec=None):
         """Every layer's [Uf; Ug] for the K-slabs of the audio-rate local conditioning (wn_tb_pack_local_weights)."""
         rt, lib, m = self.rt, native.lib(), self.rt.model
         R, nl, C = m.residual_channels, m.layers * m.blocks, m.local_condition_channels
-        prec, dev = rt.tb_precision(), rt.device()
+        prec, dev = prec or rt.tb_precision(), rt.device()
         u = torch.empty(nl, lib.wn_tb_local_weight_bytes_per_layer(C, R, prec), device=dev, dtype=torch.uint8)
         ptrs = torch.tensor([[m.filter_local_convs[i].weight.data_ptr(), m.gate_local_convs[i].weight.data_ptr()]
                              for i in range(nl)], dtype=torch.int64, device=dev)
         native.check(lib.wn_tb_pack_local_weights(ptrs.data_ptr(), nl, C, R, prec, u.data_ptr(), stream), "pack tb local")
         return u, ptrs, prec
+
+    def _build_tb_pairs(self, stream):
+        """"tb" packed for bf16 pairs whatever tc_precision says (the sampler's ring prefill, _Runtime.prefill)."""
+        return self["tb"] if self.rt.tb_precision() == native.PREC_BF16_PAIRS else self._build_tb(stream, native.PREC_BF16_PAIRS)
+
+    def _build_tb_local_pairs(self, stream):
+        return self["tb_local"] if self.rt.tb_precision() == native.PREC_BF16_PAIRS else \
+            self._build_tb_local(stream, native.PREC_BF16_PAIRS)
 
     def _build_tb_bwd(self, stream):
         rt, lib = self.rt, native.lib()
@@ -1048,16 +1073,111 @@ class _Runtime:
         self.samplers[n_streams] = s
         return s
 
+    def reset_sampler(self, s, stream):
+        lib = native.lib()
+        native.check(lib.wn_gen_reset(s["handle"], stream), "gen reset")
+        mode = getattr(self, "gen_mode", None)            # None: library default (wn_gen_set_mode 0: the tensor-core cluster kernel for 256-wide nets)
+        if mode is not None:
+            native.check(lib.wn_gen_set_mode(s["handle"], int(mode)), "gen mode")
+
+    def prefill(self, s, d_first, T, cond=None, ctab=None, local=None):
+        """Write the rings of the freshly reset sampler ``s`` as evaluations [0, T) would, from one forward over the prompt
+        window of prefill_window, and move the handle to t = T (wn_gen_prefill_*).  d_first: the (NS, >= T + 1) int32
+        prompts on the device; cond: the (NS, G) condition rows, ctab their table (s["cond"]); local: the sampler's
+        (series, hop).  256-channel nets run the fused tensor-core blocks in bf16 pairs whatever tc_precision says (fp32-class,
+        the sampler's parity class); every other net, 512 channels included (single-pass bf16 there, ~1e-3), the FFMA
+        blocks.  One launch per layer, each followed by the scatter of its output into the next layer's ring; layer 0's
+        ring comes from the fp32 start conv, which is the sampler's own gather w[:, c] + b."""
+        m, lib = self.model, native.lib()
+        dev = self.device()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        h = s["handle"]
+        R, D, Sk, Cc, k = m.residual_channels, m.dilation_channels, m.skip_channels, m.classes, m.kernel_size
+        dil = [d for d, _ in m.dilations]
+        NS, nl = d_first.shape[0], len(dil)
+        upsampled = local is not None and getattr(m, "local_upsample", None) is not None
+        P0, S, W = prefill_window(T, dil, k, 1 if local is None else local[1])
+        L = S + W
+        Wp = self.packed_weights(stream)
+        use_tb = R == 256 and bool(lib.wn_tb_supported(R, D, Sk, k))
+        f32 = dict(device=dev, dtype=torch.float32)
+        idx = torch.zeros(NS, L, device=dev, dtype=torch.int64)
+        idx[:, S:] = d_first[:, P0:T]
+        buf = torch.empty(2, NS, L, R, **f32)               # the two activation buffers (fp32 frames or bf16 pairs)
+        ws_t, bs_p = Wp["start"]
+        native.check(lib.wn_start_fwd_index_i64(idx.data_ptr(), ws_t.data_ptr(), bs_p.data_ptr(), buf[0].data_ptr(),
+                                                NS, Cc, L, R, stream), "prefill start")
+        native.check(lib.wn_gen_prefill_layer(h, 0, buf[0].data_ptr(), native.GEN_SRC_FRAMES, L, L, T, stream), "prefill layer 0")
+        frames = None                                       # (table, n_frames, hop) of repeat-upsampled local conditioning
+        if local is not None and not (upsampled and use_tb):
+            y, hop = local
+            nfw = -(-W // hop)
+            y_win = torch.zeros(NS, y.shape[1], S // hop + nfw, **f32)      # zero frames before S: never read
+            y_win[:, :, S // hop:] = y[:, :, P0 // hop:P0 // hop + nfw]
+            frames = (Wp.cond_table_frames(cond, y_win, 0, y_win.shape[2], stream), y_win.shape[2], hop)
+        elif upsampled:
+            c, Cl = local[0], m.local_condition_channels
+            c_win = torch.zeros(NS, Cl, L, **f32)
+            c_win[:, :, S:] = c[:, :, P0:T]
+            cpad = lib.wn_tb_local_padded_channels(Cl, native.PREC_BF16_PAIRS)
+            c_pair = torch.empty(NS, 2, cpad // 8, L, 8, device=dev, dtype=torch.bfloat16)
+            native.check(lib.wn_tb_local_from_channels(c_win.data_ptr(), c_pair.data_ptr(), NS, Cl, L, native.PREC_BF16_PAIRS,
+                                                       stream), "prefill local features")
+            u_all = Wp["tb_local_pairs"][0]
+            ctab = None if cond is None else Wp.cond_table(cond, stream)
+        if use_tb:
+            tb_w, tb_b, _ = Wp["tb_pairs"]
+            pairs = [buf[i].view(torch.bfloat16) for i in range(2)]
+            native.check(lib.wn_pair_from_frames(buf[0].data_ptr(), pairs[1].data_ptr(), NS, L, R, 0, stream), "prefill pairs")
+            skip = torch.empty(NS, Sk // 4, 1, 4, **f32)
+            a = native.TbBlockArgs()
+            a.B, a.L, a.n_layers, a.channels, a.precision = NS, L, nl, R, native.PREC_BF16_PAIRS
+            a.d_w_all, a.d_fg_save = tb_w.data_ptr(), None
+            src = 1
+        else:
+            skip = torch.empty(NS, 1, Sk, **f32)
+            a = native.BlockArgs()
+            a.R, a.D, a.S, a.k, a.mode = R, D, Sk, k, 0
+            a.B, a.L = NS, L
+            src = 0
+        a.d_skip, a.in_start, a.out_start, a.skip_start, a.skip_init = skip.data_ptr(), S, S, L - 1, 1
+        for i in range(nl - 1):                             # the last layer's output feeds no ring
+            a.d_h_in, a.d_h_out, a.dilation = buf[src].data_ptr(), buf[1 - src].data_ptr(), dil[i]
+            if use_tb:
+                a.layer, a.d_bias4 = i, tb_b[i].data_ptr()
+                if upsampled:
+                    rc = lib.wn_tb_block_fwd_local(ctypes.byref(a), native.ptr(None if ctab is None else ctab[i]),
+                                                   c_pair.data_ptr(), Cl, u_all.data_ptr(), stream)
+                elif frames is not None:
+                    rc = lib.wn_tb_block_fwd_cond_frames(ctypes.byref(a), frames[0][i].data_ptr(), frames[1], frames[2], stream)
+                elif ctab is not None:
+                    rc = lib.wn_tb_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream)
+                else:
+                    rc = lib.wn_tb_block_fwd(ctypes.byref(a), stream)
+            else:
+                wfg, bfg, wrs, brs = Wp["layers"][i]
+                a.d_wfg_t, a.d_bfg, a.d_wrs_t, a.d_brs = wfg.data_ptr(), bfg.data_ptr(), wrs.data_ptr(), brs.data_ptr()
+                if frames is not None:
+                    rc = lib.wn_block_fwd_cond_frames(ctypes.byref(a), frames[0][i].data_ptr(), frames[1], frames[2], stream)
+                elif ctab is not None:
+                    rc = lib.wn_block_fwd_cond(ctypes.byref(a), ctab[i].data_ptr(), stream)
+                else:
+                    rc = lib.wn_block_fwd(ctypes.byref(a), stream)
+            native.check(rc, f"prefill block {i}")
+            src = 1 - src
+            native.check(lib.wn_gen_prefill_layer(h, i + 1, buf[src].data_ptr(),
+                                                  native.GEN_SRC_PAIRS if use_tb else native.GEN_SRC_FRAMES, L, L, T, stream),
+                         f"prefill layer {i + 1}")
+        native.check(lib.wn_gen_prefill_commit(h, T), "prefill commit")
+        self.last_prefill = dict(P0=P0, S=S, W=W, blocks="tb" if use_tb else "ffma")
+
     def generate_resident(self, s, d_first, n_given, num_samples, temperature, regularize, d_out, d_uni=None,
                           d_forced=None, d_logits=None, t0=0, n_evals=None, reset=True):
         """Launch the sampler on buffers that already live on the device (no host<->device traffic, no sync)."""
         lib = native.lib()
         stream = torch.cuda.current_stream(self.device()).cuda_stream
         if reset:
-            native.check(lib.wn_gen_reset(s["handle"], stream), "gen reset")
-            mode = getattr(self, "gen_mode", None)            # None: library default (wn_gen_set_mode 0: the tensor-core cluster kernel for 256-wide nets)
-            if mode is not None:
-                native.check(lib.wn_gen_set_mode(s["handle"], int(mode)), "gen mode")
+            self.reset_sampler(s, stream)
         args = native.GenRunArgs()
         args.d_first, args.n_given = d_first.data_ptr(), n_given
         args.d_forced, args.d_uniforms = native.ptr(d_forced), native.ptr(d_uni)
@@ -1071,7 +1191,7 @@ class _Runtime:
         return t0 + args.n_evals
 
     def generate(self, num_samples, first, temperature, regularize, uniforms=None, forced=None,
-                 want_logits=False, callbacks=None, cond=None, local=None, top_k=0, top_p=1.0):
+                 want_logits=False, callbacks=None, cond=None, local=None, top_k=0, top_p=1.0, prefill=False):
         """first: (NS, n_given) int array.  Returns (indices (NS, num_samples) int64 ndarray, logits or None, t_end).
         top_k, top_p: the truncation of the temperature draw (wn_gen_set_truncation), set on the handle by every call.
         Per-stream form (see _stream_plan): first a list of NS 1-D prompts of any lengths, num_samples and the four settings
@@ -1081,7 +1201,9 @@ class _Runtime:
         callbacks: optional list of (eval_index, fn) -- fn() is called once evaluations <= eval_index are done.
         cond: the (NS, G) fp32 condition rows of a conditioned model, else None.
         local: (y, hop) of a locally conditioned model, y the (NS, C, F) fp32 series, else None.  The condition table is
-        built window by window (at most ``local_table_bytes`` each), and launches are split at the window boundaries."""
+        built window by window (at most ``local_table_bytes`` each), and launches are split at the window boundaries.
+        prefill: write the rings for the first head_from evaluations (the common prompt prefix) with one forward (prefill())
+        instead of evaluating them one by one; callbacks of those evaluations fire, in order, right after it."""
         plan = _stream_plan(first, num_samples, temperature, regularize, top_k, top_p)
         m = self.model
         dev = self.device()
@@ -1159,6 +1281,10 @@ class _Runtime:
             return t
 
         t, first_launch = 0, True
+        if prefill and plan.head_from > 0:
+            self.reset_sampler(s, stream)
+            self.prefill(s, d_first, plan.head_from, cond=cond, ctab=s.get("cond") if local is None else None, local=local)
+            t, first_launch = plan.head_from, False
         for upto, fn in sorted(callbacks or [], key=lambda c: c[0]):
             n = min(upto + 1, total_evals) - t
             if n > 0 or first_launch:
@@ -1306,6 +1432,11 @@ def _truncation(top_k, top_p):
     if not 0.0 < float(top_p) <= 1.0:
         raise ValueError(f"top_p must lie in (0, 1] (1: off), got {top_p}")
     return int(top_k), float(top_p)
+
+
+def _check_prefill(prefill):
+    if not isinstance(prefill, bool):
+        raise ValueError(f"prefill must be True or False, got {prefill!r}")
 
 
 def _exact_convolutions():
@@ -1713,7 +1844,7 @@ class WaveNetModel(nn.Module):
 
     def generate_fast(self, num_samples, first_samples=None, temperature=1., regularize=0.,
                       progress_callback=None, progress_interval=100, condition=None, local_condition=None,
-                      top_k=0, top_p=1.0):
+                      top_k=0, top_p=1.0, prefill=False):
         """Fast-WaveNet sampling; returns the mu-law expanded waveform, float64 ndarray of ``num_samples`` values.
 
         Same schedule as the reference (wavenet_model.py:237-315): the queues are reset, the given samples warm
@@ -1728,14 +1859,19 @@ class WaveNetModel(nn.Module):
         ``local_condition``: a locally conditioned model's (C, F) series for this stream; evaluation e (which reads sample
         e, the given samples first, and predicts sample e + 1) takes frame e // hop, so F >= ceil((n_given - 1 +
         num_samples) / hop).
+        ``prefill=True``: the queues are filled from the prompt by one parallel forward over its last receptive field
+        instead of one sequential evaluation per prompt sample (much faster for long prompts).  The history then comes
+        from other (fp32-class) arithmetic, so a draw within rounding of a CDF edge, or an argmax near-tie, may go the
+        other way; the default False keeps the sequential warm-up.  ValueError unless a bool.
         """
         top_k, top_p = _truncation(top_k, top_p)
+        _check_prefill(prefill)
         if self.start_conv.weight.device.type != "cuda":
             twin = self._cuda_shadow()
             audio = twin.generate_fast(num_samples, first_samples=first_samples, temperature=temperature,
                                        regularize=regularize, progress_callback=progress_callback,
                                        progress_interval=progress_interval, condition=condition,
-                                       local_condition=local_condition, top_k=top_k, top_p=top_p)
+                                       local_condition=local_condition, top_k=top_k, top_p=top_p, prefill=prefill)
             for q, tq in zip(self.dilated_queues, twin.dilated_queues):
                 q.data, q.in_pos, q.out_pos = tq.data, tq.in_pos, tq.out_pos
             self.train()
@@ -1760,14 +1896,15 @@ class WaveNetModel(nn.Module):
         rt = self._runtime()
         with torch.cuda.device(rt.device()):
             idx, _, _ = rt.generate(num_samples, first[None, :], temperature, regularize, callbacks=callbacks, cond=cond,
-                                    local=local, top_k=top_k, top_p=top_p)
+                                    local=local, top_k=top_k, top_p=top_p, prefill=prefill)
         self._export_queues()
         self.train()
         generated = (idx[0] / self.classes) * 2. - 1
         return mu_law_expansion(generated, self.classes)
 
     def generate_fast_batch(self, num_samples, first_samples, temperature=1., regularize=0., uniforms=None,
-                            forced=None, return_logits=False, condition=None, local_condition=None, top_k=0, top_p=1.0):
+                            forced=None, return_logits=False, condition=None, local_condition=None, top_k=0, top_p=1.0,
+                            prefill=False):
         """``n_streams`` independent generate_fast runs batched in one kernel (the reference has a single stream,
         wavenet_model.py:179).  first_samples: (n_streams, n_given) ints.  Returns int64 indices
         (n_streams, num_samples) [and the per-step logits].  Run through the same sampler kernel, stream s equals a
@@ -1786,7 +1923,9 @@ class WaveNetModel(nn.Module):
         generate_fast calls in order.  With a sequence of counts or prompts of different lengths the return is a list of
         per-stream index arrays (n_s,) [and a list of (n_s, classes) logits]; otherwise it is the arrays above.  Streams
         that finish early keep running until the longest job is done.  ValueError for a malformed argument, before any
-        device work."""
+        device work.  prefill: as for generate_fast, over the prompts' common length (a longer prompt's remainder is
+        still evaluated sample by sample)."""
+        _check_prefill(prefill)
         plan = _stream_plan(first_samples, num_samples, temperature, regularize, top_k, top_p)
         NS = plan.n_streams
         cond = self._condition(condition, NS)
@@ -1806,7 +1945,7 @@ class WaveNetModel(nn.Module):
         with torch.cuda.device(rt.device()):
             idx, logits, _ = rt.generate(counts, first, temperature, regularize, uniforms=uniforms,
                                          forced=forced, want_logits=return_logits, cond=cond, local=local,
-                                         top_k=top_k, top_p=top_p)
+                                         top_k=top_k, top_p=top_p, prefill=prefill)
         self._export_queues()
         self.train()
         if plan.ragged:
