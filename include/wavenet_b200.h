@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 2
+#define WN_ABI_VERSION 3
 
 /* operand precision of the tensor-core training kernels (wn_tb_*): what the MATRIX PRODUCTS see; the residual stream and
  * skip stay fp32-class and accumulation is fp32 in both */
@@ -98,33 +98,25 @@ typedef struct wn_block_args {
 int wn_block_fwd(const wn_block_args* a, void* stream);
 
 /* ---------------------------------------------------------------- (T) the same block on the tensor cores
- * wgmma tf32 with 3xTF32 operand splitting (hi*hi + lo*hi + hi*lo, fp32 accumulation in registers):
- * fp32-class accuracy (~1e-6 relative) at tensor-core rate.  Two launches per block (conv+gate -> z, then the 1x1s);
- * d_z is a caller-provided (B,L,D) workspace.  Shapes: R % 256 == 0, S % 256 == 0, D % 128 == 0 (wn_tc_supported).
- * Weights are packed K-major and pre-split: d_wa [2][2D][k*R] (rows in 256-wide tiles: 128 filter channels then the
- * same 128 gate channels; column j*R+r = tap j of input channel r; [0]=hi, [1]=lo), d_ba [2D] in the same row order,
- * d_wb [2][R+S][D] (residual rows then skip rows), d_bb [R+S]. */
+ * wgmma bf16 with bf16 (hi, lo) operand pairs (hi = bf16(x), lo = bf16(x - hi); hi*hi + lo*hi + hi*lo, fp32 accumulation
+ * in registers): fp32-class accuracy (~3e-6 relative on the logits after 50 layers) at tensor-core rate.  Two launches
+ * per block (conv+gate -> z, then the 1x1s); d_z is a caller-provided (B,L,D) workspace.  Shapes: R % 256 == 0,
+ * S % 256 == 0, D % 128 == 0 (wn_tc_supported).
+ * Weights are packed K-major as bf16 pair arrays [2][rows][K] ([0] = hi, [1] = lo): d_wa [2][2D][k*R] (rows in 256-wide
+ * tiles: 128 filter channels then the same 128 gate channels; column j*R+r = tap j of input channel r), d_ba [2D] fp32 in
+ * the same row order, d_wb [2][R+S][D] (residual rows then skip rows), d_bb [R+S] fp32. */
 int wn_tc_supported(int R, int D, int S, int k);
 int wn_tc_pack_block_weights(const float* d_wf, const float* d_wg, const float* d_bf, const float* d_bg,
                              const float* d_wr, const float* d_ws, const float* d_br, const float* d_bs,
-                             int R, int D, int S, int k, float* d_wa, float* d_ba, float* d_wb, float* d_bb, void* stream);
+                             int R, int D, int S, int k, void* d_wa, float* d_ba, void* d_wb, float* d_bb, void* stream);
 typedef struct wn_tc_block_args {
     const float* d_h_in; float* d_h_out; float* d_skip; float* d_z;
-    const float* d_wa; const float* d_ba; const float* d_wb; const float* d_bb;
+    const void* d_wa; const float* d_ba; const void* d_wb; const float* d_bb;
     int B, L, R, D, S, k, dilation;
     int in_start, out_start, skip_start, skip_init;
     float* d_fg_save;
-    int fast_tf32;      /* precision mode.  0 = 3xTF32 (hi/lo tf32 split of both operands, ~6e-7 on the logits after 50
-                         * layers).  2 = bf16 pairs (hi/lo bf16 split, the same three products at twice the MMA rate,
-                         * ~3e-6 on the logits after 50 layers; d_wa / d_wb must then be the arrays made by
-                         * wn_tc_convert_weights_bf16).  1 = single TF32 pass: ~1e-3 on the logits -- OUTSIDE the 1e-4
-                         * parity bar; opt-in, reported separately by bench.py */
 } wn_tc_block_args;
 int wn_tc_block_fwd(const wn_tc_block_args* a, void* stream);
-/* Re-split a packed fp32 pair array [2][n_per_half] (hi | lo, as written by wn_tc_pack_block_weights /
- * wn_tc_pack_block_bwd_weights) into bf16 pairs [2][n_per_half] for precision mode 2: x = hi + lo exactly,
- * out_hi = bf16(x), out_lo = bf16(x - out_hi).  d_out: 4 * n_per_half bytes. */
-int wn_tc_convert_weights_bf16(const float* d_pairs, void* d_out, long long n_per_half, void* stream);
 /* Debug aid (WN_TC_TRACE=1): per-stage clock64 stamps of CTA 0 of the most recent tensor-core launch, 8 per stage:
  * producer before/after the empty wait, MMA warp before/after the operand wait and after issue, splitter start/end
  * (first splitter warp), end of the last splitter warp. */
@@ -341,16 +333,14 @@ typedef struct wn_block_bwd_args {
 } wn_block_bwd_args;
 int wn_block_bwd_data(const wn_block_bwd_args* a, void* stream);
 
-/* The same two data-gradient GEMMs on the tensor cores (wgmma, 3xTF32), for R % 256 == 0, S % 256 == 0, D % 256 == 0:
- * weights packed K-major and pre-split by wn_tc_pack_block_bwd_weights into d_wdz [2][D][R+S] (row c: residual_conv
- * column c then skip_conv column c) and d_wdh [2][R][k*2D] (row r, column j*2D+n: [filter;gate].weight[n][r][j]).
- * d_wrs_rows / d_wfg_bwd of the args are ignored. */
+/* The same two data-gradient GEMMs on the tensor cores (wgmma, bf16 (hi, lo) operand pairs as in wn_tc_block_fwd), for
+ * R % 256 == 0, S % 256 == 0, D % 256 == 0: weights packed K-major by wn_tc_pack_block_bwd_weights into the bf16 pair arrays
+ * d_wdz [2][D][R+S] (row c: residual_conv column c then skip_conv column c) and d_wdh [2][R][k*2D] (row r, column j*2D+n:
+ * [filter;gate].weight[n][r][j]).  d_wrs_rows / d_wfg_bwd of the args are ignored. */
 int wn_tc_bwd_supported(int R, int D, int S, int k);
 int wn_tc_pack_block_bwd_weights(const float* d_wf, const float* d_wg, const float* d_wr, const float* d_ws,
-                                 int R, int D, int S, int k, float* d_wdz, float* d_wdh, void* stream);
-int wn_tc_block_bwd_data(const wn_block_bwd_args* a, const float* d_wdz, const float* d_wdh, void* stream);
-/* the same with a precision mode: 0 = 3xTF32 (fp32 pair arrays), 2 = bf16 pairs (arrays from wn_tc_convert_weights_bf16) */
-int wn_tc_block_bwd_data_prec(const wn_block_bwd_args* a, const void* d_wdz, const void* d_wdh, int precision, void* stream);
+                                 int R, int D, int S, int k, void* d_wdz, void* d_wdh, void* stream);
+int wn_tc_block_bwd_data(const wn_block_bwd_args* a, const void* d_wdz, const void* d_wdh, void* stream);
 
 /* head: given d_dlogits (B*out_len, classes) and the saved skip sum (B, L-skip_start, S) produce
  * d_y1 (B*out_len, E) = relu(W1 relu(skip)+b1) (recomputed), d_dy1 (B*out_len, E) and d_dskip (B, out_len, S).

@@ -1,5 +1,6 @@
-// tc_gemm.cu -- tensor-core (wgmma / TMA) form of the training block: exact-fp32-class numerics through
-// 3xTF32 (hi/lo split of both operands, fp32 accumulation in registers).
+// tc_gemm.cu -- tensor-core (wgmma / TMA) form of the training block: fp32-class numerics through bf16 (hi, lo) operand
+// pairs (hi = bf16(x), lo = bf16(x - hi); hi*hi + lo*hi + hi*lo per k-step, fp32 accumulation in registers): 16 mantissa
+// bits per operand, ~3e-6 on the logits after 50 layers (inside the 1e-4 bar).
 //
 // Same mathematics and frames layout as train_fwd.cu (reference wavenet_model.py:142-165), split in two launches
 // per block because the gated activation cannot stay on chip in split form (128 frames x 256 ch x {hi,lo} = 256 KB):
@@ -8,10 +9,10 @@
 //            epilogue: z = tanh(F+bf) * sigmoid(G+bg)  -> z (B,L,D)  [+ optional f,g for the backward]
 //   pass B   [O|S][128 x 256] per tile = z[128 x D] * Wb^T ;  h_out = O + br + h_in,  skip (+)= S + bs
 // Kernel anatomy (one CTA per SM, persistent over (sequence, 128-frame tile) items, 288 threads):
-//   warp 8        TMA producer: per K slab (16 fp32 = one 64-byte swizzle row) loads A raw, W_hi, W_lo (4-stage ring)
+//   warp 8        TMA producer: per K slab (16 fp32 = one 64-byte swizzle row) loads A raw, W_hi, W_lo (6-stage ring)
 //   warps 0-7     two consumer warpgroups, each owning 64 of the 128 frames: split the warpgroup's rows of the landed A
-//                 slab into hi = rna_tf32(x) (in place) and lo = x - hi, issue wgmma m64n128k8 tf32 (hi*hi + lo*hi + hi*lo
-//                 per k-step) into two 128-column register accumulators, then apply gate / residual / skip from the fragments
+//                 slab into bf16 hi / lo tiles, issue wgmma m64n128k16 bf16 (hi*hi + lo*hi + hi*lo) into two 128-column
+//                 register accumulators, then apply gate / residual / skip from the fragments
 // mbarriers: full (TMA landed), empty (every consumer thread is done with the stage).
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -26,23 +27,18 @@ using namespace px;
 
 constexpr int BM = 128;            // frames per tile (UMMA M)
 constexpr int BN = 256;            // output columns per tile (UMMA N)
-constexpr int BK = 16;             // fp32 per K slab = 64 bytes = one 64B-swizzle row (two k-steps of 8)
-constexpr int STAGES = 4;
+constexpr int BK = 16;             // fp32 per K slab = 64 bytes = one 64B-swizzle row (one bf16 k-step)
+// the operand tiles are bf16 (hi, lo) pairs with 32-byte rows; the raw fp32 A slab keeps its own buffer, so a stage is
+// A_raw 8K | A_hi 4K | A_lo 4K | W_hi 8K | W_lo 8K = 32 KB and six stages fit
+constexpr int STAGES = 6;
 constexpr int A_BYTES = BM * BK * 4;          // 8 KB
-constexpr int W_BYTES = BN * BK * 4;          // 16 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;      // A_hi | A_lo | W_hi | W_lo = 48 KB
-// bf16x2 precision (PREC_BF16X2): the operand tiles are bf16 (hi, lo) pairs with 32-byte rows; the raw fp32 A slab keeps
-// its own buffer, so a stage is A_raw 8K | A_hi 4K | A_lo 4K | W_hi 8K | W_lo 8K = 32 KB and six stages fit
-constexpr int STAGES_BF = 6;
 constexpr int ABF_BYTES = BM * BK * 2;        // 4 KB
 constexpr int WBF_BYTES = BN * BK * 2;        // 8 KB
-constexpr int STAGE_BYTES_BF = A_BYTES + 2 * ABF_BYTES + 2 * WBF_BYTES;     // 32 KB
-enum { PREC_TF32X3 = 0, PREC_TF32X1 = 1, PREC_BF16X2 = 2 };
+constexpr int STAGE_BYTES = A_BYTES + 2 * ABF_BYTES + 2 * WBF_BYTES;     // 32 KB
 constexpr int NTHREADS = 288;             // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int CONSUMERS = 256;
 
-// swizzled K-major descriptors (layout 2 = 64B, 3 = 32B swizzle): sbo = bytes between 8-row atoms
-__device__ __forceinline__ unsigned long long desc64(unsigned saddr) { return wg_desc(saddr, 16, 8 * 64, 2); }
+// swizzled K-major descriptor (layout 3 = 32B swizzle): sbo = bytes between 8-row atoms
 __device__ __forceinline__ unsigned long long desc32(unsigned saddr) { return wg_desc(saddr, 16, 8 * 32, 3); }
 
 // ---------------------------------------------------------------------------------------------- kernel
@@ -69,19 +65,11 @@ struct TcParams {
 
 __device__ __forceinline__ float sigmoid_tc(float x) { return 1.f / (1.f + expf(-x)); }
 
-// PREC_TF32X3: 3xTF32 (hi*hi + lo*hi + hi*lo, hi = rna_tf32(x)): ~6e-7 on the logits after 50 layers.
-// PREC_BF16X2: both operands as bf16 pairs (hi = bf16(x), lo = bf16(x - hi)), the same three products on bf16 MMAs at
-//              twice the tf32 rate: 16 mantissa bits per operand, ~3e-6 on the logits after 50 layers (inside the 1e-4 bar).
-// PREC_TF32X1: one TF32 MMA per k-step on the raw fp32 operands (the tensor core drops the low mantissa bits):
-//              ~1e-3 relative on the logits after 50 layers, i.e. outside the parity bar; opt-in, reported separately.
-template <int EPI, int PREC>
+template <int EPI>
 __global__ void __launch_bounds__(NTHREADS, 1)
 frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
                const __grid_constant__ CUtensorMap mapW, const TcParams p) {
-    constexpr bool EXACT = PREC == PREC_TF32X3;
-    constexpr bool BF = PREC == PREC_BF16X2;
-    constexpr int ST = BF ? STAGES_BF : STAGES;                // ring depth
-    constexpr int SB = BF ? STAGE_BYTES_BF : STAGE_BYTES;      // bytes per stage
+    constexpr int ST = STAGES, SB = STAGE_BYTES;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* stage_mem = base;                                           // ST * SB
@@ -120,19 +108,18 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         mbar_wait(empty + st, ph ^ 1);
                         if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it * 8 + 1] = clock64();
                         unsigned char* sm = stage_mem + st * SB;
-                        mbar_expect_tx(full + st, BF ? A_BYTES + 2 * WBF_BYTES : A_BYTES + (EXACT ? 2 : 1) * W_BYTES);
+                        mbar_expect_tx(full + st, A_BYTES + 2 * WBF_BYTES);
                         if (sl < slabs1) {
                             const int j = sl / slabs_per_tap, c0 = (sl % slabs_per_tap) * BK;
                             tma_load_3d(sm, &mapA, c0, t0 - (p.taps - 1 - j) * p.dil - p.a_origin, b, full + st);
                         } else {
                             tma_load_3d(sm, &mapA2, (sl - slabs1) * BK, t0 - p.a2_origin, b, full + st);
                         }
-                        constexpr int WT = BF ? WBF_BYTES : W_BYTES;        // bytes of one weight tile (hi or lo)
-                        constexpr int W0 = BF ? A_BYTES + 2 * ABF_BYTES : 2 * A_BYTES;      // offset of W_hi in the stage
+                        constexpr int W0 = A_BYTES + 2 * ABF_BYTES;         // offset of W_hi in the stage
                         for (int h = 0; h < 2; ++h) {                       // the map's box is 128 rows: two per tile
-                            tma_load_2d(sm + W0 + h * (WT / 2), &mapW, sl * BK, nt * BN + h * 128, full + st);
-                            if (EXACT || BF)
-                                tma_load_2d(sm + W0 + WT + h * (WT / 2), &mapW, sl * BK, p.n_total + nt * BN + h * 128, full + st);
+                            tma_load_2d(sm + W0 + h * (WBF_BYTES / 2), &mapW, sl * BK, nt * BN + h * 128, full + st);
+                            tma_load_2d(sm + W0 + WBF_BYTES + h * (WBF_BYTES / 2), &mapW, sl * BK, p.n_total + nt * BN + h * 128,
+                                        full + st);
                         }
                     }
             }
@@ -155,74 +142,39 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 3] = clock64();
                     unsigned char* sm = stage_mem + st * SB;
                     // ---- split this warpgroup's 64 rows of the raw A slab (rows are 64 bytes = 4 float4)
-                    if constexpr (BF) {
-                        // raw slab: 128 rows x 64 bytes, 64B-swizzled by the TMA (16-byte chunk c of row r sits at c ^ ((r>>1)&3));
-                        // operand tiles: 128 rows x 32 bytes of bf16, 32B swizzle (chunk c of row r sits at c ^ ((r>>2)&1))
-                        const float4* raw = reinterpret_cast<const float4*>(sm);
-                        unsigned char* ahi = sm + A_BYTES;
-                        unsigned char* alo = ahi + ABF_BYTES;
+                    // raw slab: 128 rows x 64 bytes, 64B-swizzled by the TMA (16-byte chunk c of row r sits at c ^ ((r>>1)&3));
+                    // operand tiles: 128 rows x 32 bytes of bf16, 32B swizzle (chunk c of row r sits at c ^ ((r>>2)&1))
+                    const float4* raw = reinterpret_cast<const float4*>(sm);
+                    unsigned char* ahi = sm + A_BYTES;
+                    unsigned char* alo = ahi + ABF_BYTES;
 #pragma unroll
-                        for (int i = g * 256 + gtid; i < g * 256 + 256; i += 128) {
-                            const float4 x = raw[i];
-                            const int row = i >> 2, lch = (i & 3) ^ ((row >> 1) & 3);      // logical chunk: fp32 k = 4*lch .. 4*lch+3
-                            const __nv_bfloat162 h01 = __floats2bfloat162_rn(x.x, x.y), h23 = __floats2bfloat162_rn(x.z, x.w);
-                            const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
-                            const __nv_bfloat162 l01 = __floats2bfloat162_rn(x.x - f01.x, x.y - f01.y);
-                            const __nv_bfloat162 l23 = __floats2bfloat162_rn(x.z - f23.x, x.w - f23.y);
-                            const unsigned off = (unsigned)row * 32u + ((unsigned)((lch >> 1) ^ ((row >> 2) & 1)) << 4) + (unsigned)(lch & 1) * 8u;
-                            uint2 hv, lv;
-                            hv.x = *reinterpret_cast<const unsigned*>(&h01); hv.y = *reinterpret_cast<const unsigned*>(&h23);
-                            lv.x = *reinterpret_cast<const unsigned*>(&l01); lv.y = *reinterpret_cast<const unsigned*>(&l23);
-                            *reinterpret_cast<uint2*>(ahi + off) = hv;
-                            *reinterpret_cast<uint2*>(alo + off) = lv;
-                        }
+                    for (int i = g * 256 + gtid; i < g * 256 + 256; i += 128) {
+                        const float4 x = raw[i];
+                        const int row = i >> 2, lch = (i & 3) ^ ((row >> 1) & 3);      // logical chunk: fp32 k = 4*lch .. 4*lch+3
+                        const __nv_bfloat162 h01 = __floats2bfloat162_rn(x.x, x.y), h23 = __floats2bfloat162_rn(x.z, x.w);
+                        const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
+                        const __nv_bfloat162 l01 = __floats2bfloat162_rn(x.x - f01.x, x.y - f01.y);
+                        const __nv_bfloat162 l23 = __floats2bfloat162_rn(x.z - f23.x, x.w - f23.y);
+                        const unsigned off = (unsigned)row * 32u + ((unsigned)((lch >> 1) ^ ((row >> 2) & 1)) << 4) + (unsigned)(lch & 1) * 8u;
+                        uint2 hv, lv;
+                        hv.x = *reinterpret_cast<const unsigned*>(&h01); hv.y = *reinterpret_cast<const unsigned*>(&h23);
+                        lv.x = *reinterpret_cast<const unsigned*>(&l01); lv.y = *reinterpret_cast<const unsigned*>(&l23);
+                        *reinterpret_cast<uint2*>(ahi + off) = hv;
+                        *reinterpret_cast<uint2*>(alo + off) = lv;
                     }
-                    if constexpr (EXACT) {
-                        float4* hi = reinterpret_cast<float4*>(sm);
-                        float4* lo = reinterpret_cast<float4*>(sm + A_BYTES);
-#pragma unroll
-                        for (int i = g * 256 + gtid; i < g * 256 + 256; i += 128) {
-                            const float4 x = hi[i];
-                            float4 h, l;
-                            unsigned u;
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.x)); h.x = __uint_as_float(u); l.x = x.x - h.x;
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.y)); h.y = __uint_as_float(u); l.y = x.y - h.y;
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.z)); h.z = __uint_as_float(u); l.z = x.z - h.z;
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x.w)); h.w = __uint_as_float(u); l.w = x.w - h.w;
-                            hi[i] = h;
-                            lo[i] = l;
-                        }
-                    }
-                    if constexpr (EXACT || BF) {
-                        fence_async_smem();                       // generic writes -> visible to the MMA
-                        wg_bar(1 + g, 128);
-                    }
+                    fence_async_smem();                       // generic writes -> visible to the MMA
+                    wg_bar(1 + g, 128);
                     if (p.dbg && blockIdx.x == 0 && it < 512 && tid == 0) p.dbg[it * 8 + 4] = clock64();
                     // ---- MMAs of this warpgroup's 64 rows against both 128-row halves of the weight tile
                     const unsigned sa = s32(sm);
                     wgmma_fence();
-                    if constexpr (BF) {
-                        const unsigned a_hi = sa + A_BYTES + g * 64 * 32, a_lo = a_hi + ABF_BYTES;
+                    const unsigned a_hi = sa + A_BYTES + g * 64 * 32, a_lo = a_hi + ABF_BYTES;
 #pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const unsigned w_hi = sa + A_BYTES + 2 * ABF_BYTES + h * (WBF_BYTES / 2), w_lo = w_hi + WBF_BYTES;
-                            wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_hi), sl != 0);
-                            wgmma_bf16_t00(acc[h], desc32(a_lo), desc32(w_hi), 1u);
-                            wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_lo), 1u);
-                        }
-                    } else {
-                        const unsigned a_hi = sa + g * 64 * 64, a_lo = a_hi + A_BYTES;
-#pragma unroll
-                        for (int kk = 0; kk < BK / 8; ++kk)          // 8 tf32 = 32 bytes per k-step
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                const unsigned w_hi = sa + 2 * A_BYTES + h * (W_BYTES / 2) + kk * 32, w_lo = w_hi + W_BYTES;
-                                wgmma_tf32(acc[h], desc64(a_hi + kk * 32), desc64(w_hi), (sl | kk) != 0);
-                                if (EXACT) {
-                                    wgmma_tf32(acc[h], desc64(a_lo + kk * 32), desc64(w_hi), 1u);
-                                    wgmma_tf32(acc[h], desc64(a_hi + kk * 32), desc64(w_lo), 1u);
-                                }
-                            }
+                    for (int h = 0; h < 2; ++h) {
+                        const unsigned w_hi = sa + A_BYTES + 2 * ABF_BYTES + h * (WBF_BYTES / 2), w_lo = w_hi + WBF_BYTES;
+                        wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_hi), sl != 0);
+                        wgmma_bf16_t00(acc[h], desc32(a_lo), desc32(w_hi), 1u);
+                        wgmma_bf16_t00(acc[h], desc32(a_hi), desc32(w_lo), 1u);
                     }
                     wgmma_commit();
                     wgmma_wait0();
@@ -296,9 +248,18 @@ frames_gemm_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 }
 
 // ---------------------------------------------------------------------------------------------- weight packing
-// pass A: rows in tile order (tile p: F channels 128p.., then G channels 128p..), columns kk = j*R + r; hi then lo copy
+// Every packed weight array is [2][rows][K] bf16: element i of a [rows][K] image as hi = bf16(x) at i, lo = bf16(x - hi) at
+// total + i.
+__device__ __forceinline__ void put_pair(__nv_bfloat16* __restrict__ w, long long total, long long i, float v) {
+    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+    w[i] = hi;
+    w[total + i] = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+
+// pass A: rows in tile order (tile p: F channels 128p.., then G channels 128p..), columns kk = j*R + r
 __global__ void pack_a_kernel(const float* __restrict__ wf, const float* __restrict__ wg, const float* __restrict__ bf,
-                              const float* __restrict__ bg, int R, int D, int k, float* __restrict__ wa, float* __restrict__ ba) {
+                              const float* __restrict__ bg, int R, int D, int k, __nv_bfloat16* __restrict__ wa,
+                              float* __restrict__ ba) {
     const int K = k * R, N = 2 * D;
     const long long total = (long long)N * K;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -306,75 +267,45 @@ __global__ void pack_a_kernel(const float* __restrict__ wf, const float* __restr
         const int tile = n / 256, w = n % 256, ch = tile * 128 + (w & 127);
         const bool is_g = w >= 128;
         const int j = kk / R, r = kk % R;
-        const float v = (is_g ? wg : wf)[((size_t)ch * R + r) * k + j];
-        unsigned u;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-        const float hi = __uint_as_float(u);
-        wa[i] = hi;
-        wa[total + i] = v - hi;
+        put_pair(wa, total, i, (is_g ? wg : wf)[((size_t)ch * R + r) * k + j]);
         if (kk == 0) {
             const float* bsrc = is_g ? bg : bf;
             ba[n] = bsrc ? bsrc[ch] : 0.f;
         }
     }
 }
-// pass B: rows = residual outputs then skip outputs, columns = dilation channel; hi then lo copy
+// pass B: rows = residual outputs then skip outputs, columns = dilation channel
 __global__ void pack_b_kernel(const float* __restrict__ wr, const float* __restrict__ ws, const float* __restrict__ br,
-                              const float* __restrict__ bs, int R, int D, int S, float* __restrict__ wb, float* __restrict__ bb) {
+                              const float* __restrict__ bs, int R, int D, int S, __nv_bfloat16* __restrict__ wb,
+                              float* __restrict__ bb) {
     const int N = R + S;
     const long long total = (long long)N * D;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int n = (int)(i / D), c = (int)(i % D);
-        const float v = n < R ? wr[(size_t)n * D + c] : ws[(size_t)(n - R) * D + c];
-        unsigned u;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-        const float hi = __uint_as_float(u);
-        wb[i] = hi;
-        wb[total + i] = v - hi;
+        put_pair(wb, total, i, n < R ? wr[(size_t)n * D + c] : ws[(size_t)(n - R) * D + c]);
         if (c == 0) bb[n] = n < R ? (br ? br[n] : 0.f) : (bs ? bs[n - R] : 0.f);
     }
 }
 
 // backward dz: rows = dilation channels c, columns k: [0,R) = residual_conv.weight[k][c], [R,R+S) = skip_conv.weight[k-R][c]
 __global__ void pack_dz_kernel(const float* __restrict__ wr, const float* __restrict__ ws, int R, int D, int S,
-                               float* __restrict__ w) {
+                               __nv_bfloat16* __restrict__ w) {
     const int K = R + S;
     const long long total = (long long)D * K;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(i / K), kk = (int)(i % K);
-        const float v = kk < R ? wr[(size_t)kk * D + c] : ws[(size_t)(kk - R) * D + c];
-        unsigned u;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-        const float hi = __uint_as_float(u);
-        w[i] = hi;
-        w[total + i] = v - hi;
+        put_pair(w, total, i, kk < R ? wr[(size_t)kk * D + c] : ws[(size_t)(kk - R) * D + c]);
     }
 }
 // backward dh_in: rows = residual channels r, columns j*2D + n: [filter;gate].weight[n][r][j]
 __global__ void pack_dh_kernel(const float* __restrict__ wf, const float* __restrict__ wg, int R, int D, int k,
-                               float* __restrict__ w) {
+                               __nv_bfloat16* __restrict__ w) {
     const int K = k * 2 * D;
     const long long total = (long long)R * K;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int r = (int)(i / K), kk = (int)(i % K);
         const int j = kk / (2 * D), n = kk % (2 * D);
-        const float v = n < D ? wf[((size_t)n * R + r) * k + j] : wg[((size_t)(n - D) * R + r) * k + j];
-        unsigned u;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-        const float hi = __uint_as_float(u);
-        w[i] = hi;
-        w[total + i] = v - hi;
-    }
-}
-
-// fp32 (hi | lo) tf32-split pair arrays -> bf16 (hi | lo) pair arrays of the same shape.  hi + lo is the original
-// weight exactly (lo = x - rna_tf32(x) is exact in fp32), so x is recovered and re-split for bf16.
-__global__ void convert_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const float x = src[i] + src[n + i];
-        const __nv_bfloat16 h = __float2bfloat16_rn(x);
-        dst[i] = h;
-        dst[n + i] = __float2bfloat16_rn(x - __bfloat162float(h));
+        put_pair(w, total, i, n < D ? wf[((size_t)n * R + r) * k + j] : wg[((size_t)(n - D) * R + r) * k + j]);
     }
 }
 
@@ -407,38 +338,33 @@ static int make_act_map(CUtensorMap* m, const float* base, int B, int L, int C, 
     WN_REQUIRE(r == CUDA_SUCCESS, WN_E_UNSUPP, "cuTensorMapEncodeTiled(activations) failed with %d", (int)r);
     return 0;
 }
-// weights (rows, K) fp32 K-major: dims {K, rows}, box {BK, 128}
-// `col0`: first K column (element offset into every row); bf16 = true: the array holds bf16 pairs (32-byte slab rows)
-static int make_w_map(CUtensorMap* m, const void* base, int rows, int K, int col0 = 0, bool bf16 = false) {
+// weights (rows, K) bf16 K-major, one plane of a [2][rows][K] pair array: dims {K, rows}, box {BK, 128} (32-byte slab rows)
+// `col0`: first K column (element offset into every row)
+static int make_w_map(CUtensorMap* m, const void* base, int rows, int K, int col0 = 0) {
     EncodeTiledFn fn = encode_fn();
     WN_REQUIRE(fn, WN_E_UNSUPP, "cuTensorMapEncodeTiled is not available from this driver");
-    const int es = bf16 ? 2 : 4;
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)K * es};
+    cuuint64_t strides[1] = {(cuuint64_t)K * 2};
     cuuint32_t box[2] = {BK, BN / 2};           // half a tile: 128 rows
     cuuint32_t estr[2] = {1, 1};
-    const int row_bytes = BK * es;
-    CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
-                    (void*)((const unsigned char*)base + (size_t)col0 * es), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B),
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)((const unsigned char*)base + (size_t)col0 * 2), dims, strides,
+                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     WN_REQUIRE(r == CUDA_SUCCESS, WN_E_UNSUPP, "cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
     return 0;
 }
 
-static size_t tc_smem_bytes(int n_total, int prec) {
-    const size_t ring = prec == PREC_BF16X2 ? (size_t)STAGES_BF * STAGE_BYTES_BF : (size_t)STAGES * STAGE_BYTES;
-    return 1024 + ring + 512 + sizeof(float) * ((n_total + 3) & ~3);
+static size_t tc_smem_bytes(int n_total) {
+    return 1024 + (size_t)STAGES * STAGE_BYTES + 512 + sizeof(float) * ((n_total + 3) & ~3);
 }
 
-template <int EPI, int PREC>
+template <int EPI>
 static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mW, const TcParams& p, cudaStream_t st) {
     int dev = 0, sms = 0;
     WN_CUDA(cudaGetDevice(&dev));
     WN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const size_t smem = tc_smem_bytes(p.n_total, PREC);
-    WN_CUDA(cudaFuncSetAttribute(frames_gemm_tc<EPI, PREC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = tc_smem_bytes(p.n_total);
+    WN_CUDA(cudaFuncSetAttribute(frames_gemm_tc<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int items = p.B * ((p.L - p.t_begin + BM - 1) / BM);
     const int grid = items < sms ? items : sms;
     cudaLaunchConfig_t cfg = {};
@@ -446,16 +372,9 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtens
     cfg.blockDim = dim3(NTHREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    WN_CUDA(cudaLaunchKernelEx(&cfg, frames_gemm_tc<EPI, PREC>, mA, mA2, mW, p));
+    WN_CUDA(cudaLaunchKernelEx(&cfg, frames_gemm_tc<EPI>, mA, mA2, mW, p));
     WN_CUDA(cudaGetLastError());
     return 0;
-}
-template <int EPI>
-static int launch_tc_prec(int prec, const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mW, const TcParams& p,
-                          cudaStream_t st) {
-    if (prec == PREC_BF16X2) return launch_tc<EPI, PREC_BF16X2>(mA, mA2, mW, p, st);
-    if (prec == PREC_TF32X1) return launch_tc<EPI, PREC_TF32X1>(mA, mA2, mW, p, st);
-    return launch_tc<EPI, PREC_TF32X3>(mA, mA2, mW, p, st);
 }
 
 
@@ -628,12 +547,12 @@ extern "C" int wn_tc_supported(int R, int D, int S, int k) {
 
 extern "C" int wn_tc_pack_block_weights(const float* d_wf, const float* d_wg, const float* d_bf, const float* d_bg,
                                         const float* d_wr, const float* d_ws, const float* d_br, const float* d_bs, int R,
-                                        int D, int S, int k, float* d_wa, float* d_ba, float* d_wb, float* d_bb, void* stream) {
+                                        int D, int S, int k, void* d_wa, float* d_ba, void* d_wb, float* d_bb, void* stream) {
     WN_REQUIRE(d_wf && d_wg && d_wr && d_ws && d_wa && d_ba && d_wb && d_bb, WN_E_BADARG, "wn_tc_pack_block_weights: null pointer");
     WN_REQUIRE(wn_tc_supported(R, D, S, k), WN_E_UNSUPP, "wn_tc_pack_block_weights: shape R=%d D=%d S=%d not supported", R, D, S);
     cudaStream_t st = (cudaStream_t)stream;
-    tc::pack_a_kernel<<<1024, 256, 0, st>>>(d_wf, d_wg, d_bf, d_bg, R, D, k, d_wa, d_ba);
-    tc::pack_b_kernel<<<512, 256, 0, st>>>(d_wr, d_ws, d_br, d_bs, R, D, S, d_wb, d_bb);
+    tc::pack_a_kernel<<<1024, 256, 0, st>>>(d_wf, d_wg, d_bf, d_bg, R, D, k, (__nv_bfloat16*)d_wa, d_ba);
+    tc::pack_b_kernel<<<512, 256, 0, st>>>(d_wr, d_ws, d_br, d_bs, R, D, S, (__nv_bfloat16*)d_wb, d_bb);
     WN_CUDA(cudaGetLastError());
     return 0;
 }
@@ -649,12 +568,9 @@ extern "C" int wn_tc_block_fwd(const wn_tc_block_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     CUtensorMap mA, mWa, mZ, mWb;
     if (int rc = tc::make_act_map(&mA, a->d_h_in, a->B, a->L, a->R, a->in_start)) return rc;
-    const int prec = a->fast_tf32;            // 0: 3xTF32, 1: single TF32, 2: bf16 pairs (d_wa / d_wb from wn_tc_convert_weights_bf16)
-    WN_REQUIRE(prec >= 0 && prec <= 2, WN_E_BADARG, "wn_tc_block_fwd: fast_tf32 (precision mode) must be 0, 1 or 2");
-    const bool bf = prec == tc::PREC_BF16X2;
-    if (int rc = tc::make_w_map(&mWa, a->d_wa, 2 * 2 * a->D, a->k * a->R, 0, bf)) return rc;
+    if (int rc = tc::make_w_map(&mWa, a->d_wa, 2 * 2 * a->D, a->k * a->R)) return rc;
     if (int rc = tc::make_act_map(&mZ, a->d_z, a->B, a->L, a->D, a->out_start)) return rc;
-    if (int rc = tc::make_w_map(&mWb, a->d_wb, 2 * (a->R + a->S), a->D, 0, bf)) return rc;
+    if (int rc = tc::make_w_map(&mWb, a->d_wb, 2 * (a->R + a->S), a->D)) return rc;
     tc::TcParams p;
     memset(&p, 0, sizeof(p));
     if (getenv("WN_TC_TRACE")) {
@@ -667,13 +583,13 @@ extern "C" int wn_tc_block_fwd(const wn_tc_block_args* a, void* stream) {
     p.taps = a->k; p.dil = a->dilation; p.C = a->R; p.a_origin = a->in_start;
     p.n_total = 2 * a->D; p.n_tiles = p.n_total / tc::BN;
     p.bias = a->d_ba; p.out0 = a->d_z; p.out1 = a->d_fg_save; p.res = nullptr;
-    if (int rc = tc::launch_tc_prec<tc::EPI_GATE>(prec, mA, mA, mWa, p, st)) return rc;
+    if (int rc = tc::launch_tc<tc::EPI_GATE>(mA, mA, mWa, p, st)) return rc;
     // pass B: residual + skip 1x1
     if (const char* which = getenv("WN_TC_TRACE_PASS")) { if (which[0] == 'A') p.dbg = nullptr; }     // keep pass A's stamps
     p.taps = 1; p.dil = 0; p.C = a->D; p.a_origin = a->out_start;
     p.n_total = a->R + a->S; p.n_tiles = p.n_total / tc::BN;
     p.bias = a->d_bb; p.out0 = a->d_h_out; p.out1 = a->d_skip; p.res = a->d_h_in;
-    return tc::launch_tc_prec<tc::EPI_RES_SKIP>(prec, mZ, mZ, mWb, p, st);
+    return tc::launch_tc<tc::EPI_RES_SKIP>(mZ, mZ, mWb, p, st);
 }
 
 extern "C" int wn_tc_bwd_supported(int R, int D, int S, int k) {
@@ -681,28 +597,20 @@ extern "C" int wn_tc_bwd_supported(int R, int D, int S, int k) {
 }
 
 extern "C" int wn_tc_pack_block_bwd_weights(const float* d_wf, const float* d_wg, const float* d_wr, const float* d_ws, int R,
-                                            int D, int S, int k, float* d_wdz, float* d_wdh, void* stream) {
+                                            int D, int S, int k, void* d_wdz, void* d_wdh, void* stream) {
     WN_REQUIRE(d_wf && d_wg && d_wr && d_ws && d_wdz && d_wdh, WN_E_BADARG, "wn_tc_pack_block_bwd_weights: null pointer");
     WN_REQUIRE(wn_tc_bwd_supported(R, D, S, k), WN_E_UNSUPP, "wn_tc_pack_block_bwd_weights: shape not supported");
     cudaStream_t st = (cudaStream_t)stream;
-    tc::pack_dz_kernel<<<512, 256, 0, st>>>(d_wr, d_ws, R, D, S, d_wdz);
-    tc::pack_dh_kernel<<<1024, 256, 0, st>>>(d_wf, d_wg, R, D, k, d_wdh);
+    tc::pack_dz_kernel<<<512, 256, 0, st>>>(d_wr, d_ws, R, D, S, (__nv_bfloat16*)d_wdz);
+    tc::pack_dh_kernel<<<1024, 256, 0, st>>>(d_wf, d_wg, R, D, k, (__nv_bfloat16*)d_wdh);
     WN_CUDA(cudaGetLastError());
     return 0;
 }
 
-// Tensor-core form of wn_block_bwd_data (same arguments; d_wrs_rows / d_wfg_bwd are replaced by the packed, pre-split
+// Tensor-core form of wn_block_bwd_data (same arguments; d_wrs_rows / d_wfg_bwd are replaced by the packed bf16 pairs
 // d_wdz [2][D][R+S] and d_wdh [2][R][k*2D] of wn_tc_pack_block_bwd_weights).
-extern "C" int wn_tc_block_bwd_data(const wn_block_bwd_args* a, const float* d_wdz, const float* d_wdh, void* stream) {
-    return wn_tc_block_bwd_data_prec(a, d_wdz, d_wdh, 0, stream);
-}
-
-// precision: 0 = 3xTF32 on the fp32 pair arrays, 2 = bf16 pairs (arrays converted by wn_tc_convert_weights_bf16)
-extern "C" int wn_tc_block_bwd_data_prec(const wn_block_bwd_args* a, const void* d_wdz, const void* d_wdh, int precision,
-                                         void* stream) {
+extern "C" int wn_tc_block_bwd_data(const wn_block_bwd_args* a, const void* d_wdz, const void* d_wdh, void* stream) {
     WN_REQUIRE(a && d_wdz && d_wdh, WN_E_BADARG, "wn_tc_block_bwd_data: null args");
-    WN_REQUIRE(precision == 0 || precision == 2, WN_E_BADARG, "wn_tc_block_bwd_data: precision must be 0 (3xTF32) or 2 (bf16 pairs)");
-    const bool bf = precision == 2;
     WN_REQUIRE(a->d_dskip && a->d_fg && a->d_dfg && a->d_z && a->d_dh_in, WN_E_BADARG, "wn_tc_block_bwd_data: null pointer");
     WN_REQUIRE(wn_tc_bwd_supported(a->R, a->D, a->S, a->k), WN_E_UNSUPP, "wn_tc_block_bwd_data: shape not supported");
     WN_REQUIRE(a->gz >= a->out_start && a->gz < a->L && a->gs_in >= a->in_start && a->gs_in <= a->gz && a->ds_start >= a->out_start &&
@@ -715,7 +623,7 @@ extern "C" int wn_tc_block_bwd_data_prec(const wn_block_bwd_args* a, const void*
     if (int rc = tc::make_act_map(&mDs, a->d_dskip, B, L - a->ds_start, S, 0)) return rc;          // (B, L-ds_start, S): own frame axis
     if (have_dh) { if (int rc = tc::make_act_map(&mDh, a->d_dh_out, B, L, R, a->gs_out)) return rc; }
     else mDh = mDs;
-    if (int rc = tc::make_w_map(&mW1, d_wdz, 2 * D, R + S, have_dh ? 0 : R, bf)) return rc;       // without dh_out: start at column R
+    if (int rc = tc::make_w_map(&mW1, d_wdz, 2 * D, R + S, have_dh ? 0 : R)) return rc;       // without dh_out: start at column R
     tc::TcParams p;
     memset(&p, 0, sizeof(p));
     p.B = B; p.L = L; p.D = D; p.R = R; p.S = S;
@@ -725,24 +633,17 @@ extern "C" int wn_tc_block_bwd_data_prec(const wn_block_bwd_args* a, const void*
     p.C2 = S; p.a2_origin = a->ds_start;
     p.n_total = D; p.n_tiles = D / tc::BN;
     p.bias = nullptr; p.out0 = a->d_dfg; p.out2 = a->d_z; p.res = a->d_fg;
-    if (int rc = tc::launch_tc_prec<tc::EPI_GATE_BWD>(precision, mDh, mDs, mW1, p, st)) return rc;
+    if (int rc = tc::launch_tc<tc::EPI_GATE_BWD>(mDh, mDs, mW1, p, st)) return rc;
     // ---- dh_in = dh_out (identity) + anti-causal taps of dfg, for frames [gs_in, L)
     if (int rc = tc::make_act_map(&mDfg, a->d_dfg, B, L, 2 * D, a->gz)) return rc;
-    if (int rc = tc::make_w_map(&mW2, d_wdh, 2 * R, a->k * 2 * D, 0, bf)) return rc;
+    if (int rc = tc::make_w_map(&mW2, d_wdh, 2 * R, a->k * 2 * D)) return rc;
     p.t_begin = a->gs_in;
     p.taps = a->k; p.dil = -a->dilation; p.C = 2 * D; p.a_origin = a->gz;
     p.C2 = 0; p.a2_origin = 0;
     p.n_total = R; p.n_tiles = R / tc::BN;
     p.out0 = a->d_dh_in; p.out2 = nullptr; p.res = a->d_dh_out;
     p.id_start = a->gs_out > a->out_start ? a->gs_out : a->out_start;
-    return tc::launch_tc_prec<tc::EPI_ADD>(precision, mDfg, mDfg, mW2, p, st);
-}
-
-extern "C" int wn_tc_convert_weights_bf16(const float* d_pairs, void* d_out, long long n_per_half, void* stream) {
-    WN_REQUIRE(d_pairs && d_out && n_per_half > 0, WN_E_BADARG, "wn_tc_convert_weights_bf16: null pointer or empty array");
-    tc::convert_bf16_kernel<<<512, 256, 0, (cudaStream_t)stream>>>(d_pairs, (__nv_bfloat16*)d_out, n_per_half);
-    WN_CUDA(cudaGetLastError());
-    return 0;
+    return tc::launch_tc<tc::EPI_ADD>(mDfg, mDfg, mW2, p, st);
 }
 
 // Tensor-core form of wn_wgrad (same argument block and workspace): C must be 256 and N a multiple of 128, pitches and

@@ -53,7 +53,7 @@ class TcBlockArgs(C.Structure):
                 ("d_wa", C.c_void_p), ("d_ba", C.c_void_p), ("d_wb", C.c_void_p), ("d_bb", C.c_void_p),
                 ("B", C.c_int), ("L", C.c_int), ("R", C.c_int), ("D", C.c_int), ("S", C.c_int), ("k", C.c_int),
                 ("dilation", C.c_int), ("in_start", C.c_int), ("out_start", C.c_int), ("skip_start", C.c_int),
-                ("skip_init", C.c_int), ("d_fg_save", C.c_void_p), ("fast_tf32", C.c_int)]
+                ("skip_init", C.c_int), ("d_fg_save", C.c_void_p)]
 
 
 PREC_BF16, PREC_BF16_PAIRS = 1, 2        # WN_PREC_* of include/wavenet_b200.h
@@ -192,8 +192,6 @@ SIGNATURES = {
     "wn_tc_bwd_supported": (C.c_int, [C.c_int] * 4),
     "wn_tc_pack_block_bwd_weights": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 4 + [C.c_void_p] * 3),
     "wn_tc_block_bwd_data": (C.c_int, [C.POINTER(BlockBwdArgs), C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wn_tc_block_bwd_data_prec": (C.c_int, [C.POINTER(BlockBwdArgs), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
-    "wn_tc_convert_weights_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "wn_ce_workspace_bytes": (C.c_size_t, []),
     "wn_ce_fwd_bwd": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 2 + [C.c_void_p]),
     "wn_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_float] * 5 + [C.c_int, C.c_void_p]),
@@ -239,7 +237,7 @@ def lib() -> C.CDLL:
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(handle, name)          # AttributeError here == header and library disagree
             fn.restype, fn.argtypes = res, args
-        if handle.wn_version() != 2:
+        if handle.wn_version() != 3:
             raise RuntimeError("wavenet_b200: ABI version mismatch between native.py and libwavenet_b200.so")
         _lib = handle
     return _lib

@@ -1,11 +1,13 @@
 """WaveNetModel with the reference's constructor, attributes, state_dict and methods
 (reference wavenet_model.py), running its two hot paths on hand-written sm_90a CUDA kernels:
 
-* ``forward`` / ``wavenet``   -> start gather/GEMM, the residual blocks (256-channel nets: two wgmma launches per
-                                 block with bf16-pair operands, wn_tc_block_fwd; any other shape: ONE fused fp32 kernel
-                                 per block, wn_block_fwd), fused head (wn_start_fwd_*, wn_head_fwd)
-* ``loss.backward()``         -> wn_head_bwd_data, per block wn_tc_block_bwd_data_prec / wn_block_bwd_data for the data
-                                 gradients and wn_tc_wgrad / wn_wgrad for the weight gradients (a custom autograd node)
+* ``forward`` / ``wavenet``   -> start gather/GEMM, the residual blocks (R = D = S = 256 or 512 with k = 2: the fused
+                                 tensor-core block, wn_tb_*; other shapes the tensor cores cover: two wgmma launches per
+                                 block with bf16-pair operands, wn_tc_block_fwd; any other shape: ONE fused fp32 kernel per
+                                 block, wn_block_fwd), fused head (wn_start_fwd_*, wn_head_fwd)
+* ``loss.backward()``         -> wn_head_bwd_data, per block wn_tb_block_bwd_data / wn_tc_block_bwd_data / wn_block_bwd_data
+                                 for the data gradients and wn_tb_wgrad / wn_tc_wgrad / wn_wgrad for the weight gradients
+                                 (a custom autograd node)
 * ``generate_fast``           -> ONE persistent kernel for the whole sampling loop (wn_gen_run)
 
 Host code is plumbing only (shape planning, buffer ownership, weight packing cache).  There is no eager /
@@ -72,8 +74,8 @@ def prefill_window(T, dilations, kernel_size, hop=1):
 class _Packs:
     """Lazily built packed weight groups of one model state (see _Runtime.packed_weights):
       layers              K-outer fp32 copies for the SIMT block kernels
-      tc_layers[_bf16]    K-major pre-split pairs for the two-launch tensor-core blocks (fp32 tf32-split / bf16)
-      tc_bwd_layers[_bf16] the same for the tensor-core data-gradient GEMMs
+      tc_layers           K-major bf16 (hi, lo) pair arrays for the two-launch tensor-core blocks
+      tc_bwd_layers       the same for the tensor-core data-gradient GEMMs
       tb                  all layers' slot images + biases for the fused tensor-core block (wn_tb_block_fwd)
       start / end1 / end2 K-outer 1x1 weights
     """
@@ -119,12 +121,13 @@ class _Packs:
         R, D, S, E, Cc, k, nl = self._dims()
         P = rt._params()
         f32 = dict(device=rt.device(), dtype=torch.float32)
+        bf16 = dict(device=rt.device(), dtype=torch.bfloat16)
         out = []
         for i in range(nl):
             (wf, bf), (wg, bg) = P["filt"][i], P["gate"][i]
             (wr, br), (wsk, bs) = P["res"][i], P["skip"][i]
-            wa, ba = torch.empty(2, 2 * D, k * R, **f32), torch.empty(2 * D, **f32)
-            wb, bb = torch.empty(2, R + S, D, **f32), torch.empty(R + S, **f32)
+            wa, ba = torch.empty(2, 2 * D, k * R, **bf16), torch.empty(2 * D, **f32)
+            wb, bb = torch.empty(2, R + S, D, **bf16), torch.empty(R + S, **f32)
             native.check(lib.wn_tc_pack_block_weights(
                 wf.data_ptr(), wg.data_ptr(), native.ptr(bf), native.ptr(bg), wr.data_ptr(), wsk.data_ptr(),
                 native.ptr(br), native.ptr(bs), R, D, S, k, wa.data_ptr(), ba.data_ptr(), wb.data_ptr(),
@@ -132,25 +135,19 @@ class _Packs:
             out.append((wa, ba, wb, bb))
         return out
 
-    def _build_tc_layers_bf16(self, stream):
-        return [(self.rt._bf16_pairs(wa, stream), ba, self.rt._bf16_pairs(wb, stream), bb) for wa, ba, wb, bb in self["tc_layers"]]
-
     def _build_tc_bwd_layers(self, stream):
         rt, lib = self.rt, native.lib()
         R, D, S, E, Cc, k, nl = self._dims()
         P = rt._params()
-        f32 = dict(device=rt.device(), dtype=torch.float32)
+        bf16 = dict(device=rt.device(), dtype=torch.bfloat16)
         out = []
         for i in range(nl):
             wf, wg, wr, wsk = P["filt"][i][0], P["gate"][i][0], P["res"][i][0], P["skip"][i][0]
-            wdz, wdh = torch.empty(2, D, R + S, **f32), torch.empty(2, R, k * 2 * D, **f32)
+            wdz, wdh = torch.empty(2, D, R + S, **bf16), torch.empty(2, R, k * 2 * D, **bf16)
             native.check(lib.wn_tc_pack_block_bwd_weights(wf.data_ptr(), wg.data_ptr(), wr.data_ptr(), wsk.data_ptr(),
                                                           R, D, S, k, wdz.data_ptr(), wdh.data_ptr(), stream), "pack tc bwd")
             out.append((wdz, wdh))
         return out
-
-    def _build_tc_bwd_layers_bf16(self, stream):
-        return [(self.rt._bf16_pairs(a, stream), self.rt._bf16_pairs(b, stream)) for a, b in self["tc_bwd_layers"]]
 
     def _ptr_table(self):
         """DEVICE table [n_layers][8] of parameter pointers {wf, wg, bf, bg, wr, ws, br, bs} (0 = no bias), cached on the
@@ -300,9 +297,8 @@ class _Runtime:
         self.samplers = {}
         self.weights_epoch = 0                # bumped by invalidate(): parameters were written behind the version counters
         self.block_mode = "auto"     # "auto": tensor-core blocks when the shape allows, "ffma": exact-fp32 SIMT, "tc"
-        self.fast_tf32 = False       # opt-in single-pass TF32 blocks (~1e-3 on the logits: outside the parity bar)
-        self.tc_precision = "bf16x2"  # tensor-core operand split: "tf32x3" (3xTF32) or "bf16x2" (bf16 pairs, 2x the MMA rate)
-        self.wgrad_mode = "tc"        # weight gradients: "tc" (tensor cores where the shape allows), "native" (fp32 FMA), "cublas"
+        self.tc_precision = "bf16x2"  # "bf16x2" (bf16 pairs, fp32-class) or "bf16" (single-pass on the fused blocks, tb_precision)
+        self.wgrad_mode = "tc"        # weight gradients: "tc" (tensor cores where the shape allows) or "native" (fp32 FMA)
         self.local_table_bytes = 256 << 20   # sampler: largest local-conditioning table window (at least one frame is built)
 
     # ------------------------------------------------------------------ weights
@@ -338,14 +334,6 @@ class _Runtime:
             raise RuntimeError("wavenet_b200: the model must be on a CUDA device (model.cuda()); "
                                "there is no CPU path in this implementation")
         return dev
-
-    @staticmethod
-    def _bf16_pairs(pairs, stream):
-        """(2, rows, K) fp32 tf32-split pair array -> (2, rows, K) bf16 pair array (wn_tc_convert_weights_bf16)."""
-        out = torch.empty(pairs.shape, device=pairs.device, dtype=torch.bfloat16)
-        native.check(native.lib().wn_tc_convert_weights_bf16(pairs.data_ptr(), out.data_ptr(), pairs.numel() // 2, stream),
-                     "convert bf16")
-        return out
 
     def packed_weights(self, stream):
         """The packed weight copies, built per group on first use (a path packs only what it reads) and forgotten when a
@@ -398,18 +386,17 @@ class _Runtime:
         n_layers = len(dil)
         if os.environ.get("WN_CHECK_INDICES") and index_input and (int(x.min()) < 0 or int(x.max()) >= Cc):
             raise RuntimeError(f"wavenet_b200: class index outside [0, {Cc}) (the reference's one-hot scatter raises here)")
-        if self.tc_precision not in ("tf32x3", "bf16x2", "bf16"):
-            raise ValueError(f"tc_precision must be 'bf16x2', 'bf16' or (two-launch blocks only) 'tf32x3', not {self.tc_precision!r}")
+        if self.tc_precision not in ("bf16x2", "bf16"):
+            raise ValueError(f"tc_precision must be 'bf16x2' or 'bf16', not {self.tc_precision!r}")
         if self.block_mode not in ("auto", "tb", "tc", "ffma"):
             raise ValueError(f"block_mode must be 'auto', 'tb', 'tc' or 'ffma', not {self.block_mode!r}")
-        use_tb = (self.block_mode in ("auto", "tb") and not self.fast_tf32 and self.tc_precision != "tf32x3" and
-                  bool(lib.wn_tb_supported(R, D, S, k)))
+        use_tb = self.block_mode in ("auto", "tb") and bool(lib.wn_tb_supported(R, D, S, k))
         if self.block_mode == "tb" and not use_tb:
             raise RuntimeError("wavenet_b200: the fused tensor-core block needs R = D = S in (256, 512), kernel_size = 2 "
                                f"(got {R},{D},{S},{k})")
         ctab, frames = None, None
         if cond is not None or local is not None or upsampled is not None:
-            if self.block_mode == "tc" or (self.fast_tf32 and not use_tb):
+            if self.block_mode == "tc":
                 raise RuntimeError("wavenet_b200: a conditioned model runs on the fused tensor-core blocks (block_mode 'tb' / "
                                    "'auto') or the FFMA blocks ('ffma'); the two-launch 'tc' blocks have no conditioned kernel")
             if cond is not None and cond.shape[0] != B:
@@ -467,8 +454,6 @@ class _Runtime:
             a = native.TcBlockArgs()
             a.B, a.L, a.R, a.D, a.S, a.k = B, L, R, D, S, k
             a.d_z = zws.data_ptr()
-            a.fast_tf32 = 1 if self.fast_tf32 else (0 if self.tc_precision == "tf32x3" else 2)
-            tc_key = "tc_layers_bf16" if a.fast_tf32 == 2 else "tc_layers"
         else:
             a = native.BlockArgs()
             a.B, a.L, a.R, a.D, a.S, a.k, a.mode = B, L, R, D, S, k, 0
@@ -482,7 +467,7 @@ class _Runtime:
             a.dilation, a.in_start, a.out_start, a.skip_init = d, plan.in_start[i], plan.out_start[i], int(i == 0)
             a.d_fg_save = None if save is None else fg_all[i].data_ptr()
             if use_tc:
-                wa, ba, wb, bb = W[tc_key][i]
+                wa, ba, wb, bb = W["tc_layers"][i]
                 a.d_wa, a.d_ba, a.d_wb, a.d_bb = wa.data_ptr(), ba.data_ptr(), wb.data_ptr(), bb.data_ptr()
                 native.check(lib.wn_tc_block_fwd(ctypes.byref(a), stream), f"tc block {i}")
             else:
@@ -888,40 +873,35 @@ class _Runtime:
         ds_start = L - OL
         rskip = torch.relu(skip[:, ds_start - plan.skip_start:, :])
         # weight gradients: wgrad_mode "native" = wn_wgrad (split-frames fp32 FMA kernel, wgrad.cu); "tc" = wn_tc_wgrad
-        # (tensor cores, bf16 pairs) where the shape allows, else wn_wgrad; "cublas" = torch einsums (library GEMMs)
+        # (tensor cores, bf16 pairs) where the shape allows, else wn_wgrad
         wgrad_mode = getattr(self, "wgrad_mode", "tc")
-        if wgrad_mode not in ("native", "tc", "cublas"):
-            raise ValueError(f"wgrad_mode must be 'native', 'tc' or 'cublas', not {wgrad_mode!r}")
-        native_wgrad = wgrad_mode != "cublas"
+        if wgrad_mode not in ("native", "tc"):
+            raise ValueError(f"wgrad_mode must be 'native' or 'tc', not {wgrad_mode!r}")
         self.wgrad_tc_calls = 0
-        if native_wgrad:
-            wg_work = torch.empty(max(lib.wn_wgrad_workspace_bytes(n_, c_) for n_, c_ in
-                                      ((Cc, E), (E, S), (S, D), (R, D), (2 * D, R))) // 4, **f32)
-            wa = native.WgradArgs()
-            wa.d_work, wa.B = wg_work.data_ptr(), B
+        wg_work = torch.empty(max(lib.wn_wgrad_workspace_bytes(n_, c_) for n_, c_ in
+                                  ((Cc, E), (E, S), (S, D), (R, D), (2 * D, R))) // 4, **f32)
+        wa = native.WgradArgs()
+        wa.d_work, wa.B = wg_work.data_ptr(), B
 
-            def wgrad(out, g, g_off, ldg, g_seq, x, x_off, ldx, x_seq, rows, N, C, n_stride=None, c_stride=1, out_off=0):
-                """out[n, c] (+ strides) = sum_b sum_t g[b, t, n] * x[b, t, c]; offsets in floats from the tensors' bases"""
-                wa.d_g, wa.d_x = g.data_ptr() + 4 * g_off, x.data_ptr() + 4 * x_off
-                wa.d_dw = out.data_ptr() + 4 * out_off
-                wa.ldg, wa.ldx, wa.g_seq_stride, wa.x_seq_stride = ldg, ldx, g_seq, x_seq
-                wa.rows, wa.N, wa.C = rows, N, C
-                wa.dw_n_stride, wa.dw_c_stride = (C * c_stride if n_stride is None else n_stride), c_stride
-                if (wgrad_mode == "tc" and rows >= 64 and lib.wn_tc_wgrad_supported(N, C) and ldg % 4 == 0 and ldx % 4 == 0
-                        and g_seq % 4 == 0 and x_seq % 4 == 0 and wa.d_g % 16 == 0 and wa.d_x % 16 == 0):
-                    native.check(lib.wn_tc_wgrad(ctypes.byref(wa), stream), "tc wgrad")
-                    self.wgrad_tc_calls += 1
-                else:
-                    native.check(lib.wn_wgrad(ctypes.byref(wa), stream), "wgrad")
+        def wgrad(out, g, g_off, ldg, g_seq, x, x_off, ldx, x_seq, rows, N, C, n_stride=None, c_stride=1, out_off=0):
+            """out[n, c] (+ strides) = sum_b sum_t g[b, t, n] * x[b, t, c]; offsets in floats from the tensors' bases"""
+            wa.d_g, wa.d_x = g.data_ptr() + 4 * g_off, x.data_ptr() + 4 * x_off
+            wa.d_dw = out.data_ptr() + 4 * out_off
+            wa.ldg, wa.ldx, wa.g_seq_stride, wa.x_seq_stride = ldg, ldx, g_seq, x_seq
+            wa.rows, wa.N, wa.C = rows, N, C
+            wa.dw_n_stride, wa.dw_c_stride = (C * c_stride if n_stride is None else n_stride), c_stride
+            if (wgrad_mode == "tc" and rows >= 64 and lib.wn_tc_wgrad_supported(N, C) and ldg % 4 == 0 and ldx % 4 == 0
+                    and g_seq % 4 == 0 and x_seq % 4 == 0 and wa.d_g % 16 == 0 and wa.d_x % 16 == 0):
+                native.check(lib.wn_tc_wgrad(ctypes.byref(wa), stream), "tc wgrad")
+                self.wgrad_tc_calls += 1
+            else:
+                native.check(lib.wn_wgrad(ctypes.byref(wa), stream), "wgrad")
 
-            rskip = rskip.contiguous()
-            gw2, gw1 = torch.empty(Cc, E, 1, **f32), torch.empty(E, S, 1, **f32)
-            wgrad(gw2, dlogits, 0, Cc, OL * Cc, y1, 0, E, OL * E, OL, Cc, E)
-            wgrad(gw1, dy1, 0, E, OL * E, rskip, 0, S, OL * S, OL, E, S)
-            grads["end_conv_2.weight"], grads["end_conv_1.weight"] = gw2, gw1
-        else:
-            grads["end_conv_2.weight"] = torch.einsum("btc,bte->ce", dlogits, y1).unsqueeze(-1)
-            grads["end_conv_1.weight"] = torch.einsum("bte,bts->es", dy1, rskip).unsqueeze(-1)
+        rskip = rskip.contiguous()
+        gw2, gw1 = torch.empty(Cc, E, 1, **f32), torch.empty(E, S, 1, **f32)
+        wgrad(gw2, dlogits, 0, Cc, OL * Cc, y1, 0, E, OL * E, OL, Cc, E)
+        wgrad(gw1, dy1, 0, E, OL * E, rskip, 0, S, OL * S, OL, E, S)
+        grads["end_conv_2.weight"], grads["end_conv_1.weight"] = gw2, gw1
         grads["end_conv_2.bias"] = dlogits.sum((0, 1))
         grads["end_conv_1.bias"] = dy1.sum((0, 1))
         reducer = getattr(self, "grad_reducer", None)      # data_parallel.GradientAverager or None
@@ -933,8 +913,7 @@ class _Runtime:
         zbuf = torch.empty(B, L, D, **f32)
         dh_a, dh_b = torch.empty(B, L, R, **f32), torch.empty(B, L, R, **f32)
         dh_out, gs_out = None, L
-        bwd_mode = getattr(self, "bwd_mode", None) or self.block_mode      # "tc" / "ffma" / "auto"; defaults to block_mode
-        use_tc_bwd = bwd_mode != "ffma" and bool(lib.wn_tc_bwd_supported(R, D, S, k))
+        use_tc_bwd = self.block_mode != "ffma" and bool(lib.wn_tc_bwd_supported(R, D, S, k))
         self.last_bwd_mode = "tc" if use_tc_bwd else "ffma"
         a = native.BlockBwdArgs()
         a.B, a.L, a.R, a.D, a.S, a.k, a.ds_start = B, L, R, D, S, k, ds_start
@@ -953,53 +932,30 @@ class _Runtime:
             a.dilation, a.in_start, a.out_start = d, in_s, out_s
             a.gs_out, a.gz, a.gs_in = gs_out, gz, gs_in
             if use_tc_bwd:
-                if self.tc_precision == "bf16x2":
-                    wdz, wdh = W["tc_bwd_layers_bf16"][i]
-                    native.check(lib.wn_tc_block_bwd_data_prec(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), 2, stream),
-                                 f"tc block bwd {i}")
-                else:
-                    wdz, wdh = W["tc_bwd_layers"][i]
-                    native.check(lib.wn_tc_block_bwd_data(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), stream), f"tc block bwd {i}")
+                wdz, wdh = W["tc_bwd_layers"][i]
+                native.check(lib.wn_tc_block_bwd_data(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), stream), f"tc block bwd {i}")
             else:
                 wrs_rows, wfg_bwd = self.ffma_bwd_weights(i)
                 a.d_wrs_rows, a.d_wfg_bwd = wrs_rows.data_ptr(), wfg_bwd.data_ptr()
                 native.check(lib.wn_block_bwd_data(ctypes.byref(a), stream), f"block bwd {i}")
             # weight gradients: plain GEMMs over (frames x channels) slices
             h_in = h_all[i]
-            if native_wgrad:
-                gws = torch.empty(S, D, 1, **f32)
-                wgrad(gws, dskip, 0, S, OL * S, zbuf, ds_start * D, D, L * D, OL, S, D)
-                grads[f"skip_convs.{i}.weight"] = gws
-                if dh_out is not None and id_start < L:
-                    gwr = torch.empty(R, D, 1, **f32)
-                    wgrad(gwr, dh_out, id_start * R, R, L * R, zbuf, id_start * D, D, L * D, L - id_start, R, D)
-                    grads[f"residual_convs.{i}.weight"] = gwr
-                else:
-                    grads[f"residual_convs.{i}.weight"] = torch.zeros_like(wr)
-                gfg = torch.empty(2 * D, R, k, **f32)          # filter rows then gate rows, like the packed dfg columns
-                for j in range(k):
-                    sh = (k - 1 - j) * d
-                    lo = min(L, max(gz, in_s + sh))           # frames whose tap j lands on real (non-padded) input
-                    wgrad(gfg, dfg, lo * 2 * D, 2 * D, L * 2 * D, h_in, (lo - sh) * R, R, L * R, L - lo, 2 * D, R,
-                          n_stride=R * k, c_stride=k, out_off=j)
-                gwf, gwg = gfg[:D], gfg[D:]
+            gws = torch.empty(S, D, 1, **f32)
+            wgrad(gws, dskip, 0, S, OL * S, zbuf, ds_start * D, D, L * D, OL, S, D)
+            grads[f"skip_convs.{i}.weight"] = gws
+            if dh_out is not None and id_start < L:
+                gwr = torch.empty(R, D, 1, **f32)
+                wgrad(gwr, dh_out, id_start * R, R, L * R, zbuf, id_start * D, D, L * D, L - id_start, R, D)
+                grads[f"residual_convs.{i}.weight"] = gwr
             else:
-                zs = zbuf[:, ds_start:, :]
-                grads[f"skip_convs.{i}.weight"] = torch.einsum("bts,btc->sc", dskip, zs).unsqueeze(-1)
-                if dh_out is not None and id_start < L:
-                    grads[f"residual_convs.{i}.weight"] = torch.einsum("btr,btc->rc", dh_out[:, id_start:, :],
-                                                                       zbuf[:, id_start:, :]).unsqueeze(-1)
-                else:
-                    grads[f"residual_convs.{i}.weight"] = torch.zeros_like(wr)
-                gwf, gwg = torch.empty_like(wf), torch.empty_like(wg)
-                for j in range(k):
-                    sh = (k - 1 - j) * d
-                    lo = max(gz, in_s + sh)
-                    if lo < L:
-                        g2 = torch.einsum("btn,btr->nr", dfg[:, lo:, :], h_in[:, lo - sh:L - sh, :])
-                    else:
-                        g2 = torch.zeros(2 * D, R, **f32)
-                    gwf[:, :, j], gwg[:, :, j] = g2[:D], g2[D:]
+                grads[f"residual_convs.{i}.weight"] = torch.zeros_like(wr)
+            gfg = torch.empty(2 * D, R, k, **f32)          # filter rows then gate rows, like the packed dfg columns
+            for j in range(k):
+                sh = (k - 1 - j) * d
+                lo = min(L, max(gz, in_s + sh))           # frames whose tap j lands on real (non-padded) input
+                wgrad(gfg, dfg, lo * 2 * D, 2 * D, L * 2 * D, h_in, (lo - sh) * R, R, L * R, L - lo, 2 * D, R,
+                      n_stride=R * k, c_stride=k, out_off=j)
+            gwf, gwg = gfg[:D], gfg[D:]
             if bs is not None:
                 grads[f"skip_convs.{i}.bias"] = dskip.sum((0, 1))
             if br is not None:

@@ -19,7 +19,6 @@ rounding of the kernels is modelled:
     "exact"   the float64 value of each operand
     "pairs"   hi*hi + lo*hi + hi*lo over bf16 (hi, lo) splits (stored pair planes are used as they are)
     "bf16"    hi*hi only: the hi plane of a stored pair, bf16(x) of an fp32 operand
-    "tf32x3"  hi*hi + lo*hi + hi*lo over rna-tf32 splits
 An activation operand is either a float tensor (its fp32 value is split) or a tuple (hi, lo) of stored bf16 planes.  Outside
 "exact", every output is also rounded the way the kernel stores it: ``pair_out`` -> a bf16 (hi, lo) pair of the fp32 value
 (about 16 significant bits), otherwise fp32.
@@ -27,7 +26,7 @@ An activation operand is either a float tensor (its fp32 value is split) or a tu
 Layout converters between frames (B, L, C) and the kernels' chunked layouts are at the end."""
 import torch
 
-MODES = ("exact", "pairs", "bf16", "tf32x3")
+MODES = ("exact", "pairs", "bf16")
 
 
 # ---------------------------------------------------------------------------------------------------- operand splits
@@ -58,8 +57,7 @@ def _parts(x, mode):
         raise ValueError(f"stored bf16 pairs have no {mode} form")
     if mode == "exact":
         return x.double(), None
-    split = split_tf32 if mode == "tf32x3" else split_bf16
-    hi, lo = split(x)
+    hi, lo = split_bf16(x)
     return hi.double(), (None if mode == "bf16" else lo.double())
 
 

@@ -39,8 +39,8 @@ def classify_stream(got_idx, ref_idx, ref_margins, tol=1e-4):
 
 
 def separate_head_relu_ties(params, spec, x, out_len, margin=2e-5, step=None):
-    """Gradients are discontinuous where a head ReLU input is exactly zero: an fp32-class difference (3xTF32 tensor
-    cores vs FFMA, or just another summation order) that flips the sign of a pre-activation of size 1e-7 switches one
+    """Gradients are discontinuous where a head ReLU input is exactly zero: an fp32-class difference (tensor cores
+    vs FFMA, or just another summation order) that flips the sign of a pre-activation of size 1e-7 switches one
     mask element and moves a weight gradient by percent.  The analogue of the argmax near-tie rule for the backward
     tests: nudge the last skip bias and the end_conv_1 bias (per channel, in float64 on the oracle) until no head ReLU
     input of this test case lies within `margin` of zero.  Returns a new fp32 parameter dict."""
@@ -90,14 +90,13 @@ def kernel_rel(a, b):
 def tc_acc(K):
     """Allowance for the fp32 accumulation of a K-long contraction on the tensor cores, which the float64 emulation does not
     model: measured on an H100 it reaches ~1e-5 (max-relative) at K = 512 and grows with K, also where the operand error
-    is tiny (3xTF32: e_emu ~ 1e-7), while spread over all frames and channels rather than on a range boundary.
+    is tiny, while spread over all frames and channels rather than on a range boundary.
 
     What the bar then still catches, per output tensor (~4e-5 to 7e-5 for the K of these tests): any frame-range, tap,
     tile, plane or bias error (the controls miss by 10^3 or more); for bf16 pairs, a dropped lo-plane product of either
     operand (the operand-term controls of test_two_launch_and_ffma_block_fwd); single-pass bf16 against its own emulation
     at 0.25 e_emu.  What it cannot catch: an error below about 2^-16 of the output scale -- one missing lo-plane product on
-    a single k-slab, or for 3xTF32 a dropped tf32 lo plane altogether (~2^-12 per operand); the 50-layer model tests of
-    test_gpu_tc.py carry that case."""
+    a single k-slab."""
     return 2.0 ** -16 * (max(K, 256) / 256) ** 0.5
 
 
@@ -109,13 +108,11 @@ def worst_element(got, exact):
 
 
 def kernel_check(what, got, exact, emu=None, kind="emu", K=256):
-    """Assert the bar of `kind` ("emu": operand-split kernels, "bf16": single pass, "ffma", "tf32x1"); returns the bar.
+    """Assert the bar of `kind` ("emu": operand-split kernels, "bf16": single pass, "ffma"); returns the bar.
     K: the longest contraction feeding the output (sets the accumulation allowance of the tensor-core kernels)."""
     e = kernel_rel(got, exact)
     if kind == "ffma":
         bar, msg = 1e-5, ""
-    elif kind == "tf32x1":
-        bar, msg = 2e-2, ""
     else:
         e_emu = kernel_rel(emu, exact)
         bar, msg = 2 * e_emu + tc_acc(K), f" e_emu {e_emu:.2e}"

@@ -8,7 +8,7 @@ are filled with a sentinel (NaN) first: frames outside a kernel's write range mu
 Bars follow from the operand widths (block_ref's emulation of exactly these inputs):
     rel_err(kernel, exact) <= 2 e_emu + acc(K),     e_emu = rel_err(emulated, exact)
     single-pass bf16 also   rel_err(kernel, emulated) <= 0.25 e_emu   (a wrong operand plane or a dropped term fails this)
-    FFMA kernels            rel_err(kernel, exact) <= 1e-5;   single TF32 pass: <= 2e-2 (hardware truncation not emulated)
+    FFMA kernels            rel_err(kernel, exact) <= 1e-5
 acc(K) = 2^-16 sqrt(K / 256) allows for the tensor cores' fp32 accumulation over a contraction of length K, which the
 emulation (float64 sums) leaves out; see helpers.tc_acc.
 rel_err is max|a - b| / max|b| per output tensor (per tap for weight gradients).  Every measured value is printed (-s)."""
@@ -263,7 +263,7 @@ TC_BWD_CASES = [  # B, L, dilation, in_start, out_start, gs_out (= L: no dh_out)
 ]
 
 
-@pytest.mark.parametrize("impl", ["tf32x3", "pairs", "ffma"])
+@pytest.mark.parametrize("impl", ["pairs", "ffma"])
 @pytest.mark.parametrize("case", range(len(TC_FWD_CASES)))
 @pytest.mark.parametrize("shape", TC_SHAPES)
 def test_two_launch_and_ffma_block_fwd(shape, case, impl):
@@ -285,8 +285,7 @@ def test_two_launch_and_ffma_block_fwd(shape, case, impl):
         a.d_wfg_t, a.d_bfg, a.d_wrs_t, a.d_brs, a.mode = wfg.data_ptr(), bfg.data_ptr(), wrs.data_ptr(), brs.data_ptr(), 0
     else:
         a = native.TcBlockArgs()
-        a.fast_tf32 = 0 if impl == "tf32x3" else 2
-        wa, ba, wb, bb = packs["tc_layers" if impl == "tf32x3" else "tc_layers_bf16"][1]
+        wa, ba, wb, bb = packs["tc_layers"][1]
         a.d_wa, a.d_ba, a.d_wb, a.d_bb, a.d_z = wa.data_ptr(), ba.data_ptr(), wb.data_ptr(), bb.data_ptr(), z.data_ptr()
     a.d_h_in, a.d_h_out, a.d_skip, a.d_fg_save = h_in.data_ptr(), h_out.data_ptr(), skip.data_ptr(), fg.data_ptr()
     a.B, a.L, a.R, a.D, a.S, a.k = B, L, R, D, S, k
@@ -313,52 +312,21 @@ def test_two_launch_and_ffma_block_fwd(shape, case, impl):
     if impl == "pairs" and case == 0 and shape == TC_SHAPES[0]:
         _miss("dilation + 1", h_out.cpu()[:, out_s:], BR.block_forward(h, W, d + 1, in_s, out_s, sk_s, skip0)["h_out"], bar)
         _miss("in_start + 1", h_out.cpu()[:, out_s:], BR.block_forward(h, W, d, in_s + 1, out_s, sk_s, skip0)["h_out"], bar)
-    if impl != "ffma" and case == 0 and shape == TC_SHAPES[0]:
+    if impl == "pairs" and case == 0 and shape == TC_SHAPES[0]:
         # operand-term controls: the same products with the weights' lo plane dropped (hi*hi + lo*hi only), and with
-        # the activations' lo plane dropped (hi*hi + hi*lo only).  bf16 pairs: the bar catches both (measured on an H100:
-        # 10.8x and 7.5x the bar).  3xTF32: a dropped tf32 lo plane costs ~2^-12 per operand, ~4e-5 at the output, the
-        # size of the tensor cores' accumulation error, so the kernel-level bar cannot see it; only reported here.  That
-        # case is caught at model level: test_gpu_tc.py::test_tc_full_size_batch_independence holds 3xTF32 within 2e-5 of
-        # the FFMA blocks through 50 layers, where one pass of TF32 operands is ~1e-3 (test_fast_tf32_mode_is_opt_in_and_close).
-        split = BR.split_tf32 if impl == "tf32x3" else BR.split_bf16
-        W_hi = {n: split(v)[0] if n[0] == "w" else v for n, v in W.items()}
+        # the activations' lo plane dropped (hi*hi + hi*lo only).  The bar catches both (measured on an H100: 10.8x and
+        # 7.5x the bar).
+        W_hi = {n: BR.split_bf16(v)[0] if n[0] == "w" else v for n, v in W.items()}
         got_h = h_out.cpu()[:, out_s:]
-        h_hi = split(h)[0]
+        h_hi = BR.split_bf16(h)[0]
         wrongs = {"weights' lo plane dropped": BR.block_forward(h, W_hi, d, in_s, out_s, sk_s, skip0, mode=impl)["h_out"],
                   "activations' lo plane dropped": (BR.block_forward(h_hi, W, d, in_s, out_s, sk_s, skip0, mode=impl)["h_out"]
                                                     + (h - h_hi)[:, out_s:].double())}
         for what, wrong in wrongs.items():
-            if impl == "pairs":
-                _miss(what, got_h, wrong, bar, factor=5)
-            else:
-                print(f"  {what} (3xTF32, not asserted): rel_err {_rel(got_h, wrong):.2e} = {_rel(got_h, wrong) / bar:.1f}x bar")
+            _miss(what, got_h, wrong, bar, factor=5)
 
 
-def test_two_launch_single_tf32_pass_is_close():
-    """precision mode 1 (one TF32 pass, opt-in): only a loose bar, the hardware's operand truncation is not emulated"""
-    import native
-    lib = native.lib()
-    R, D, S, k = 256, 256, 256, 2
-    B, L, d, in_s, out_s, sk_s, _ = TC_FWD_CASES[0]
-    m = _model(R, D, S, k)
-    W = _weights(m, 1)
-    wa, ba, wb, bb = m._runtime().packed_weights(_stream())["tc_layers"][1]
-    h = torch.randn(B, L, R, generator=_gen(600))
-    h_in, h_out, z, skip = h.cuda(), _nan(B, L, R), _nan(B, L, D), _nan(B, L - sk_s, S)
-    a = native.TcBlockArgs()
-    a.d_h_in, a.d_h_out, a.d_skip, a.d_z, a.d_fg_save = h_in.data_ptr(), h_out.data_ptr(), skip.data_ptr(), z.data_ptr(), None
-    a.d_wa, a.d_ba, a.d_wb, a.d_bb, a.fast_tf32 = wa.data_ptr(), ba.data_ptr(), wb.data_ptr(), bb.data_ptr(), 1
-    a.B, a.L, a.R, a.D, a.S, a.k = B, L, R, D, S, k
-    a.dilation, a.in_start, a.out_start, a.skip_start, a.skip_init = d, in_s, out_s, sk_s, 1
-    native.check(lib.wn_tc_block_fwd(ctypes.byref(a), _stream()), "tf32x1 block fwd")
-    torch.cuda.synchronize()
-    ex = BR.block_forward(h, W, d, in_s, out_s, sk_s)
-    print("\nwn_tc_block_fwd tf32x1")
-    _check("h_out", h_out.cpu()[:, out_s:], ex["h_out"], kind="tf32x1")
-    _check("skip", skip.cpu(), ex["skip"], kind="tf32x1")
-
-
-@pytest.mark.parametrize("impl", ["tf32x3", "pairs", "ffma"])
+@pytest.mark.parametrize("impl", ["pairs", "ffma"])
 @pytest.mark.parametrize("case", range(len(TC_BWD_CASES)))
 @pytest.mark.parametrize("shape", [s for s in TC_SHAPES if s[1] % 256 == 0])
 def test_two_launch_and_ffma_block_bwd_data(shape, case, impl):
@@ -385,9 +353,8 @@ def test_two_launch_and_ffma_block_bwd_data(shape, case, impl):
         native.check(lib.wn_block_bwd_data(ctypes.byref(a), _stream()), "ffma block bwd")
     else:
         packs = m._runtime().packed_weights(_stream())
-        wdz, wdh = packs["tc_bwd_layers" if impl == "tf32x3" else "tc_bwd_layers_bf16"][1]
-        native.check(lib.wn_tc_block_bwd_data_prec(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), 0 if impl == "tf32x3" else 2,
-                                                   _stream()), f"{impl} block bwd")
+        wdz, wdh = packs["tc_bwd_layers"][1]
+        native.check(lib.wn_tc_block_bwd_data(ctypes.byref(a), wdz.data_ptr(), wdh.data_ptr(), _stream()), f"{impl} block bwd")
     torch.cuda.synchronize()
     for n, t, lo in (("dFG", dfg, gz), ("z", z, gz), ("dh_in", dh_in, gs_in)):
         _sentinel_kept(n, t, lo)
@@ -395,7 +362,7 @@ def test_two_launch_and_ffma_block_bwd_data(shape, case, impl):
     ex = BR.block_backward_data(*args)
     em = None if impl == "ffma" else BR.block_backward_data(*args, mode=impl)
     kind = "ffma" if impl == "ffma" else "emu"
-    print(f"\n{'wn_block_bwd_data' if impl == 'ffma' else 'wn_tc_block_bwd_data_prec ' + impl} R={R} D={D} S={S} k={k}: "
+    print(f"\n{'wn_block_bwd_data' if impl == 'ffma' else 'wn_tc_block_bwd_data ' + impl} R={R} D={D} S={S} k={k}: "
           f"B={B} L={L} d={d} in={in_s} out={out_s} gs_out={gs_out} ds={ds_s} gz={gz} gs_in={gs_in}")
     got = dict(dfg=dfg.cpu()[:, gz:], z=z.cpu()[:, gz:], dh_in=dh_in.cpu()[:, gs_in:])
     for n in ("dfg", "z", "dh_in"):

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     lib = native.lib()
     for name in declared:
         assert getattr(lib, name) is not None
-    assert lib.wn_version() == 2
+    assert lib.wn_version() == 3
     assert lib.wn_n1p(256) == 512 and lib.wn_n1p(16) == 128 and lib.wn_n2p(32 + 1024) == 1152
     # argument errors are reported through the return code + message, never by crashing
     assert lib.wn_block_fwd(None, None) == -1
@@ -157,8 +157,7 @@ def test_shape_predicates_and_workspace_sizes_are_host_side():
     assert lib.wn_wgrad(ctypes.byref(a), None) < 0 and b"bad sizes" in lib.wn_last_error_string()
     a.N, a.C = 512, 128
     assert lib.wn_tc_wgrad(ctypes.byref(a), None) < 0 and b"C == 256" in lib.wn_last_error_string()
-    assert lib.wn_tc_block_bwd_data_prec(None, None, None, 0, None) < 0
-    assert lib.wn_tc_convert_weights_bf16(None, None, 0, None) < 0
+    assert lib.wn_tc_block_bwd_data(None, None, None, None) < 0
 
 
 def test_sampler_workspace_and_argument_errors_are_host_side():

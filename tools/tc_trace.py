@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """Per-stage timeline of the tensor-core block kernel (CTA 0, first 512 stages of the last traced launch).
-TC_PREC=tf32x3|bf16x2 selects the operand split, WN_TC_TRACE_PASS=A keeps the conv+gate launch of the last layer
-instead of its 1x1 launch."""
+WN_TC_TRACE_PASS=A keeps the conv+gate launch of the last layer instead of its 1x1 launch."""
 import ctypes, os, sys
 os.environ["WN_TC_TRACE"] = "1"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -9,8 +8,6 @@ for p in (ROOT, os.path.join(ROOT, "pytorch-wavenet_b200")):
     sys.path.insert(0, p)
 import numpy as np, torch, bench, native
 model = bench.build_model(bench.GEN_KW).cuda()
-rt = model._runtime()
-rt.tc_precision = os.environ.get("TC_PREC", rt.tc_precision)
 pass_a = os.environ.get("WN_TC_TRACE_PASS", "B")[0] == "A"
 slabs = 32 if pass_a else 16                                       # K slabs per output tile (k*R/16 or D/16 at 256 channels)
 idx = torch.randint(0, 256, (8, 16000), generator=torch.Generator().manual_seed(1)).to(torch.uint8).cuda()
@@ -31,7 +28,7 @@ tma_to_full = t[:, 5] - t[:, 1]
 split_to_mma = t[:, 3] - t[:, 6]
 period = np.diff(t[:, 4])
 pos = (np.arange(lo, hi)[1:]) % slabs
-print(f"precision {rt.tc_precision}, pass {'A (conv+gate)' if pass_a else 'B (1x1)'}: {slabs} slabs per tile")
+print(f"pass {'A (conv+gate)' if pass_a else 'B (1x1)'}: {slabs} slabs per tile")
 print(f"stage period (MMA issue to MMA issue)     mean {period.mean():7.0f}  median {np.median(period):7.0f}")
 print(f"  ... first slab of a tile (incl. waiting for a free accumulator)  mean {period[pos == 0].mean():7.0f}")
 print(f"  ... other slabs                                                   mean {period[pos != 0].mean():7.0f}")
