@@ -546,6 +546,41 @@ typedef struct wn_gen_stream_params {
  * otherwise), and d_uniforms is required when any stream has temperature > 0.  The library keeps a device copy of the
  * records (allocated at the first call, freed by wn_gen_destroy) and uploads it in stream order before the next launch. */
 int wn_gen_set_stream_params(wn_gen_handle* h, const wn_gen_stream_params* params);
+/* Stream positions (continuous batching): one record per stream, {origin, sample0, first0}; params is a HOST array
+ * [n_streams], copied before the call returns; NULL clears them (wn_gen_create starts cleared, which is origin = sample0 =
+ * first0 = 0 for every stream: the schedule above exactly).  Positions need per-stream records (WN_E_STATE otherwise);
+ * WN_E_BADARG for sample0 < 0 or first0 < 0.  The handle's time t still drives the rings, the exchange and the head; with
+ * positions set, per stream s:
+ *   - evaluation t is position q = t - origin of the stream;
+ *   - its input is d_first[s*pitch + q - first0] for q < n_given[s] (pitch = a->n_given: a row may hold just the prompt
+ *     positions the launch reads), else d_forced[s*n_samples + (q - n_given[s]) - sample0] when teacher forcing, else the
+ *     stream's own last choice;
+ *   - at q >= n_given[s] - 1 it selects sample i = q - (n_given[s] - 1) into column i - sample0 of d_out_idx, d_out_logits
+ *     and d_uniforms;
+ *   - the head runs from head_from = min_s (origin + n_given[s] - 1).
+ * wn_gen_run returns WN_E_BADARG, before launching, for origin > t0, a prompt read outside [0, pitch), a forced read or a
+ * selection column outside [0, n_samples), and a first evaluation of a newly seated stream that reads no prompt sample.
+ * A stream whose origin differs from the one it last ran with (after wn_gen_reset: 0; after wn_gen_set_time: none) must have
+ * been seated at every layer at the current t for that origin (WN_E_STATE otherwise).  With positions set one stream runs
+ * kernel 2 (or 4) where auto would pick kernel 3, which reads no records; mode 3 returns WN_E_UNSUPP. */
+typedef struct wn_gen_stream_pos {
+    int origin, sample0, first0;
+} wn_gen_stream_pos;
+int wn_gen_set_stream_positions(wn_gen_handle* h, const wn_gen_stream_pos* pos);
+/* Seat new jobs in the listed streams ("slots") of a running handle at its current time t, one layer per call: the slot's
+ * ring of layer l is written for every time of [t - ring_len_l, t), as the kernel wn_gen_run would launch now keeps it
+ * ({value, tag = time + 1} pairs, plain floats for kernel 1).  With q_end[j] the position of slot slots[j] at t (its
+ * origin is t - q_end[j]: 0 for a job that starts at its first prompt sample, T for one primed through position T - 1), the
+ * value at a time of position q is 0 for q < 0 or when d_src is NULL, else frame frame_of_end - (q_end[j] - q) of sequence j
+ * of d_src (B = n, L frames, in either WN_GEN_SRC_* layout, as for wn_gen_prefill_layer).  Every slot time a new position
+ * reads is written: a reused slot's previous job wrote the same times with the same tags, so no tag could tell them apart.
+ * No other stream is touched.  Works at any t, between launches.  WN_E_BADARG for a bad or repeated slot, q_end < 0, a
+ * source frame below 0, or source positions that would lie at times < 0 (every kernel reads those as zero history).
+ * wn_gen_set_time(h, t), right after wn_gen_reset only, moves the handle to t without evaluating, so that a primed job's
+ * history lies at times >= 0 (t >= the longest ring); every stream must then be seated before the next wn_gen_run. */
+int wn_gen_seat_layer(wn_gen_handle* h, int layer, int n, const int* slots, const int* q_end, const void* d_src, int layout,
+                      int L, int frame_of_end, void* stream);
+int wn_gen_set_time(wn_gen_handle* h, int t);
 /* Synchronise the stream and report whether a launch aborted (a CTA waited > ~3 s for a tag): 0 = fine. */
 int wn_gen_check(wn_gen_handle* h, void* stream);
 /* Debug aid: with WN_GEN_TRACE=1 in the environment at wn_gen_create, CTA 0 stamps clock64() at 8 points of every layer

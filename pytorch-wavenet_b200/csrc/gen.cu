@@ -19,6 +19,7 @@
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -37,9 +38,12 @@ struct GenLayer {
 };
 
 // One stream's sampling settings: the library's device copy of a wn_gen_stream_params record; trunc = 1 when the truncation
-// rule applies to the stream (temperature > 0 and a bound that drops classes).
+// rule applies to the stream (temperature > 0 and a bound that drops classes).  origin / sample0 / first0: its
+// wn_gen_stream_pos record (all 0 without positions): evaluation t is position t - origin of the stream, its prompt row
+// starts at position first0 and its output / uniform / forced columns at sample sample0.
 struct GenStream {
     int n_given, top_k, trunc;
+    int origin, sample0, first0;
     float temperature, regularize;
     double top_p;
 };
@@ -98,24 +102,35 @@ __device__ __forceinline__ GenStream stream_set(const GenParams& p, int s) {
     if (has_records<PS>(p)) return p.ps[s];
     GenStream g;
     g.n_given = p.n_given; g.top_k = p.top_k; g.trunc = p.trunc;
+    g.origin = g.sample0 = g.first0 = 0;
     g.temperature = p.temperature; g.regularize = p.regularize; g.top_p = p.top_p;
     return g;
 }
 
-// The given input of evaluation t of stream s: its prompt sample (first has pitch p.n_given), else its forced sample when
-// teacher forcing.  false: the stream feeds back its own last choice.
+// The given input of evaluation t of stream s at its position q = t - origin: its prompt sample (first has pitch
+// p.n_given; the row starts at position first0), else its forced sample when teacher forcing (the row starts at sample
+// sample0).  false: the stream feeds back its own last choice.
 template <int PS = PS_ANY>
 __device__ __forceinline__ bool given_input(const GenParams& p, int s, int t, int& v) {
-    const int ng = has_records<PS>(p) ? p.ps[s].n_given : p.n_given;
-    if (t < ng) { v = p.first[(size_t)s * p.n_given + t]; return true; }
-    if (p.forced != nullptr) { v = p.forced[(size_t)s * p.n_samples + (t - ng)]; return true; }
+    int ng = p.n_given, q = t, f0 = 0, s0 = 0;
+    if (has_records<PS>(p)) {
+        const GenStream& g = p.ps[s];
+        ng = g.n_given; q = t - g.origin; f0 = g.first0; s0 = g.sample0;
+    }
+    if (q < ng) { v = p.first[(size_t)s * p.n_given + (q - f0)]; return true; }
+    if (p.forced != nullptr) { v = p.forced[(size_t)s * p.n_samples + (q - ng - s0)]; return true; }
     return false;
 }
 
-// The sample stream s chooses at evaluation t (negative while t is still inside its prompt: no selection then).
+// The output / uniform column of the sample stream s chooses at evaluation t: sample q - (n_given - 1) minus sample0
+// (negative while the stream is still inside its prompt: no selection then; wn_gen_run keeps it so).
 template <int PS = PS_ANY>
 __device__ __forceinline__ int sample_of(const GenParams& p, int s, int t) {
-    return t - ((has_records<PS>(p) ? p.ps[s].n_given : p.n_given) - 1);
+    if (has_records<PS>(p)) {
+        const GenStream& g = p.ps[s];
+        return t - g.origin - (g.n_given - 1) - g.sample0;
+    }
+    return t - (p.n_given - 1);
 }
 
 // This evaluation's condition table: the window row of t's frame under local conditioning (once per evaluation).
@@ -561,7 +576,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
         float* pw = prob + warp * C;
         for (int s = warp; s < NS; s += GEN_WARPS) {
             const GenStream ss = stream_set(p, s);
-            const int samp = t - (ss.n_given - 1);         // sample number this evaluation chooses
+            const int samp = sample_of(p, s, t);           // output column of the sample this evaluation chooses
             if (samp < 0) continue;                        // still inside its prompt
             // the logits (written by other CTAs: through the L2) into the warp's scratch
             const float* lg = p.logitbuf + (size_t)s * C;
@@ -967,7 +982,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         double* cw = cdf + warp * C;
         for (int s = warp; s < NS; s += GEN_WARPS) {
             const GenStream ss = stream_set(p, s);
-            const int samp = t - (ss.n_given - 1);
+            const int samp = sample_of(p, s, t);
             if (samp < 0) continue;                        // still inside its prompt
             const float* lg = regA + (size_t)s * C;
             int choice;
@@ -1852,7 +1867,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
         WORKER_SYNC();
         if (warp == 0) {
             const GenStream ss = stream_set(p, stream);
-            const int samp = t - (ss.n_given - 1);
+            const int samp = sample_of(p, stream, t);
             if (samp >= 0) {                                     // no selection while the stream is inside its prompt
                 const int choice = ss.trunc ? choose_truncated(logit_s, reinterpret_cast<unsigned*>(cdf),
                                                                reinterpret_cast<float*>(cdf) + C, C, lane, ss.temperature,
@@ -2477,7 +2492,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         // every CTA holds all logits of its 8 streams: warp = stream draws the next index (all CTAs agree)
         if (hs_g < NS) {
             const GenStream ss = stream_set<PS ? PS_ON : PS_OFF>(p, hs_g);
-            const int samp = t - (ss.n_given - 1);
+            const int samp = sample_of<PS ? PS_ON : PS_OFF>(p, hs_g, t);
             if (samp >= 0) {                              // no selection while the stream is inside its prompt
                 float* lg = logit_s + warp * W;
                 const float* xl = reinterpret_cast<const float*>(Xl);
@@ -2503,27 +2518,39 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     cluster_sync_all();                                  // peers may still be storing into this CTA's shared memory
 }
 
-// ------------------------------------------------------------------------------------------------ ring prefill
+// ------------------------------------------------------------------------------------------------ ring prefill / seating
 // One layer's input at times [t_lo, t_end), computed by a forward pass, into the ring slots t % ring_len: frame
-// f_end - (t_end - t) of stream s in src, fp32 frames (B, L, R) or chunked bf16 pairs (B, 2, R/8, L, 8) (value hi + lo).
+// f_end - (t_end - t) of sequence j of src, fp32 frames (B, L, R) or chunked bf16 pairs (B, 2, R/8, L, 8) (value hi + lo).
 // plain: kernel 1's ring of floats; otherwise the {value, tag = t + 1} pairs the flag-exchange kernels poll for.
+// seats.n == 0 (wn_gen_prefill_layer): sequence j is stream j, for every stream.  seats.n > 0 (wn_gen_seat_layer): sequence
+// j is stream seats.slot[j], whose position at t_end is seats.q_end[j]; times of negative positions, and every time when
+// src is null, get 0 (times t < 0 go to slot t mod ring_len, the slot kernel 1 reads for them).
+constexpr int GEN_SEAT_MAX = 128;
+struct GenSeatList { int n; int slot[GEN_SEAT_MAX]; int q_end[GEN_SEAT_MAX]; };
+
 __global__ void gen_prefill_kernel(const void* __restrict__ src, int pairs, int L, int f_end, int t_lo, int t_end, int NS,
-                                   int R, int ring_len, float* __restrict__ rings, long long ring_off, int plain) {
-    const long long n = (long long)(t_end - t_lo) * NS * R;
+                                   int R, int ring_len, float* __restrict__ rings, long long ring_off, int plain,
+                                   const GenSeatList seats) {
+    const int rows = seats.n ? seats.n : NS;
+    const long long n = (long long)(t_end - t_lo) * rows * R;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int r = (int)(i % R);
         const long long q = i / R;
-        const int s = (int)(q % NS), t = t_lo + (int)(q / NS);
+        const int j = (int)(q % rows), t = t_lo + (int)(q / rows);
+        const int s = seats.n ? seats.slot[j] : j;
+        const bool live = src != nullptr && (seats.n == 0 || seats.q_end[j] - (t_end - t) >= 0);
         const long long f = f_end - (t_end - t);
-        float v;
-        if (pairs) {
+        float v = 0.f;
+        if (live && pairs) {
             const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(src);
-            const size_t hi = ((((size_t)s * 2) * (R / 8) + r / 8) * L + f) * 8 + (r & 7);
+            const size_t hi = ((((size_t)j * 2) * (R / 8) + r / 8) * L + f) * 8 + (r & 7);
             v = __bfloat162float(b[hi]) + __bfloat162float(b[hi + (size_t)(R / 8) * L * 8]);
-        } else {
-            v = reinterpret_cast<const float*>(src)[((size_t)s * L + f) * R + r];
+        } else if (live) {
+            v = reinterpret_cast<const float*>(src)[((size_t)j * L + f) * R + r];
         }
-        const size_t e = ((size_t)(t % ring_len) * NS + s) * R + r;
+        int slot = t % ring_len;
+        if (slot < 0) slot += ring_len;
+        const size_t e = ((size_t)slot * NS + s) * R + r;
         if (plain) rings[ring_off + e] = v;                          // ring_off counts elements of either kind
         else reinterpret_cast<uint2*>(rings)[ring_off + e] = make_uint2(__float_as_uint(v), (unsigned)t + 1u);
     }
@@ -2613,6 +2640,13 @@ struct wn_gen_handle {
     // the fill wrote (-1: none; 1: plain floats of kernel 1, 0: {value, tag} pairs of every other kernel)
     std::vector<int> pf_t_end;
     int pf_plain;
+    // wn_gen_set_stream_positions: one record per stream (empty: cleared).  run_origin: each stream's origin at the last
+    // wn_gen_run (0 after wn_gen_reset, INT_MIN after wn_gen_set_time: every stream must then be seated); seat_t /
+    // seat_origin [layer * n_streams + stream]: the t a stream's ring was last seated at (wn_gen_seat_layer) and the origin
+    // that seat implied; seat_plain: the ring layout the seats wrote (as pf_plain)
+    std::vector<wn_gen_stream_pos> pos;
+    std::vector<int> run_origin, seat_t, seat_origin;
+    int seat_plain;
 };
 
 static int validate_shape(const wn_gen_shape* s) {
@@ -2675,7 +2709,8 @@ static int pick_kernel(const wn_gen_handle* h) {
         if (h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok)) return 4;
         // kernel 3 only where kernel 2 or 4 fits too: a net too deep for kernel 2's shared memory (on an H100 from ~2 240
         // layers of 256 channels with 512 end channels and classes) keeps kernel 1, which auto has always run there
-        if (h->fast_ok && (h->ll_ok || h->cluster_ok)) return 3;
+        // kernel 3 reads no per-stream records: with positions set one stream runs kernel 2 (same sums) or 4
+        if (h->fast_ok && (h->ll_ok || h->cluster_ok)) return h->pos.empty() ? 3 : (h->ll_ok ? 2 : 4);
     }
     if (m != 1 && h->ll_ok) return 2;                       // modes 0 and 2
     return h->generic_ok ? 1 : 0;
@@ -2914,6 +2949,10 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     h->cur_t = 0;
     h->pf_t_end.assign(s->n_layers, -1);
     h->pf_plain = -1;
+    h->run_origin.assign(NS, 0);
+    h->seat_t.assign((size_t)s->n_layers * NS, -1);
+    h->seat_origin.assign((size_t)s->n_layers * NS, 0);
+    h->seat_plain = -1;
     *out = h;
     return 0;
 }
@@ -2939,6 +2978,9 @@ extern "C" int wn_gen_reset(wn_gen_handle* h, void* stream) {
     h->cur_t = 0;
     h->pf_t_end.assign(h->shape.n_layers, -1);
     h->pf_plain = -1;
+    h->run_origin.assign(h->shape.n_streams, 0);
+    h->seat_t.assign(h->seat_t.size(), -1);
+    h->seat_plain = -1;
     return 0;
 }
 
@@ -2969,8 +3011,10 @@ extern "C" int wn_gen_prefill_layer(wn_gen_handle* h, int layer, const void* d_s
                "wn_gen_prefill_layer: the sampler kernel changed between layers (ring layout differs)");
     const long long n = (long long)n_t * NS * R;
     const int grid = (int)std::min<long long>((n + 255) / 256, 4LL * h->sm_count);
+    GenSeatList all;
+    all.n = 0;
     gen_prefill_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(d_src, layout == WN_GEN_SRC_PAIRS, L, frame_of_t_end, t_end - n_t,
-                                                               t_end, NS, R, Lr.ring_len, h->base.rings, Lr.ring_off, plain);
+                                                               t_end, NS, R, Lr.ring_len, h->base.rings, Lr.ring_off, plain, all);
     WN_CUDA(cudaGetLastError());
     h->pf_plain = plain;
     h->pf_t_end[layer] = t_end;
@@ -2985,6 +3029,75 @@ extern "C" int wn_gen_prefill_commit(wn_gen_handle* h, int t_end) {
         WN_REQUIRE(h->pf_t_end[l] == t_end, WN_E_STATE, "wn_gen_prefill_commit: layer %d was filled for t_end %d, not %d", l,
                    h->pf_t_end[l], t_end);
     h->cur_t = t_end;
+    return 0;
+}
+
+extern "C" int wn_gen_set_time(wn_gen_handle* h, int t) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_time: null handle");
+    WN_REQUIRE(h->tables_uploaded && h->cur_t == 0 && h->pf_plain < 0 && h->seat_plain < 0, WN_E_STATE,
+               "wn_gen_set_time: only right after wn_gen_reset (the handle is at t = %d)", h->cur_t);
+    WN_REQUIRE(t >= 0, WN_E_BADARG, "wn_gen_set_time: t must be >= 0, got %d", t);
+    h->cur_t = t;
+    h->run_origin.assign(h->shape.n_streams, INT_MIN);       // no stream's rings hold anything for these times
+    return 0;
+}
+
+extern "C" int wn_gen_seat_layer(wn_gen_handle* h, int layer, int n, const int* slots, const int* q_end, const void* d_src,
+                                 int layout, int L, int frame_of_end, void* stream) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_seat_layer: null handle");
+    WN_REQUIRE(h->tables_uploaded, WN_E_STATE, "wn_gen_seat_layer: call wn_gen_reset first");
+    const int NS = h->shape.n_streams, R = h->shape.R, t = h->cur_t;
+    WN_REQUIRE(layer >= 0 && layer < h->shape.n_layers && n >= 1 && slots && q_end, WN_E_BADARG,
+               "wn_gen_seat_layer: bad arguments (layer %d, %d slots)", layer, n);
+    const GenLayer& Lr = h->layers[layer];
+    if (d_src) {
+        WN_REQUIRE((layout == WN_GEN_SRC_FRAMES || (layout == WN_GEN_SRC_PAIRS && R % 8 == 0)) && L >= 1 && frame_of_end <= L,
+                   WN_E_BADARG, "wn_gen_seat_layer: bad source (layout %d, L %d, frame %d)", layout, L, frame_of_end);
+    }
+    std::vector<char> seen(NS, 0);
+    for (int j = 0; j < n; ++j) {
+        WN_REQUIRE(slots[j] >= 0 && slots[j] < NS && !seen[slots[j]], WN_E_BADARG,
+                   "wn_gen_seat_layer: slot %d is out of range or listed twice", slots[j]);
+        seen[slots[j]] = 1;
+        WN_REQUIRE(q_end[j] >= 0 && (long long)t - q_end[j] >= INT_MIN / 2, WN_E_BADARG,
+                   "wn_gen_seat_layer: slot %d: bad prompt end position %d", slots[j], q_end[j]);
+        const int need = std::min(q_end[j], Lr.ring_len);    // positions [q_end - need, q_end) come from the source
+        if (d_src && need > 0) {
+            WN_REQUIRE(frame_of_end - need >= 0, WN_E_BADARG,
+                       "wn_gen_seat_layer: layer %d needs frames [%d, %d), the buffer starts at 0", layer, frame_of_end - need,
+                       frame_of_end);
+            // every kernel reads times < 0 as zero history without looking at the ring
+            WN_REQUIRE(t - need >= 0, WN_E_BADARG,
+                       "wn_gen_seat_layer: slot %d: positions [%d, %d) would lie at times [%d, %d), and times < 0 read as "
+                       "zero (start the handle later with wn_gen_set_time)", slots[j], q_end[j] - need, q_end[j], t - need, t);
+        }
+    }
+    const int kid = pick_kernel(h);
+    WN_REQUIRE(kid != 0, WN_E_UNSUPP, "wn_gen_seat_layer: no sampler kernel fits this net in mode %d", h->mode);
+    const int plain = kid == 1;
+    WN_REQUIRE(h->seat_plain < 0 || h->seat_plain == plain, WN_E_STATE,
+               "wn_gen_seat_layer: the sampler kernel changed between seats (ring layout differs)");
+    for (int j0 = 0; j0 < n; j0 += GEN_SEAT_MAX) {
+        GenSeatList list;
+        list.n = std::min(GEN_SEAT_MAX, n - j0);
+        for (int j = 0; j < list.n; ++j) { list.slot[j] = slots[j0 + j]; list.q_end[j] = q_end[j0 + j]; }
+        // sequence j of the source is listed slot j: offset the source to this chunk's first sequence
+        const void* src = d_src;
+        if (d_src)
+            src = static_cast<const char*>(d_src) + (size_t)j0 * L * R * (layout == WN_GEN_SRC_PAIRS ? 2 * sizeof(__nv_bfloat16)
+                                                                                                      : sizeof(float));
+        const long long cnt = (long long)Lr.ring_len * list.n * R;
+        const int grid = (int)std::min<long long>((cnt + 255) / 256, 4LL * h->sm_count);
+        gen_prefill_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, layout == WN_GEN_SRC_PAIRS, L, frame_of_end,
+                                                                   t - Lr.ring_len, t, NS, R, Lr.ring_len, h->base.rings,
+                                                                   Lr.ring_off, plain, list);
+        WN_CUDA(cudaGetLastError());
+    }
+    h->seat_plain = plain;
+    for (int j = 0; j < n; ++j) {
+        h->seat_t[(size_t)layer * NS + slots[j]] = t;
+        h->seat_origin[(size_t)layer * NS + slots[j]] = t - q_end[j];
+    }
     return 0;
 }
 
@@ -3166,8 +3279,28 @@ extern "C" int wn_gen_set_stream_params(wn_gen_handle* h, const wn_gen_stream_pa
     }
     if (NS > 1) {                                           // one stream: wn_gen_run folds the record into the scalars
         if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, sizeof(GenStream) * (size_t)NS));
-        h->sp_dirty = true;
     }
+    h->sp_dirty = true;
+    return 0;
+}
+
+extern "C" int wn_gen_set_stream_positions(wn_gen_handle* h, const wn_gen_stream_pos* pos) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_stream_positions: null handle");
+    if (pos == nullptr) {
+        h->pos.clear();
+        h->sp_dirty = true;
+        return 0;
+    }
+    WN_REQUIRE(!h->sp.empty(), WN_E_STATE, "wn_gen_set_stream_positions: positions need per-stream records "
+                                           "(wn_gen_set_stream_params) first");
+    const int NS = h->shape.n_streams;
+    for (int s = 0; s < NS; ++s)
+        WN_REQUIRE(pos[s].sample0 >= 0 && pos[s].first0 >= 0, WN_E_BADARG,
+                   "wn_gen_set_stream_positions: stream %d: sample0 %d and first0 %d must be >= 0", s, pos[s].sample0,
+                   pos[s].first0);
+    if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, sizeof(GenStream) * (size_t)NS));
+    h->pos.assign(pos, pos + NS);
+    h->sp_dirty = true;
     return 0;
 }
 
@@ -3187,9 +3320,10 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
     WN_REQUIRE(a->n_given >= 1 && a->n_samples >= 0 && a->n_evals >= 0 && a->t0 >= 0, WN_E_BADARG, "wn_gen_run: bad counts");
     WN_REQUIRE(a->t0 == h->cur_t, WN_E_STATE, "wn_gen_run: t0=%d does not continue the previous call (expected %d)", a->t0,
                h->cur_t);
-    const bool per_stream = !h->sp.empty();
+    const bool per_stream = !h->sp.empty(), positions = !h->pos.empty();
+    WN_REQUIRE(!positions || per_stream, WN_E_STATE, "wn_gen_run: stream positions need per-stream records");
     if (per_stream) {
-        WN_REQUIRE(a->n_given == h->sp_max_given, WN_E_BADARG,
+        WN_REQUIRE(positions || a->n_given == h->sp_max_given, WN_E_BADARG,
                    "wn_gen_run: with per-stream parameters n_given is the pitch of d_first and must equal the longest prompt "
                    "(%d), got %d", h->sp_max_given, a->n_given);
         WN_REQUIRE(a->temperature == 0.f && a->regularize == 0.f && h->top_k == 0 && h->top_p == 1.0, WN_E_BADARG,
@@ -3197,10 +3331,51 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                    "handle's truncation off (the records hold them)");
         WN_REQUIRE(!h->sp_any_temp || a->d_uniforms, WN_E_BADARG, "wn_gen_run: a stream with temperature > 0 needs d_uniforms");
     }
-    const int head_from = per_stream ? h->sp_head_from : a->n_given - 1;
-    WN_REQUIRE(a->t0 + a->n_evals <= head_from + a->n_samples, WN_E_BADARG,
-               "wn_gen_run: evaluations [%d,%d) exceed the schedule of %d samples from evaluation %d", a->t0,
-               a->t0 + a->n_evals, a->n_samples, head_from);
+    int head_from = per_stream ? h->sp_head_from : a->n_given - 1;
+    const int NS = h->shape.n_streams;
+    if (positions) {
+        // per stream: positions [q0, q1] of the launch; every read of first / forced and every written column in its row
+        head_from = INT_MAX;
+        for (int s = 0; s < NS; ++s) {
+            const wn_gen_stream_pos& o = h->pos[s];
+            const int ng = h->sp[s].n_given;
+            WN_REQUIRE(o.origin <= a->t0, WN_E_BADARG, "wn_gen_run: stream %d starts at t = %d, after t0 = %d", s, o.origin,
+                       a->t0);
+            const long long q0 = (long long)a->t0 - o.origin, q1 = q0 + a->n_evals - 1;
+            head_from = (int)std::min<long long>(head_from, (long long)o.origin + ng - 1);
+            if (a->n_evals == 0) continue;
+            if (q0 < ng)
+                WN_REQUIRE(q0 - o.first0 >= 0 && std::min<long long>(q1, ng - 1) - o.first0 < a->n_given, WN_E_BADARG,
+                           "wn_gen_run: stream %d reads prompt positions [%lld, %lld], its row holds [%d, %d)", s, q0,
+                           std::min<long long>(q1, ng - 1), o.first0, o.first0 + a->n_given);
+            if (a->d_forced && q1 >= ng)
+                WN_REQUIRE(std::max<long long>(q0, ng) - ng - o.sample0 >= 0 && q1 - ng - o.sample0 < a->n_samples,
+                           WN_E_BADARG, "wn_gen_run: stream %d reads forced samples outside its row", s);
+            const long long i0 = std::max<long long>(q0 - (ng - 1), 0), i1 = q1 - (ng - 1);
+            if (i1 >= i0)
+                WN_REQUIRE(i0 - o.sample0 >= 0 && i1 - o.sample0 < a->n_samples, WN_E_BADARG,
+                           "wn_gen_run: stream %d selects samples [%lld, %lld] into columns [%lld, %lld], outside [0, %d)", s,
+                           i0, i1, i0 - o.sample0, i1 - o.sample0, a->n_samples);
+        }
+    } else {
+        WN_REQUIRE(a->t0 + a->n_evals <= head_from + a->n_samples, WN_E_BADARG,
+                   "wn_gen_run: evaluations [%d,%d) exceed the schedule of %d samples from evaluation %d", a->t0,
+                   a->t0 + a->n_evals, a->n_samples, head_from);
+    }
+    // a stream that starts at another origin than it ran with: its rings must have been seated for it at this t, and its
+    // first evaluation must read a prompt sample (cur_idx holds the previous job's last choice)
+    for (int s = 0; s < NS; ++s) {
+        const int origin = positions ? h->pos[s].origin : 0;
+        if (origin == h->run_origin[s]) continue;
+        for (int l = 0; l < h->shape.n_layers; ++l) {
+            const size_t e = (size_t)l * NS + s;
+            WN_REQUIRE(h->seat_t[e] == h->cur_t && h->seat_origin[e] == origin, WN_E_STATE,
+                       "wn_gen_run: stream %d starts at t = %d but layer %d was not seated for it at t = %d", s, origin, l,
+                       h->cur_t);
+        }
+        WN_REQUIRE(!positions || (long long)a->t0 - origin < h->sp[s].n_given || a->n_evals == 0, WN_E_BADARG,
+                   "wn_gen_run: the first evaluation of newly seated stream %d must read a prompt sample", s);
+    }
     WN_REQUIRE(!(a->temperature > 0.f) || a->d_uniforms, WN_E_BADARG, "wn_gen_run: temperature > 0 needs d_uniforms");
     if (a->n_evals == 0) return 0;
     if (h->base.cond && h->base.cond_hop) {
@@ -3213,6 +3388,9 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
     WN_REQUIRE(kid != 0, WN_E_UNSUPP,
                "wn_gen_run: %d streams need a cluster kernel (modes 4, 6) for this net; mode %d does not fit in shared memory",
                h->shape.n_streams, h->mode);
+    WN_REQUIRE(!(positions && kid == 3), WN_E_UNSUPP, "wn_gen_run: kernel 3 reads no stream positions (mode 2 sums alike)");
+    WN_REQUIRE(h->seat_plain < 0 || h->seat_plain == (kid == 1), WN_E_STATE,
+               "wn_gen_run: the rings were seated for another kernel's ring layout than kernel %d keeps", kid);
     if (h->pf_plain >= 0) {
         WN_REQUIRE(h->cur_t > 0, WN_E_STATE, "wn_gen_run: rings were prefilled but not committed (wn_gen_prefill_commit)");
         WN_REQUIRE(h->pf_plain == (kid == 1), WN_E_STATE,
@@ -3224,13 +3402,18 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                    head_from + 1);
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (per_stream && h->shape.n_streams > 1 && h->sp_dirty) {
+    // one stream without positions folds its record into the scalars (kernel 3 reads only those)
+    const bool records = per_stream && (h->shape.n_streams > 1 || positions);
+    if (records && h->sp_dirty) {
         // in stream order, so that a launch still reading the previous records finishes first
         std::vector<GenStream> recs(h->sp.size());
         for (size_t s = 0; s < recs.size(); ++s) {
             const wn_gen_stream_params& q = h->sp[s];
             recs[s].n_given = q.n_given; recs[s].top_k = q.top_k; recs[s].trunc = stream_truncates(q, h->shape.classes);
             recs[s].temperature = q.temperature; recs[s].regularize = q.regularize; recs[s].top_p = q.top_p;
+            recs[s].origin = positions ? h->pos[s].origin : 0;
+            recs[s].sample0 = positions ? h->pos[s].sample0 : 0;
+            recs[s].first0 = positions ? h->pos[s].first0 : 0;
         }
         WN_CUDA(cudaMemcpyAsync(h->d_sp, recs.data(), sizeof(GenStream) * recs.size(), cudaMemcpyHostToDevice, st));
         WN_CUDA(cudaStreamSynchronize(st));                   // recs is pageable host memory that dies with this scope
@@ -3251,11 +3434,11 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         p.trunc = a->temperature > 0.f && ((h->top_k > 0 && h->top_k < h->shape.classes) || h->top_p < 1.0);
         p.ps = nullptr;
         p.head_from = head_from;
-        if (per_stream && h->shape.n_streams == 1) {           // the single record becomes the scalars (kernel 3 reads only those)
+        if (per_stream && !records) {                          // the single record becomes the scalars (kernel 3 reads only those)
             const wn_gen_stream_params& q = h->sp[0];
             p.temperature = q.temperature; p.regularize = q.regularize; p.top_k = q.top_k; p.top_p = q.top_p;
             p.trunc = stream_truncates(q, h->shape.classes);
-        } else if (per_stream) {
+        } else if (records) {
             p.ps = h->d_sp;
             p.trunc = h->sp_any_trunc;                          // sizes kernel 1's truncation scratch; the records decide
         }
@@ -3288,6 +3471,7 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         done += n;
     }
     h->cur_t = a->t0 + a->n_evals;
+    for (int s = 0; s < NS; ++s) h->run_origin[s] = positions ? h->pos[s].origin : 0;
     return 0;
 }
 

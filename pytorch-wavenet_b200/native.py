@@ -118,6 +118,10 @@ class GenStreamParams(C.Structure):
                 ("top_p", C.c_double)]
 
 
+class GenStreamPos(C.Structure):
+    _fields_ = [("origin", C.c_int), ("sample0", C.c_int), ("first0", C.c_int)]
+
+
 class GenRunArgs(C.Structure):
     _fields_ = [("d_first", C.c_void_p), ("n_given", C.c_int),
                 ("d_forced", C.c_void_p), ("d_uniforms", C.c_void_p),
@@ -216,6 +220,10 @@ SIGNATURES = {
     "wn_gen_set_condition_frames": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3),
     "wn_gen_set_truncation": (C.c_int, [C.c_void_p, C.c_int, C.c_double]),
     "wn_gen_set_stream_params": (C.c_int, [C.c_void_p, C.POINTER(GenStreamParams)]),
+    "wn_gen_set_stream_positions": (C.c_int, [C.c_void_p, C.POINTER(GenStreamPos)]),
+    "wn_gen_seat_layer": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]
+                          + [C.c_int] * 3 + [C.c_void_p]),
+    "wn_gen_set_time": (C.c_int, [C.c_void_p, C.c_int]),
     "wn_gen_kernel_id": (C.c_int, [C.c_void_p]),
     "wn_gen_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_read_trace": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_void_p]),

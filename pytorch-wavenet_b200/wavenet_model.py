@@ -988,12 +988,15 @@ class _Runtime:
         return grads
 
     # ------------------------------------------------------------------ sampler
+    def sampler_keys(self, n_streams):
+        """(key, wkey) of a sampler handle: the parameter tensors it reads, and the state of their values"""
+        m = self.model
+        return ((n_streams, tuple(p.data_ptr() for p in m.parameters())),
+                (tuple(p._version for p in m.parameters()), self.weights_epoch))
+
     def sampler(self, n_streams):
-        m, lib = self.model, native.lib()
-        dev = self.device()
-        P = self._params()
-        key = (n_streams, tuple(p.data_ptr() for p in m.parameters()))
-        wkey = (tuple(p._version for p in m.parameters()), self.weights_epoch)
+        lib = native.lib()
+        key, wkey = self.sampler_keys(n_streams)
         s = self.samplers.get(n_streams)
         if s is not None and s["key"] == key:
             if s["wkey"] != wkey:                 # same tensors, new values: the batched kernel re-splits its weight images
@@ -1002,6 +1005,16 @@ class _Runtime:
             return s
         if s is not None:
             lib.wn_gen_destroy(s["handle"])
+        s = self.new_sampler(n_streams)
+        self.samplers[n_streams] = s
+        return s
+
+    def new_sampler(self, n_streams):
+        """A fresh sampler handle for n_streams streams with its workspaces (the caller owns it: wn_gen_destroy)."""
+        m, lib = self.model, native.lib()
+        dev = self.device()
+        P = self._params()
+        key, wkey = self.sampler_keys(n_streams)
         n = m.layers * m.blocks
         dil = (ctypes.c_int * n)(*[d for d, _ in m.dilations])
         shape = native.GenShape(n, m.kernel_size, m.residual_channels, m.dilation_channels, m.skip_channels,
@@ -1025,9 +1038,7 @@ class _Runtime:
         handle = ctypes.c_void_p()
         native.check(lib.wn_gen_create(ctypes.byref(shape), ctypes.byref(wts), rings.data_ptr(), scratch.data_ptr(),
                                        ctypes.byref(handle)), "gen create")
-        s = dict(key=key, wkey=wkey, handle=handle, rings=rings, scratch=scratch, n_streams=n_streams)
-        self.samplers[n_streams] = s
-        return s
+        return dict(key=key, wkey=wkey, handle=handle, rings=rings, scratch=scratch, n_streams=n_streams)
 
     def reset_sampler(self, s, stream):
         lib = native.lib()
@@ -1038,16 +1049,25 @@ class _Runtime:
 
     def prefill(self, s, d_first, T, cond=None, ctab=None, local=None):
         """Write the rings of the freshly reset sampler ``s`` as evaluations [0, T) would, from one forward over the prompt
-        window of prefill_window, and move the handle to t = T (wn_gen_prefill_*).  d_first: the (NS, >= T + 1) int32
-        prompts on the device; cond: the (NS, G) condition rows, ctab their table (s["cond"]); local: the sampler's
-        (series, hop).  256-channel nets run the fused tensor-core blocks in bf16 pairs whatever tc_precision says (fp32-class,
-        the sampler's parity class); every other net, 512 channels included (single-pass bf16 there, ~1e-3), the FFMA
-        blocks.  One launch per layer, each followed by the scatter of its output into the next layer's ring; layer 0's
-        ring comes from the fp32 start conv, which is the sampler's own gather w[:, c] + b."""
+        window of prefill_window (prefill_forward), and move the handle to t = T (wn_gen_prefill_*)."""
+        lib, h = native.lib(), s["handle"]
+
+        def scatter(layer, src, layout, L, stream):
+            native.check(lib.wn_gen_prefill_layer(h, layer, src, layout, L, L, T, stream), f"prefill layer {layer}")
+        self.prefill_forward(d_first, T, scatter, cond=cond, ctab=ctab, local=local)
+        native.check(lib.wn_gen_prefill_commit(h, T), "prefill commit")
+
+    def prefill_forward(self, d_first, T, scatter, cond=None, ctab=None, local=None):
+        """One forward over the prompt window of prefill_window(T): scatter(layer, src, layout, L, stream) receives every
+        layer's input over the window (sequence b of src = prompt b, frame L - 1 = position T - 1) right after it is
+        computed.  d_first: the (B, >= T + 1) int32 prompts on the device; cond: the (B, G) condition rows, ctab their table;
+        local: the sampler's (series, hop).  256-channel nets run the fused tensor-core blocks in bf16 pairs whatever
+        tc_precision says (fp32-class, the sampler's parity class); every other net, 512 channels included (single-pass bf16
+        there, ~1e-3), the FFMA blocks.  One launch per layer, each followed by the scatter of its output; layer 0's input
+        comes from the fp32 start conv, which is the sampler's own gather w[:, c] + b."""
         m, lib = self.model, native.lib()
         dev = self.device()
         stream = torch.cuda.current_stream(dev).cuda_stream
-        h = s["handle"]
         R, D, Sk, Cc, k = m.residual_channels, m.dilation_channels, m.skip_channels, m.classes, m.kernel_size
         dil = [d for d, _ in m.dilations]
         NS, nl = d_first.shape[0], len(dil)
@@ -1063,7 +1083,7 @@ class _Runtime:
         ws_t, bs_p = Wp["start"]
         native.check(lib.wn_start_fwd_index_i64(idx.data_ptr(), ws_t.data_ptr(), bs_p.data_ptr(), buf[0].data_ptr(),
                                                 NS, Cc, L, R, stream), "prefill start")
-        native.check(lib.wn_gen_prefill_layer(h, 0, buf[0].data_ptr(), native.GEN_SRC_FRAMES, L, L, T, stream), "prefill layer 0")
+        scatter(0, buf[0].data_ptr(), native.GEN_SRC_FRAMES, L, stream)
         frames = None                                       # (table, n_frames, hop) of repeat-upsampled local conditioning
         if local is not None and not (upsampled and use_tb):
             y, hop = local
@@ -1121,10 +1141,7 @@ class _Runtime:
                     rc = lib.wn_block_fwd(ctypes.byref(a), stream)
             native.check(rc, f"prefill block {i}")
             src = 1 - src
-            native.check(lib.wn_gen_prefill_layer(h, i + 1, buf[src].data_ptr(),
-                                                  native.GEN_SRC_PAIRS if use_tb else native.GEN_SRC_FRAMES, L, L, T, stream),
-                         f"prefill layer {i + 1}")
-        native.check(lib.wn_gen_prefill_commit(h, T), "prefill commit")
+            scatter(i + 1, buf[src].data_ptr(), native.GEN_SRC_PAIRS if use_tb else native.GEN_SRC_FRAMES, L, stream)
         self.last_prefill = dict(P0=P0, S=S, W=W, blocks="tb" if use_tb else "ffma")
 
     def generate_resident(self, s, d_first, n_given, num_samples, temperature, regularize, d_out, d_uni=None,
@@ -1258,6 +1275,276 @@ class _Runtime:
             (forced.nbytes if d_forced is not None else 0)
         self.d2h_bytes_last = NS * num_samples * 4 + (logits.nbytes if want_logits else 0)
         return idx, logits, total_evals
+
+
+class _Job:
+    """One submitted sampling job of a SamplingSession and what it has produced so far."""
+
+    def __init__(self, jid, prompt, count, temperature, regularize, top_k, top_p, cond, uniforms):
+        self.id, self.prompt, self.count = jid, prompt, count
+        self.temperature, self.regularize, self.top_k, self.top_p = temperature, regularize, top_k, top_p
+        self.cond, self.uniforms = cond, uniforms
+        self.idx, self.logits = [], []
+        self.made = 0
+
+
+class SamplingSession:
+    """Continuous batching on one sampler handle of ``n_slots`` streams (WaveNetModel.sampling_session).
+
+    Jobs queue FIFO (submit); every step() seats queued jobs into free slots, runs ``n_evals`` evaluations of all slots in
+    one launch and hands each job its new samples.  A slot whose job is done takes the next queued job at the next step, at
+    its own position: the handle's time t is global, a job's position is t - origin (wn_gen_set_stream_positions), and
+    seating writes the slot's rings for the times its new positions read (wn_gen_seat_layer), zeros or, with
+    ``prefill=True``, the values of one forward over the job's prompt window (as generate_fast(prefill=True) computes them).
+    An empty slot runs a parked temperature-0 job whose outputs are discarded.  Each job gives, bit for bit, what a
+    generate_fast_batch launch of the same slot count carrying that job in every stream gives, with the same uniforms and
+    the same ``prefill``.  The session owns its handle: generate_fast* calls on the model never touch it.  Global
+    conditioning is per job; local conditioning is not supported (it would need per-stream frame windows)."""
+
+    _T_MAX = 2 ** 31 - 1
+
+    def __init__(self, model, n_slots, prefill=False, return_logits=False):
+        if isinstance(n_slots, (bool, np.bool_)) or not isinstance(n_slots, (int, np.integer)) or n_slots < 1:
+            raise ValueError(f"n_slots must be an integer >= 1, got {n_slots!r}")
+        _check_prefill(prefill)
+        if getattr(model, "local_condition_channels", 0):
+            raise ValueError("sampling sessions do not support local conditioning (it would need per-stream frame windows); "
+                             "use generate_fast_batch")
+        self.model, self.n_slots, self.prefill, self.return_logits = model, int(n_slots), prefill, bool(return_logits)
+        self.rt = rt = model._runtime()
+        self.dev = rt.device()
+        self.queue, self.jobs, self.next_id = [], {}, 0
+        self.slot_job = [None] * self.n_slots          # the job in each slot, None: parked
+        self.origin = [0] * self.n_slots
+        self.seated = [False] * self.n_slots           # False: the slot must be (re)seated at the next step
+        dil = [d for d, _ in model.dilations]
+        self.t_start = (model.kernel_size - 1) * max(dil) + 1     # past the longest ring: primed history lies at t >= 0
+        with torch.cuda.device(self.dev):
+            self.s = rt.new_sampler(self.n_slots)
+            self.G = getattr(model, "condition_channels", 0)
+            self.ctab = None
+            if self.G:                                 # rows of parked slots: the zero condition (the biases)
+                stream = torch.cuda.current_stream(self.dev).cuda_stream
+                zero = torch.zeros(self.n_slots, self.G, device=self.dev, dtype=torch.float32)
+                self.ctab = rt.packed_weights(stream).cond_table(zero, stream)
+            self.reset()
+
+    def __del__(self):
+        s = self.__dict__.get("s")
+        if s is not None:
+            native.lib().wn_gen_destroy(s["handle"])
+
+    # ------------------------------------------------------------------ public
+    @property
+    def pending(self):
+        """jobs submitted and not yet seated"""
+        return len(self.queue)
+
+    @property
+    def active(self):
+        """jobs seated and not yet done"""
+        return sum(j is not None for j in self.slot_job)
+
+    def reset(self):
+        """Restart the handle's time (allowed only while no job is active); queued jobs stay queued."""
+        if self.active:
+            raise RuntimeError(f"reset() with {self.active} active jobs")
+        lib, h = native.lib(), self.s["handle"]
+        with torch.cuda.device(self.dev):
+            self.rt.reset_sampler(self.s, torch.cuda.current_stream(self.dev).cuda_stream)
+        native.check(lib.wn_gen_set_time(h, self.t_start), "session time")
+        native.check(lib.wn_gen_set_condition(h, native.ptr(self.ctab)), "session condition")
+        self.t = self.t_start
+        self.seated = [False] * self.n_slots
+
+    def submit(self, first_samples, num_samples, temperature=1., regularize=0., top_k=0, top_p=1.0, condition=None,
+               uniforms=None):
+        """Queue one job: generate_fast(num_samples, first_samples, temperature, regularize, top_k=, top_p=, condition=)
+        with ``uniforms`` (num_samples,) float64 for its draws; None draws them from numpy's global RNG now when
+        temperature > 0.  Returns the job id.  ValueError for a malformed argument, before any device work."""
+        if torch.is_tensor(first_samples):
+            first_samples = first_samples.detach().cpu().numpy()
+        prompt = np.asarray(first_samples)
+        if prompt.ndim == 0:
+            prompt = prompt.reshape(1)
+        plan = _stream_plan([prompt], [num_samples], [temperature], [regularize], [top_k], [top_p])
+        count = plan.counts[0]
+        cond = self.model._condition(self.model._one_condition(condition), 1)
+        if plan.temperature[0] > 0:
+            if uniforms is None:
+                uniforms = np.random.random_sample(count)
+            u = np.asarray(uniforms.detach().cpu().numpy() if torch.is_tensor(uniforms) else uniforms, dtype=np.float64)
+            if u.ndim != 1 or u.shape[0] < count:
+                raise ValueError(f"uniforms must be a 1-D array of at least {count} values, got shape {u.shape}")
+            uniforms = u[:count].copy()
+        else:
+            uniforms = None
+        jid = self.next_id
+        self.next_id += 1
+        job = _Job(jid, plan.first[0, :plan.n_given[0]].copy(), count, plan.temperature[0], plan.regularize[0],
+                   plan.top_k[0], plan.top_p[0], cond, uniforms)
+        self.jobs[jid] = job
+        self.queue.append(job)
+        return jid
+
+    def result(self, job_id):
+        """A done job's indices (int64 (n,)) [and logits (n, classes)]; None while it is queued or running."""
+        job = self.jobs[job_id]
+        if job.made < job.count:
+            return None
+        idx = np.concatenate(job.idx).astype(np.int64) if job.idx else np.zeros(0, dtype=np.int64)
+        if not self.return_logits:
+            return idx
+        C = self.model.classes
+        return idx, (np.concatenate(job.logits) if job.logits else np.zeros((0, C), dtype=np.float32))
+
+    def step(self, n_evals):
+        """Seat queued jobs into free slots, run n_evals evaluations of every slot, return {job_id: new indices} (with
+        return_logits: {job_id: (indices, logits)}) for the jobs that ran."""
+        if isinstance(n_evals, (bool, np.bool_)) or not isinstance(n_evals, (int, np.integer)) or n_evals < 1:
+            raise ValueError(f"n_evals must be an integer >= 1, got {n_evals!r}")
+        n_evals = int(n_evals)
+        key, wkey = self.rt.sampler_keys(self.n_slots)
+        if (key, wkey) != (self.s["key"], self.s["wkey"]):
+            raise RuntimeError("the model's parameters changed after the session was created; create a new session")
+        if self.t + n_evals >= self._T_MAX:
+            raise RuntimeError(f"step({n_evals}) would move the session's time past 2^31 - 1; reset() it between jobs")
+        with torch.cuda.device(self.dev):
+            return self._step(n_evals)
+
+    # ------------------------------------------------------------------ internals
+    def _seat(self, seats, stream):
+        lib, h = native.lib(), self.s["handle"]
+        nl = self.model.layers * self.model.blocks
+        zeros, primed = [], {}
+        for b, job in seats:
+            self.slot_job[b] = job
+            T = 0 if job is None or not self.prefill else job.prompt.shape[0] - 1
+            self.origin[b] = self.t - T
+            if T == 0:
+                zeros.append(b)
+            else:
+                primed.setdefault(T, []).append((b, job))    # windows line up: one forward per prompt length
+            if job is not None and job.cond is not None:
+                self.ctab[:, b, :] = self.rt.packed_weights(stream).cond_table(job.cond, stream)[:, 0, :]
+            self.seated[b] = True
+        if zeros:
+            sl = (ctypes.c_int * len(zeros))(*zeros)
+            qe = (ctypes.c_int * len(zeros))(*([0] * len(zeros)))
+            for l in range(nl):
+                native.check(lib.wn_gen_seat_layer(h, l, len(zeros), sl, qe, None, 0, 1, 0, stream), "seat")
+        for T, group in primed.items():
+            slots = [b for b, _ in group]
+            sl = (ctypes.c_int * len(slots))(*slots)
+            qe = (ctypes.c_int * len(slots))(*([T] * len(slots)))
+            d_first = torch.from_numpy(np.stack([j.prompt for _, j in group]).astype(np.int32)).to(self.dev)
+            cond = ctab = None
+            if self.G:
+                cond = torch.cat([j.cond for _, j in group])
+                ctab = self.rt.packed_weights(stream).cond_table(cond, stream)
+
+            def scatter(layer, src, layout, L, st, sl=sl, qe=qe, n=len(slots)):
+                native.check(lib.wn_gen_seat_layer(h, layer, n, sl, qe, src, layout, L, L, st), f"seat layer {layer}")
+            self.rt.prefill_forward(d_first, T, scatter, cond=cond, ctab=ctab)
+
+    def _step(self, n_evals):
+        lib, h = native.lib(), self.s["handle"]
+        stream = torch.cuda.current_stream(self.dev).cuda_stream
+        seats = _session_admit(self.slot_job, self.seated, self.queue)
+        if seats:
+            self._seat(seats, stream)
+        NS, t = self.n_slots, self.t
+        recs, pos, first, uni, plans = _session_records(t, n_evals, self.slot_job, self.origin)
+        native.check(lib.wn_gen_set_stream_params(h, recs), "session stream params")
+        native.check(lib.wn_gen_set_stream_positions(h, pos), "session positions")
+        d_first = torch.from_numpy(first).to(self.dev, non_blocking=True)
+        d_uni = torch.from_numpy(uni).to(self.dev, non_blocking=True)
+        d_out = torch.zeros(NS, n_evals, device=self.dev, dtype=torch.int32)
+        d_logits = torch.zeros(NS, n_evals, self.model.classes, device=self.dev, dtype=torch.float32) \
+            if self.return_logits else None
+        args = native.GenRunArgs()
+        args.d_first, args.n_given = d_first.data_ptr(), first.shape[1]
+        args.d_forced, args.d_uniforms = None, d_uni.data_ptr()
+        args.d_out_idx, args.d_out_logits = d_out.data_ptr(), native.ptr(d_logits)
+        args.n_samples, args.t0, args.n_evals = n_evals, t, n_evals
+        args.temperature, args.regularize = 0.0, 0.0
+        native.check(lib.wn_gen_run(h, ctypes.byref(args), stream), "session run")
+        self.t = t + n_evals
+        idx = d_out.cpu().numpy().astype(np.int64)          # synchronises
+        native.check(lib.wn_gen_check(h, stream), "session check")
+        logits = d_logits.cpu().numpy() if self.return_logits else None
+        out = {}
+        for b, job, c0, n in plans:
+            new = idx[b, c0:c0 + n]
+            job.idx.append(new)
+            job.made += n
+            if self.return_logits:
+                lg = logits[b, c0:c0 + n]
+                job.logits.append(lg)
+                out[job.id] = (new, lg)
+            else:
+                out[job.id] = new
+        for b in range(NS):                                  # done jobs give their slot to the next step's admission
+            job = self.slot_job[b]
+            if job is not None and job.made >= job.count:
+                self.slot_job[b] = None
+                self.seated[b] = False
+        return out
+
+
+def _session_admit(slot_job, seated, queue):
+    """A session step's admission: queued jobs (FIFO) go to the free slots, lowest slot first; a job of 0 samples is done
+    without a slot; a free slot left over is parked (seated with no job) unless it is parked already.  Pops the admitted
+    jobs off ``queue``; returns [(slot, job or None)], the slots to seat."""
+    seats = []
+    for b, job in enumerate(slot_job):
+        if job is not None:
+            continue
+        nxt = None
+        while queue:
+            cand = queue.pop(0)
+            if cand.count > 0:
+                nxt = cand
+                break
+        if nxt is None and seated[b]:
+            continue
+        seats.append((b, nxt))
+    return seats
+
+
+def _session_records(t, n_evals, slot_job, origin):
+    """The launch of a session step of n_evals evaluations from time t: (stream params, stream positions, (NS, pitch) int32
+    prompt rows, (NS, n_evals) float64 uniforms, [(slot, job, first column, new samples)]).  Slot b's job is at position
+    q0 = t - origin[b]: its prompt row holds positions [first0, min(n_given, q0 + n_evals)) with first0 = q0 while the
+    launch still reads the prompt; its output columns start at sample sample0 = max(0, q0 - (n_given - 1)).  A parked slot
+    (job None) runs a temperature-0 job of the prompt [0]."""
+    NS = len(slot_job)
+    recs = (native.GenStreamParams * NS)()
+    pos = (native.GenStreamPos * NS)()
+    rows, plans = [], []
+    uni = np.zeros((NS, n_evals), dtype=np.float64)
+    for b, job in enumerate(slot_job):
+        prompt = job.prompt if job is not None else np.zeros(1, dtype=np.int32)
+        ng = prompt.shape[0]
+        q0 = t - origin[b]
+        first0 = q0 if q0 < ng else 0
+        rows.append(prompt[first0:min(ng, q0 + n_evals)] if q0 < ng else prompt[:0])
+        i0 = q0 - (ng - 1)
+        sample0 = max(i0, 0)
+        pos[b] = native.GenStreamPos(origin[b], sample0, first0)
+        if job is None:
+            recs[b] = native.GenStreamParams(1, 0, 0.0, 0.0, 1.0)
+            continue
+        recs[b] = native.GenStreamParams(ng, job.top_k, job.temperature, job.regularize, job.top_p)
+        hi = min(job.count, i0 + n_evals)               # the job's new samples [sample0, hi) in columns [0, hi - sample0)
+        if hi > sample0:
+            plans.append((b, job, 0, hi - sample0))
+            if job.uniforms is not None:
+                uni[b, :hi - sample0] = job.uniforms[sample0:hi]
+    first = np.zeros((NS, max(1, max(r.shape[0] for r in rows))), dtype=np.int32)
+    for b, r in enumerate(rows):
+        first[b, :r.shape[0]] = r
+    return recs, pos, first, uni, plans
 
 
 class _StreamPlan:
@@ -1911,6 +2198,19 @@ class WaveNetModel(nn.Module):
             idx = idx[:, :plan.counts[0]]
             logits = logits[:, :plan.counts[0]] if return_logits else None
         return (idx, logits) if return_logits else idx
+
+    def sampling_session(self, n_slots, prefill=False, return_logits=False):
+        """Continuous batching: a SamplingSession of ``n_slots`` streams on its own sampler handle.  ``submit(first_samples,
+        num_samples, temperature=1., regularize=0., top_k=0, top_p=1.0, condition=None, uniforms=None)`` queues a job and
+        returns its id; ``step(n_evals)`` seats queued jobs into free slots, runs n_evals evaluations of every slot and
+        returns {job_id: new indices} (with return_logits: {job_id: (indices, logits)}); ``result(job_id)`` gives a done
+        job's output; ``pending`` / ``active`` count queued and running jobs.  Each job gives, bit for bit, what a
+        generate_fast_batch call of n_slots copies of that job gives (same uniforms, same prefill); with uniforms=None a
+        seeded sequence of submits draws what seeded generate_fast calls in the same order draw.  ``prefill=True`` primes
+        each job's rings from its prompt with one forward (see generate_fast).  Global conditioning is per job; a locally
+        conditioned model raises ValueError (local conditioning would need per-stream frame windows).  The model's
+        parameters must not change while the session lives (RuntimeError at the next step)."""
+        return SamplingSession(self, n_slots, prefill=prefill, return_logits=return_logits)
 
     def _per_stream_local(self, local_condition, positions, n_evals):
         """The sampler's (series, hop) for per-stream jobs (None: no local conditioning).  local_condition: an (NS, C, F)
