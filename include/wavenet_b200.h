@@ -507,6 +507,16 @@ int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond);
  * launch falls outside the window, so a long run is sampled window by window, each launch continuing through t0.  The same
  * lifetime rules as wn_gen_set_condition apply; NULL clears the table, and the last wn_gen_set_condition* call wins. */
 int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond, int frame0, int n_frames, int hop);
+/* Local conditioning with a window per stream (continuous batching: streams at their own positions): d_cond has the layout
+ * above, [n_layers][n_streams][n_frames][2D], but stream s's rows hold frames [frame0[s], frame0[s] + n_frames) of its own
+ * series; frame0 is a HOST array [n_streams], copied before the call returns.  Evaluation t of stream s reads row
+ * (t - origin) / hop - frame0[s] of its stream, origin from wn_gen_set_stream_positions (0 without positions): the frame of
+ * the stream's own position.  Per-stream windows need per-stream records: wn_gen_run returns WN_E_STATE without
+ * wn_gen_set_stream_params, and WN_E_BADARG, before launching and with t unchanged, when a stream's frames over the launch
+ * leave its window.  WN_E_BADARG for frame0[s] < 0, n_frames < 1 or hop < 1.  The lifetime rules of wn_gen_set_condition
+ * apply; NULL clears the table, and the last wn_gen_set_condition* call wins (wn_gen_set_condition_frames returns to one
+ * shared window). */
+int wn_gen_set_condition_stream_frames(wn_gen_handle* h, const float* d_cond, const int* frame0, int n_frames, int hop);
 /* Top-k and nucleus (top-p) truncation of the temperature draw, for every stream and every kernel.  Off is top_k = 0,
  * top_p = 1, which wn_gen_create starts with; the values stay on the handle until the next call.  WN_E_BADARG for
  * top_k < 0 or top_p outside (0, 1] (NaN included).  The rule, per stream and selection, on the fp32 logits l that

@@ -74,7 +74,8 @@ struct GenParams {
     const unsigned char* cl8_img;              // batched cluster kernel: fragment-ordered bf16 hi/lo weight images (cl8_pack_kernel)
     const float* cond;      // optional condition table [n_layers][NS][2D]: each stream's filter / gate biases (bf + Vf h | bg + Vg h)
     // local conditioning (cond_hop > 0): cond is a window [n_layers][NS][cond_frames][2D] of frames [cond_frame0, +cond_frames);
-    // evaluation t reads row t / cond_hop - cond_frame0.  cond_sstride = floats per stream (2D for a global table).
+    // evaluation t reads row t / cond_hop - cond_frame0 (per-stream windows: see cond_row).  cond_sstride = floats per
+    // stream (2D for a global table).
     int cond_hop, cond_frame0, cond_frames, cond_sstride;
     // top-k / nucleus truncation (wn_gen_set_truncation): trunc = 1 when the rule applies to this launch (temperature > 0
     // and a bound that drops classes); the kernels branch to choose_truncated on it and run their own selection otherwise
@@ -85,6 +86,9 @@ struct GenParams {
     // pitch of `first`, and trunc is set when any stream truncates (it only sizes kernel 1's scratch)
     const GenStream* ps;
     int head_from;
+    // with ps: each stream's local-conditioning window {cond_origin, cond_frame0} (cond_row; {0, 0} under one shared window).
+    // Kept apart from GenStream so that the kernels which never read it keep their record layout.
+    const int2* pcw;
 };
 
 // Every role of every multi-stream kernel (workers, weight producers, pusher) decides whether evaluation t runs the head
@@ -136,6 +140,21 @@ __device__ __forceinline__ int sample_of(const GenParams& p, int s, int t) {
 // This evaluation's condition table: the window row of t's frame under local conditioning (once per evaluation).
 __device__ __forceinline__ const float* cond_at(const GenParams& p, int t, int D) {
     return p.cond_hop ? p.cond + (size_t)(t / p.cond_hop - p.cond_frame0) * 2 * D : p.cond;
+}
+
+// Stream s's condition row at evaluation t, in floats from the stream's first row: under local conditioning window row
+// (t - cond_origin) / cond_hop - cond_frame0 - p.cond_frame0 with the stream's p.pcw[s] = {cond_origin, cond_frame0}
+// (wn_gen_set_condition_stream_frames: the stream's origin and first frame, p.cond_frame0 = 0; a shared window: 0 and 0),
+// t / cond_hop - p.cond_frame0 without records; 0 for a global table.  Formed once per evaluation and stream.
+template <int PS = PS_ANY>
+__device__ __forceinline__ int cond_row(const GenParams& p, int s, int t, int D) {
+    if (!p.cond_hop) return 0;
+    int q = t, f0 = p.cond_frame0;
+    if (has_records<PS>(p)) {
+        const int2 w = p.pcw[s];
+        q = t - w.x; f0 += w.y;
+    }
+    return (q / p.cond_hop - f0) * 2 * D;
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -410,7 +429,8 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
     float* pre = regB + p.regB;                // per-item results [items][NS]
     float* skacc = pre + p.pre_n;              // running skip sums of the rows this CTA owns [rows][NS]
     int* idx_s = reinterpret_cast<int*>(skacc + p.skacc_n);     // current input index per stream [NS]
-    float* prob = reinterpret_cast<float*>(idx_s + p.NS);       // [GEN_WARPS][C] softmax scratch
+    int* crow_s = idx_s + p.NS;                                 // this evaluation's condition row per stream [NS] (cond_row)
+    float* prob = reinterpret_cast<float*>(crow_s + p.NS);      // [GEN_WARPS][C] softmax scratch
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x, G = gridDim.x;
@@ -431,12 +451,12 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
 
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;                           // absolute evaluation counter == time
-        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = head_at(p, t);
-        // ---- input index of this evaluation
+        // ---- input index and condition row of this evaluation
         for (int s = tid; s < NS; s += GEN_NT) {
             int v;
             if (given_input(p, s, t, v)) idx_s[s] = v;
+            if (p.cond) crow_s[s] = cond_row(p, s, t, D);
         }
         for (int i = tid; i < nS * NS; i += GEN_NT) skacc[i] = 0.f;
         __syncthreads();
@@ -469,14 +489,15 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel(const GenParams p) {
                 const float* w = ((it & 1) ? L.wg : L.wf) + (size_t)c * K1;
                 const float* bp = (it & 1) ? L.bg : L.bf;
                 const float bias = bp ? __ldg(bp + c) : 0.f;
-                const float* cb = ct ? ct + (size_t)l * NS * p.cond_sstride + ((it & 1) ? D : 0) + c : nullptr;
+                const float* cb = p.cond ? p.cond + (size_t)l * NS * p.cond_sstride + ((it & 1) ? D : 0) + c : nullptr;
                 for (int s0 = 0; s0 < NS; s0 += SB) {
                     float acc[SB];
                     row_dot<SB>(w, regA, K1, NS, s0, lane, acc);
                     if (lane == 0) {
 #pragma unroll
                         for (int j = 0; j < SB; ++j)
-                            if (s0 + j < NS) pre[it * NS + s0 + j] = acc[j] + (cb ? __ldg(cb + (size_t)(s0 + j) * p.cond_sstride) : bias);
+                            if (s0 + j < NS)
+                                pre[it * NS + s0 + j] = acc[j] + (cb ? __ldg(cb + (size_t)(s0 + j) * p.cond_sstride + crow_s[s0 + j]) : bias);
                     }
                 }
             }
@@ -778,6 +799,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
     GenLayer* lay_s = reinterpret_cast<GenLayer*>(fullb + 8);           // per-layer table, copied from global once
     int* idx_s = reinterpret_cast<int*>(lay_s + p.n_layers);            // current input index per stream [NS]
     int* abort_s = idx_s + p.NS;
+    int* crow_s = abort_s + 1;                                          // this evaluation's condition row per stream [NS]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x, G = gridDim.x;
@@ -862,11 +884,11 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
         const int t = p.t0 + ev;
         const unsigned tag = (unsigned)t + 1u;
         const int par = t & 1;
-        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
         const bool want_head = head_at(p, t);
         for (int s = tid; s < NS; s += GEN_NT) {
             int v;
             if (given_input(p, s, t, v)) idx_s[s] = v;
+            if (p.cond) crow_s[s] = cond_row(p, s, t, D);
         }
         for (int i = tid; i < nS * NS; i += GEN_NT) skacc[i] = 0.f;
         __syncthreads();
@@ -903,7 +925,7 @@ __global__ void __launch_bounds__(GEN_NT, 1) gen_kernel_ll(const GenParams p) {
             uint2* zl = p.zLL + ((size_t)(par * NL + l) * NS) * D;
             for (int i = tid; i < nD * NS; i += GEN_NT) {
                 const int ci = i / NS, s = i - ci * NS, c = oD + ci;
-                const float* cb = ct ? ct + ((size_t)l * NS + s) * p.cond_sstride : nullptr;     // this stream's biases
+                const float* cb = p.cond ? p.cond + ((size_t)l * NS + s) * p.cond_sstride + crow_s[s] : nullptr;   // this stream's biases
                 const float f = sum_parts(2 * ci, nw, s) + (cb ? __ldg(cb + c) : (L.bf ? __ldg(L.bf + c) : 0.f));
                 const float g = sum_parts(2 * ci + 1, nw, s) + (cb ? __ldg(cb + D + c) : (L.bg ? __ldg(L.bg + c) : 0.f));
                 st_pair(zl + (size_t)s * D + c, tanh_(f) * sigmoid_(g), tag);
@@ -1667,7 +1689,7 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
     for (int ev = 0; ev < p.n_evals; ++ev) {
         const int t = p.t0 + ev;
         const unsigned rtag = (unsigned)t + 1u;                  // ring tag of time t
-        const float* ct = p.cond ? cond_at(p, t, D) : nullptr;
+        const float* ct = p.cond ? p.cond + cond_row(p, stream, t, D) : nullptr;     // this stream's row of evaluation t
         const bool want_head = head_at(p, t);
         if (tid == 0) {
             int v;
@@ -2308,8 +2330,10 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         const bool want_head = head_at(p, t);
         const bool tr_on = p.trace != nullptr && blockIdx.x == 0 && tid == 0 && ev == p.n_evals - 1;
         // FRAMES: this stream's rows of evaluation t's frame; layer l's row is l * NS * cond_sstride further
+        // (PS: the row of the finishing stream's own window)
         const float* cs_t = nullptr;
-        if constexpr (FRAMES) cs_t = cond_at(p, t, W) + (size_t)fsg * p.cond_sstride;
+        if constexpr (FRAMES && PS) cs_t = p.cond + (size_t)fsg * p.cond_sstride + (fs_on ? cond_row<PS_ON>(p, fsg, t, W) : 0);
+        else if constexpr (FRAMES) cs_t = cond_at(p, t, W) + (size_t)fsg * p.cond_sstride;
         int tr_n = 0;
 #define TR8() do { if (tr_on && tr_n < 2040) p.trace[tr_n++] = clock64(); } while (0)
         if (tr_on) p.trace[2040] = clock64();             // whole-evaluation stamps live at [2040..2047]
@@ -2631,7 +2655,8 @@ struct wn_gen_handle {
     int top_k;              // wn_gen_set_truncation (0, 1.0: off)
     double top_p;
     // wn_gen_set_stream_params: the host records (empty: the scalar path), their device copy (allocated at the first call,
-    // outside the workspace), whether it still has to be uploaded, and what wn_gen_run checks and derives from them
+    // outside the workspace; GenStream [NS] then the windows of GenParams::pcw, int2 [NS]), whether it still has to be
+    // uploaded, and what wn_gen_run checks and derives from them
     std::vector<wn_gen_stream_params> sp;
     GenStream* d_sp;
     bool sp_dirty, sp_any_trunc, sp_any_temp;
@@ -2647,6 +2672,8 @@ struct wn_gen_handle {
     std::vector<wn_gen_stream_pos> pos;
     std::vector<int> run_origin, seat_t, seat_origin;
     int seat_plain;
+    // wn_gen_set_condition_stream_frames: each stream's first window frame (empty: one window shared by all streams)
+    std::vector<int> cond_f0;
 };
 
 static int validate_shape(const wn_gen_shape* s) {
@@ -2800,7 +2827,7 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     if (p.skacc_n < 4) p.skacc_n = 4;
     p.regA = (p.regA + 3) / 4 * 4; p.regB = (p.regB + 3) / 4 * 4; p.pre_n = (p.pre_n + 3) / 4 * 4;
     p.skacc_n = (p.skacc_n + 3) / 4 * 4;
-    h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + NS + (size_t)GEN_WARPS * s->classes);
+    h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + 2 * NS + (size_t)GEN_WARPS * s->classes);
     // the grid-barrier / generic kernels stage all streams' vectors in every CTA; the cluster kernels do not
     const bool cluster_shape = s->k == 2 && s->n_layers >= 2 && s->D % CL == 0 && s->R % CL == 0 && s->S % CL == 0 &&
                                s->E % CL == 0 && s->classes % CL == 0;
@@ -2834,7 +2861,7 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
         slot = (slot + 3) / 4 * 4;
         const size_t base = sizeof(float) * ((size_t)regA_ll + p.regB + p.part_n + p.skacc_n + (size_t)GEN_WARPS * s->classes) +
                             sizeof(double) * (size_t)GEN_WARPS * s->classes + 64 + sizeof(GenLayer) * (size_t)s->n_layers +
-                            sizeof(int) * (size_t)(NS + 4);
+                            sizeof(int) * (size_t)(2 * NS + 4);
         const bool k_ok = ((s->k * s->R) % 4 == 0) && (s->D % 4 == 0) && (s->S % 4 == 0) && (s->E % 4 == 0);
         int nslots = 0;
         if (k_ok && base < (size_t)smem_optin) {
@@ -2848,7 +2875,7 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
         // regA of the LL kernel also stages the logits; keep one GenParams for both kernels
         if (regA_ll > p.regA) {
             p.regA = regA_ll;
-            h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + NS + (size_t)GEN_WARPS * s->classes);
+            h->smem = sizeof(float) * ((size_t)p.regA + p.regB + p.pre_n + p.skacc_n + 2 * NS + (size_t)GEN_WARPS * s->classes);
         }
         // ---- fast kernel eligibility (same K split as the generic kernel so both sum in the same order)
         auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
@@ -3216,8 +3243,16 @@ extern "C" int wn_gen_weights_changed(wn_gen_handle* h) {
     return 0;
 }
 
+// Leaves per-stream windows: the records' cond_origin / cond_frame0 go back to 0 at the next upload.
+static void clear_stream_frames(wn_gen_handle* h) {
+    if (h->cond_f0.empty()) return;
+    h->cond_f0.clear();
+    h->sp_dirty = true;
+}
+
 extern "C" int wn_gen_set_condition(wn_gen_handle* h, const float* d_cond) {
     WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_condition: null handle");
+    clear_stream_frames(h);
     h->base.cond = d_cond;
     h->base.cond_hop = h->base.cond_frame0 = 0;
     h->base.cond_frames = 1;
@@ -3230,9 +3265,29 @@ extern "C" int wn_gen_set_condition_frames(wn_gen_handle* h, const float* d_cond
     if (d_cond == nullptr) return wn_gen_set_condition(h, nullptr);
     WN_REQUIRE(frame0 >= 0 && n_frames >= 1 && hop >= 1, WN_E_BADARG,
                "wn_gen_set_condition_frames: bad window (frame0 %d, %d frames, hop %d)", frame0, n_frames, hop);
+    clear_stream_frames(h);
     h->base.cond = d_cond;
     h->base.cond_hop = hop; h->base.cond_frame0 = frame0; h->base.cond_frames = n_frames;
     h->base.cond_sstride = n_frames * 2 * h->shape.D;
+    return 0;
+}
+
+extern "C" int wn_gen_set_condition_stream_frames(wn_gen_handle* h, const float* d_cond, const int* frame0, int n_frames,
+                                                  int hop) {
+    WN_REQUIRE(h, WN_E_STATE, "wn_gen_set_condition_stream_frames: null handle");
+    if (d_cond == nullptr) return wn_gen_set_condition(h, nullptr);
+    WN_REQUIRE(frame0 && n_frames >= 1 && hop >= 1, WN_E_BADARG,
+               "wn_gen_set_condition_stream_frames: bad window (%d frames, hop %d, frame0 %s)", n_frames, hop,
+               frame0 ? "set" : "null");
+    const int NS = h->shape.n_streams;
+    for (int s = 0; s < NS; ++s)
+        WN_REQUIRE(frame0[s] >= 0, WN_E_BADARG, "wn_gen_set_condition_stream_frames: stream %d: frame0 %d must be >= 0", s,
+                   frame0[s]);
+    h->base.cond = d_cond;
+    h->base.cond_hop = hop; h->base.cond_frame0 = 0; h->base.cond_frames = n_frames;   // the records carry the windows
+    h->base.cond_sstride = n_frames * 2 * h->shape.D;
+    h->cond_f0.assign(frame0, frame0 + NS);
+    h->sp_dirty = true;
     return 0;
 }
 
@@ -3278,7 +3333,7 @@ extern "C" int wn_gen_set_stream_params(wn_gen_handle* h, const wn_gen_stream_pa
         h->sp_any_temp = h->sp_any_temp || q.temperature > 0.f;
     }
     if (NS > 1) {                                           // one stream: wn_gen_run folds the record into the scalars
-        if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, sizeof(GenStream) * (size_t)NS));
+        if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, (sizeof(GenStream) + sizeof(int2)) * (size_t)NS));
     }
     h->sp_dirty = true;
     return 0;
@@ -3298,7 +3353,7 @@ extern "C" int wn_gen_set_stream_positions(wn_gen_handle* h, const wn_gen_stream
         WN_REQUIRE(pos[s].sample0 >= 0 && pos[s].first0 >= 0, WN_E_BADARG,
                    "wn_gen_set_stream_positions: stream %d: sample0 %d and first0 %d must be >= 0", s, pos[s].sample0,
                    pos[s].first0);
-    if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, sizeof(GenStream) * (size_t)NS));
+    if (h->d_sp == nullptr) WN_CUDA(cudaMalloc(&h->d_sp, (sizeof(GenStream) + sizeof(int2)) * (size_t)NS));
     h->pos.assign(pos, pos + NS);
     h->sp_dirty = true;
     return 0;
@@ -3377,8 +3432,22 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
                    "wn_gen_run: the first evaluation of newly seated stream %d must read a prompt sample", s);
     }
     WN_REQUIRE(!(a->temperature > 0.f) || a->d_uniforms, WN_E_BADARG, "wn_gen_run: temperature > 0 needs d_uniforms");
+    const bool stream_frames = !h->cond_f0.empty();
+    WN_REQUIRE(!stream_frames || per_stream, WN_E_STATE,
+               "wn_gen_run: per-stream condition windows need per-stream records (wn_gen_set_stream_params)");
     if (a->n_evals == 0) return 0;
-    if (h->base.cond && h->base.cond_hop) {
+    if (stream_frames) {
+        // per stream: the frames of positions [q0, q0 + n_evals) inside its own window
+        const int hop = h->base.cond_hop, nf = h->base.cond_frames;
+        for (int s = 0; s < NS; ++s) {
+            const int origin = positions ? h->pos[s].origin : 0;
+            const long long q0 = (long long)a->t0 - origin, q1 = q0 + a->n_evals - 1;
+            const long long f_lo = q0 / hop, f_hi = q1 / hop;
+            WN_REQUIRE(f_lo >= h->cond_f0[s] && f_hi < (long long)h->cond_f0[s] + nf, WN_E_BADARG,
+                       "wn_gen_run: stream %d at positions [%lld, %lld) reads frames %lld..%lld, its window holds [%d, %d)", s,
+                       q0, q1 + 1, f_lo, f_hi, h->cond_f0[s], h->cond_f0[s] + nf);
+        }
+    } else if (h->base.cond && h->base.cond_hop) {
         const int f_lo = a->t0 / h->base.cond_hop, f_hi = (a->t0 + a->n_evals - 1) / h->base.cond_hop;
         WN_REQUIRE(f_lo >= h->base.cond_frame0 && f_hi < h->base.cond_frame0 + h->base.cond_frames, WN_E_BADARG,
                    "wn_gen_run: evaluations [%d,%d) read frames [%d,%d], outside the condition window [%d,%d)", a->t0,
@@ -3406,16 +3475,19 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
     const bool records = per_stream && (h->shape.n_streams > 1 || positions);
     if (records && h->sp_dirty) {
         // in stream order, so that a launch still reading the previous records finishes first
-        std::vector<GenStream> recs(h->sp.size());
-        for (size_t s = 0; s < recs.size(); ++s) {
+        const size_t NSr = h->sp.size();
+        std::vector<GenStream> recs(NSr + (NSr * sizeof(int2) + sizeof(GenStream) - 1) / sizeof(GenStream));
+        int2* wins = reinterpret_cast<int2*>(recs.data() + NSr);
+        for (size_t s = 0; s < NSr; ++s) {
             const wn_gen_stream_params& q = h->sp[s];
             recs[s].n_given = q.n_given; recs[s].top_k = q.top_k; recs[s].trunc = stream_truncates(q, h->shape.classes);
             recs[s].temperature = q.temperature; recs[s].regularize = q.regularize; recs[s].top_p = q.top_p;
             recs[s].origin = positions ? h->pos[s].origin : 0;
             recs[s].sample0 = positions ? h->pos[s].sample0 : 0;
             recs[s].first0 = positions ? h->pos[s].first0 : 0;
+            wins[s] = make_int2(stream_frames && positions ? h->pos[s].origin : 0, stream_frames ? h->cond_f0[s] : 0);
         }
-        WN_CUDA(cudaMemcpyAsync(h->d_sp, recs.data(), sizeof(GenStream) * recs.size(), cudaMemcpyHostToDevice, st));
+        WN_CUDA(cudaMemcpyAsync(h->d_sp, recs.data(), (sizeof(GenStream) + sizeof(int2)) * NSr, cudaMemcpyHostToDevice, st));
         WN_CUDA(cudaStreamSynchronize(st));                   // recs is pageable host memory that dies with this scope
         h->sp_dirty = false;
     }
@@ -3432,14 +3504,16 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         p.t0 = a->t0 + done; p.n_evals = n; p.temperature = a->temperature; p.regularize = a->regularize;
         p.top_k = h->top_k; p.top_p = h->top_p;
         p.trunc = a->temperature > 0.f && ((h->top_k > 0 && h->top_k < h->shape.classes) || h->top_p < 1.0);
-        p.ps = nullptr;
+        p.ps = nullptr; p.pcw = nullptr;
         p.head_from = head_from;
         if (per_stream && !records) {                          // the single record becomes the scalars (kernel 3 reads only those)
             const wn_gen_stream_params& q = h->sp[0];
             p.temperature = q.temperature; p.regularize = q.regularize; p.top_k = q.top_k; p.top_p = q.top_p;
             p.trunc = stream_truncates(q, h->shape.classes);
+            if (stream_frames) p.cond_frame0 = h->cond_f0[0];  // and its window the shared one (origin 0 without positions)
         } else if (records) {
             p.ps = h->d_sp;
+            p.pcw = reinterpret_cast<const int2*>(h->d_sp + h->shape.n_streams);
             p.trunc = h->sp_any_trunc;                          // sizes kernel 1's truncation scratch; the records decide
         }
         WN_CUDA(cudaMemsetAsync(p.bar, 0, sizeof(unsigned), st));

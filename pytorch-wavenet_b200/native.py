@@ -218,6 +218,7 @@ SIGNATURES = {
     "wn_gen_weights_changed": (C.c_int, [C.c_void_p]),
     "wn_gen_set_condition": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wn_gen_set_condition_frames": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3),
+    "wn_gen_set_condition_stream_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_int]),
     "wn_gen_set_truncation": (C.c_int, [C.c_void_p, C.c_int, C.c_double]),
     "wn_gen_set_stream_params": (C.c_int, [C.c_void_p, C.POINTER(GenStreamParams)]),
     "wn_gen_set_stream_positions": (C.c_int, [C.c_void_p, C.POINTER(GenStreamPos)]),

@@ -197,11 +197,11 @@ class _Packs:
                                                   None, None, C, D, 1, out[i].data_ptr(), bias.data_ptr(), stream), "pack local U")
         return out
 
-    def cond_table_frames(self, h, y, f0, n_frames, stream):
+    def cond_table_frames(self, h, y, f0, n_frames, stream, out=None):
         """Condition table [n_layers][N][n_frames][2D] of a locally conditioned model (wn_cond_table_frames) for frames
         [f0, f0 + n_frames) of the (N, C, F) fp32 series ``y``, with the (N, G) condition rows ``h`` of a globally conditioned
         one (else None): bf + Vf h + Uf y_f | bg + Vg h + Ug y_f for every item and frame.  The global part is the global
-        table (cond_table), built once per item."""
+        table (cond_table), built once per item.  ``out``: a contiguous fp32 tensor of that shape to build it into."""
         rt, lib, m = self.rt, native.lib(), self.rt.model
         nl, D = m.layers * m.blocks, m.dilation_channels
         P = rt._params()
@@ -213,7 +213,10 @@ class _Packs:
             cached = (key, torch.tensor(rows, dtype=torch.int64, device=rt.device()))
             rt._lcond_ptr_cache = cached
         N, C, F = y.shape
-        out = torch.empty(nl, N, n_frames, 2 * D, device=rt.device(), dtype=torch.float32)
+        if out is None:
+            out = torch.empty(nl, N, n_frames, 2 * D, device=rt.device(), dtype=torch.float32)
+        elif tuple(out.shape) != (nl, N, n_frames, 2 * D) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise RuntimeError(f"wavenet_b200: a condition table of shape {tuple(out.shape)} for {N} items x {n_frames} frames")
         native.check(lib.wn_cond_table_frames(cached[1].data_ptr(), self["local_u"].data_ptr(), nl, D, native.ptr(base), C,
                                               y.data_ptr() + 4 * f0, F, N, n_frames, out.data_ptr(), stream),
                      "local condition table")
@@ -1280,10 +1283,11 @@ class _Runtime:
 class _Job:
     """One submitted sampling job of a SamplingSession and what it has produced so far."""
 
-    def __init__(self, jid, prompt, count, temperature, regularize, top_k, top_p, cond, uniforms):
+    def __init__(self, jid, prompt, count, temperature, regularize, top_k, top_p, cond, uniforms, local=None):
         self.id, self.prompt, self.count = jid, prompt, count
         self.temperature, self.regularize, self.top_k, self.top_p = temperature, regularize, top_k, top_p
         self.cond, self.uniforms = cond, uniforms
+        self.local = local              # (C, F) device series the sampler reads (learned upsampler: its hop-1 features)
         self.idx, self.logits = [], []
         self.made = 0
 
@@ -1299,17 +1303,24 @@ class SamplingSession:
     An empty slot runs a parked temperature-0 job whose outputs are discarded.  Each job gives, bit for bit, what a
     generate_fast_batch launch of the same slot count carrying that job in every stream gives, with the same uniforms and
     the same ``prefill``.  The session owns its handle: generate_fast* calls on the model never touch it.  Global
-    conditioning is per job; local conditioning is not supported (it would need per-stream frame windows)."""
+    conditioning is per job.  Local conditioning is per job too: every slot reads its own frame window, indexed by its own
+    position (wn_gen_set_condition_stream_frames); a step runs in launches of at most ``local_window`` evaluations, and
+    before each one the slots' windows are gathered from their jobs' series and built into one table buffer allocated at
+    creation (_session_windows)."""
 
     _T_MAX = 2 ** 31 - 1
 
-    def __init__(self, model, n_slots, prefill=False, return_logits=False):
+    def __init__(self, model, n_slots, prefill=False, return_logits=False, local_window=None):
         if isinstance(n_slots, (bool, np.bool_)) or not isinstance(n_slots, (int, np.integer)) or n_slots < 1:
             raise ValueError(f"n_slots must be an integer >= 1, got {n_slots!r}")
         _check_prefill(prefill)
-        if getattr(model, "local_condition_channels", 0):
-            raise ValueError("sampling sessions do not support local conditioning (it would need per-stream frame windows); "
-                             "use generate_fast_batch")
+        self.Cl = getattr(model, "local_condition_channels", 0)
+        if self.Cl:
+            if isinstance(local_window, (bool, np.bool_)) or not isinstance(local_window, (int, np.integer)) or local_window < 1:
+                raise ValueError("a locally conditioned model needs local_window= (an integer >= 1: the evaluations one "
+                                 f"condition-table build covers per slot), got {local_window!r}")
+        elif local_window is not None:
+            raise ValueError("local_window applies to a locally conditioned model only (this one has local_condition_channels=0)")
         self.model, self.n_slots, self.prefill, self.return_logits = model, int(n_slots), prefill, bool(return_logits)
         self.rt = rt = model._runtime()
         self.dev = rt.device()
@@ -1322,8 +1333,19 @@ class SamplingSession:
         with torch.cuda.device(self.dev):
             self.s = rt.new_sampler(self.n_slots)
             self.G = getattr(model, "condition_channels", 0)
-            self.ctab = None
-            if self.G:                                 # rows of parked slots: the zero condition (the biases)
+            self.ctab = self.hrows = None
+            if self.Cl:
+                # one table buffer for the session: n_layers x n_slots x nf x 2D floats (see sampling_session)
+                self.window = int(local_window)
+                self.hop = 1 if getattr(model, "local_upsample", None) is not None else model.local_condition_hop
+                self.nf = _session_frames(self.window, self.hop)
+                nl, D = model.layers * model.blocks, model.dilation_channels
+                f32 = dict(device=self.dev, dtype=torch.float32)
+                self.ltab = torch.empty(nl, self.n_slots, self.nf, 2 * D, **f32)
+                self.ywin = torch.zeros(self.n_slots, self.Cl, self.nf, **f32)     # the slots' gathered frames
+                if self.G:                             # each slot's global condition row (parked: zero)
+                    self.hrows = torch.zeros(self.n_slots, self.G, **f32)
+            elif self.G:                               # rows of parked slots: the zero condition (the biases)
                 stream = torch.cuda.current_stream(self.dev).cuda_stream
                 zero = torch.zeros(self.n_slots, self.G, device=self.dev, dtype=torch.float32)
                 self.ctab = rt.packed_weights(stream).cond_table(zero, stream)
@@ -1358,10 +1380,12 @@ class SamplingSession:
         self.seated = [False] * self.n_slots
 
     def submit(self, first_samples, num_samples, temperature=1., regularize=0., top_k=0, top_p=1.0, condition=None,
-               uniforms=None):
-        """Queue one job: generate_fast(num_samples, first_samples, temperature, regularize, top_k=, top_p=, condition=)
-        with ``uniforms`` (num_samples,) float64 for its draws; None draws them from numpy's global RNG now when
-        temperature > 0.  Returns the job id.  ValueError for a malformed argument, before any device work."""
+               uniforms=None, local_condition=None):
+        """Queue one job: generate_fast(num_samples, first_samples, temperature, regularize, top_k=, top_p=, condition=,
+        local_condition=) with ``uniforms`` (num_samples,) float64 for its draws; None draws them from numpy's global RNG
+        now when temperature > 0.  ``local_condition``: a locally conditioned model's (C, F) series for this job, F >=
+        ceil((n_given - 1 + num_samples) / hop) (required there, refused elsewhere); a learned upsampler runs on it here, at
+        the job's own length.  Returns the job id.  ValueError for a malformed argument, before any device work."""
         if torch.is_tensor(first_samples):
             first_samples = first_samples.detach().cpu().numpy()
         prompt = np.asarray(first_samples)
@@ -1379,10 +1403,21 @@ class SamplingSession:
             uniforms = u[:count].copy()
         else:
             uniforms = None
+        positions = plan.n_given[0] - 1 + count
+        if local_condition is not None:
+            local_condition = local_condition[None] if torch.is_tensor(local_condition) else np.asarray(local_condition)[None]
+        y = self.model._local_condition(local_condition, 1, positions)
+        if y is not None and count > 0:
+            # as _per_stream_local: a learned upsampler runs on the job alone, at its own length
+            with torch.no_grad(), torch.cuda.device(self.dev):
+                y = y.detach()
+                if getattr(self.model, "local_upsample", None) is not None:
+                    y = self.model._upsample(y, positions)
+                y = y[0].contiguous()
         jid = self.next_id
         self.next_id += 1
         job = _Job(jid, plan.first[0, :plan.n_given[0]].copy(), count, plan.temperature[0], plan.regularize[0],
-                   plan.top_k[0], plan.top_p[0], cond, uniforms)
+                   plan.top_k[0], plan.top_p[0], cond, uniforms, local=y)
         self.jobs[jid] = job
         self.queue.append(job)
         return jid
@@ -1425,7 +1460,9 @@ class SamplingSession:
                 zeros.append(b)
             else:
                 primed.setdefault(T, []).append((b, job))    # windows line up: one forward per prompt length
-            if job is not None and job.cond is not None:
+            if self.hrows is not None:
+                self.hrows[b] = 0.0 if job is None else job.cond[0]
+            elif job is not None and job.cond is not None:
                 self.ctab[:, b, :] = self.rt.packed_weights(stream).cond_table(job.cond, stream)[:, 0, :]
             self.seated[b] = True
         if zeros:
@@ -1438,22 +1475,71 @@ class SamplingSession:
             sl = (ctypes.c_int * len(slots))(*slots)
             qe = (ctypes.c_int * len(slots))(*([T] * len(slots)))
             d_first = torch.from_numpy(np.stack([j.prompt for _, j in group]).astype(np.int32)).to(self.dev)
-            cond = ctab = None
+            cond = ctab = local = None
             if self.G:
                 cond = torch.cat([j.cond for _, j in group])
                 ctab = self.rt.packed_weights(stream).cond_table(cond, stream)
+            if self.Cl:
+                # each job's own series, zero-padded to the frames the prompt window reads
+                P0, _, W = prefill_window(T, [d for d, _ in self.model.dilations], self.model.kernel_size, self.hop)
+                width = max(P0 // self.hop + -(-W // self.hop), max(j.local.shape[1] for _, j in group))
+                y = torch.zeros(len(group), self.Cl, width, device=self.dev, dtype=torch.float32)
+                for i, (_, j) in enumerate(group):
+                    y[i, :, :j.local.shape[1]] = j.local
+                local = (y, self.hop)
 
             def scatter(layer, src, layout, L, st, sl=sl, qe=qe, n=len(slots)):
                 native.check(lib.wn_gen_seat_layer(h, layer, n, sl, qe, src, layout, L, L, st), f"seat layer {layer}")
-            self.rt.prefill_forward(d_first, T, scatter, cond=cond, ctab=ctab)
+            self.rt.prefill_forward(d_first, T, scatter, cond=cond, ctab=ctab, local=local)
 
     def _step(self, n_evals):
-        lib, h = native.lib(), self.s["handle"]
         stream = torch.cuda.current_stream(self.dev).cuda_stream
         seats = _session_admit(self.slot_job, self.seated, self.queue)
         if seats:
             self._seat(seats, stream)
-        NS, t = self.n_slots, self.t
+        if not self.Cl:
+            out = self._launch(self.t, n_evals, stream)
+        else:
+            got = []
+            for t0, n, frame0 in _session_windows(self.t, n_evals, self.origin, self.hop, self.window):
+                self._set_windows(frame0, stream)
+                got.append(self._launch(t0, n, stream))
+            out = {}
+            for part in got:                                 # a job's samples of the step, launch after launch
+                for jid, v in part.items():
+                    out.setdefault(jid, []).append(v)
+            cat = lambda vs: np.concatenate(vs) if len(vs) > 1 else vs[0]
+            out = {jid: ((cat([v[0] for v in vs]), cat([v[1] for v in vs])) if self.return_logits else cat(vs))
+                   for jid, vs in out.items()}
+        for b in range(self.n_slots):                        # done jobs give their slot to the next step's admission
+            job = self.slot_job[b]
+            if job is not None and job.made >= job.count:
+                self.slot_job[b] = None
+                self.seated[b] = False
+        return out
+
+    def _set_windows(self, frame0, stream):
+        """Slot b's window: frames [frame0[b], frame0[b] + nf) of its job's series (zeros for a parked slot and past the
+        series' end: only discarded outputs read those), built into the session's table buffer and set on the handle.
+        The build is ordered on the stream after the previous launch, which still reads the buffer, so one buffer serves
+        every launch."""
+        lib, h, nf = native.lib(), self.s["handle"], self.nf
+        self.ywin.zero_()
+        for b, job in enumerate(self.slot_job):
+            if job is None:
+                continue
+            f0, F = frame0[b], job.local.shape[1]
+            if f0 < F:
+                self.ywin[b, :, :min(nf, F - f0)] = job.local[:, f0:f0 + nf]
+        self.rt.packed_weights(stream).cond_table_frames(self.hrows, self.ywin, 0, nf, stream, out=self.ltab)
+        f0s = (ctypes.c_int * self.n_slots)(*frame0)
+        native.check(lib.wn_gen_set_condition_stream_frames(h, self.ltab.data_ptr(), f0s, nf, self.hop),
+                     "session local condition")
+
+    def _launch(self, t, n_evals, stream):
+        """One launch of every slot over evaluations [t, t + n_evals): {job_id: new indices [, logits]}."""
+        lib, h = native.lib(), self.s["handle"]
+        NS = self.n_slots
         recs, pos, first, uni, plans = _session_records(t, n_evals, self.slot_job, self.origin)
         native.check(lib.wn_gen_set_stream_params(h, recs), "session stream params")
         native.check(lib.wn_gen_set_stream_positions(h, pos), "session positions")
@@ -1484,11 +1570,6 @@ class SamplingSession:
                 out[job.id] = (new, lg)
             else:
                 out[job.id] = new
-        for b in range(NS):                                  # done jobs give their slot to the next step's admission
-            job = self.slot_job[b]
-            if job is not None and job.made >= job.count:
-                self.slot_job[b] = None
-                self.seated[b] = False
         return out
 
 
@@ -1510,6 +1591,24 @@ def _session_admit(slot_job, seated, queue):
             continue
         seats.append((b, nxt))
     return seats
+
+
+def _session_frames(window, hop):
+    """Frames one slot's table window holds: any run of ``window`` consecutive positions touches at most
+    ceil((window - 1) / hop) + 1 frames of ``hop`` positions."""
+    return -(-(window - 1) // hop) + 1
+
+
+def _session_windows(t, n_evals, origin, hop, window):
+    """The launches of a session step of n_evals evaluations from time t under local conditioning: [(t0, n, frame0)], each
+    at most ``window`` evaluations, frame0[b] = q0 // hop the first frame of slot b (origin[b]) at its position q0 = t0 -
+    origin[b].  Its positions [q0, q0 + n) then read frames [frame0[b], frame0[b] + _session_frames(window, hop))."""
+    out = []
+    while n_evals > 0:
+        n = min(window, n_evals)
+        out.append((t, n, [(t - o) // hop for o in origin]))
+        t, n_evals = t + n, n_evals - n
+    return out
 
 
 def _session_records(t, n_evals, slot_job, origin):
@@ -2199,18 +2298,27 @@ class WaveNetModel(nn.Module):
             logits = logits[:, :plan.counts[0]] if return_logits else None
         return (idx, logits) if return_logits else idx
 
-    def sampling_session(self, n_slots, prefill=False, return_logits=False):
+    def sampling_session(self, n_slots, prefill=False, return_logits=False, local_window=None):
         """Continuous batching: a SamplingSession of ``n_slots`` streams on its own sampler handle.  ``submit(first_samples,
-        num_samples, temperature=1., regularize=0., top_k=0, top_p=1.0, condition=None, uniforms=None)`` queues a job and
-        returns its id; ``step(n_evals)`` seats queued jobs into free slots, runs n_evals evaluations of every slot and
-        returns {job_id: new indices} (with return_logits: {job_id: (indices, logits)}); ``result(job_id)`` gives a done
-        job's output; ``pending`` / ``active`` count queued and running jobs.  Each job gives, bit for bit, what a
-        generate_fast_batch call of n_slots copies of that job gives (same uniforms, same prefill); with uniforms=None a
-        seeded sequence of submits draws what seeded generate_fast calls in the same order draw.  ``prefill=True`` primes
-        each job's rings from its prompt with one forward (see generate_fast).  Global conditioning is per job; a locally
-        conditioned model raises ValueError (local conditioning would need per-stream frame windows).  The model's
-        parameters must not change while the session lives (RuntimeError at the next step)."""
-        return SamplingSession(self, n_slots, prefill=prefill, return_logits=return_logits)
+        num_samples, temperature=1., regularize=0., top_k=0, top_p=1.0, condition=None, uniforms=None,
+        local_condition=None)`` queues a job and returns its id; ``step(n_evals)`` seats queued jobs into free slots, runs
+        n_evals evaluations of every slot and returns {job_id: new indices} (with return_logits: {job_id: (indices,
+        logits)}); ``result(job_id)`` gives a done job's output; ``pending`` / ``active`` count queued and running jobs.  Each
+        job gives, bit for bit, what a generate_fast_batch call of n_slots copies of that job gives (same uniforms, same
+        prefill); with uniforms=None a seeded sequence of submits draws what seeded generate_fast calls in the same order
+        draw.  ``prefill=True`` primes each job's rings from its prompt with one forward (see generate_fast).  Global
+        conditioning is per job.  The model's parameters must not change while the session lives (RuntimeError at the next
+        step).
+
+        A locally conditioned model (a vocoder) needs ``local_window``, an int >= 1, and every job its own (C, F) series
+        (``submit(..., local_condition=y)``); ValueError otherwise, and for ``local_window`` on any other model.  Each slot
+        reads its own frames at its own position.  A step runs in launches of at most ``local_window`` evaluations, each
+        after one table build of every slot's nf = ceil((local_window - 1) / hop) + 1 frames (hop 1 under a learned
+        upsampler: nf = local_window) into one buffer of n_layers x n_slots x nf x 2 x dilation_channels floats, allocated
+        here.  On the cfg-2 net (50 layers of 256 dilation channels): 64 slots at hop 80 and local_window 1 000 take about
+        90 MB; 64 slots of a learned upsampler at local_window 64 about 420 MB.  A larger window builds less often and
+        holds more memory."""
+        return SamplingSession(self, n_slots, prefill=prefill, return_logits=return_logits, local_window=local_window)
 
     def _per_stream_local(self, local_condition, positions, n_evals):
         """The sampler's (series, hop) for per-stream jobs (None: no local conditioning).  local_condition: an (NS, C, F)
