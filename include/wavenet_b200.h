@@ -474,20 +474,22 @@ typedef struct wn_gen_run_args {
 int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stream);
 int wn_gen_destroy(wn_gen_handle* h);
 /* Which sampler kernel runs (all implement the same schedule; call right after wn_gen_reset):
- *   0  auto: 256-wide k = 2 nets -> the tensor-core cluster kernel 6, for any number of streams;
+ *   0  auto: 256- and 512-wide k = 2 nets of 256 classes -> the tensor-core cluster kernel 6, for any number of streams;
  *            other nets: one stream -> the single-stream L2 kernel 3, several streams -> one cluster per stream
  *            (kernel 4) where it applies, otherwise the generic kernel
  *   1  atomic grid barrier between stages (the simple reference kernel)
  *   2  generic flag-in-data exchange through L2 (any shape, any number of streams)
  *   3  single-stream L2 kernel with register-free cooperative polling (k = 2, power-of-two row split)
  *   4  cluster kernel: one 16-CTA thread-block cluster per stream, exchange through distributed shared memory
- *   6  tensor-core cluster kernel: up to 8 streams per thread-block cluster (256-wide nets: R = D = S = E = classes = 256,
- *      k = 2).  The weights of a stage enter shared memory once per 8 streams, as bf16 hi/lo pairs pre-split into MMA
- *      fragment order at wn_gen_reset (wn_gen_workspace_bytes includes the images; wn_gen_weights_changed after in-place
- *      weight updates); dot products are mma.sync m16n8k16 with three MMAs per product (fp32-class: ~1e-6 on the
- *      logits); the exchange is one 512-byte st.async.v4 block per destination CTA, credited to an mbarrier there.
- *      Clusters of 16 CTAs while all of them are co-resident (as reported by the occupancy query), else clusters of 8
- *      CTAs that own two 16-channel slices each (more clusters per wave); wn_gen_create fixes the size
+ *   6  tensor-core cluster kernel: up to 8 streams per thread-block cluster (R = D = S = E = W with W = 256 or 512,
+ *      classes = 256, k = 2).  The weights of a stage enter shared memory once per 8 streams, as bf16 hi/lo pairs
+ *      pre-split into MMA fragment order at wn_gen_reset (wn_gen_workspace_bytes includes the images: 1.5 MB per layer
+ *      at W = 256, 6 MB per layer at W = 512, so about 505 MB for an 80-layer 512-wide net, per handle;
+ *      wn_gen_weights_changed after in-place weight updates); dot products are mma.sync m16n8k16 with three MMAs per
+ *      product (fp32-class: ~1e-6 on the logits); the exchange is one 512-byte st.async.v4 block per destination CTA,
+ *      credited to an mbarrier there.  W = 256: clusters of 16 CTAs while all of them are co-resident (as reported by
+ *      the occupancy query), else clusters of 8 CTAs that own two 16-channel slices each (more clusters per wave);
+ *      wn_gen_create fixes the size.  W = 512: clusters of 16 CTAs that own two 16-channel slices each
  * WN_E_BADARG for any other mode (5 included), WN_E_UNSUPP for a kernel that does not apply to the shape.
  * Kernels 2 and 3 sum in the same order (bit-identical results); kernel 4 splits rows differently (rounding-level
  * differences). */

@@ -1909,11 +1909,12 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
 }
 
 // ================================================================================================ batched cluster kernel
-// Tensor-core sampler for 256-wide nets (R = D = S = E = classes = 256, k = 2), one stream or many: a thread-block cluster
-// advances up to CL8_SB = 8 independent streams together, so the weights of a stage enter shared memory ONCE per 8 streams
-// and step (gen_kernel_cluster streams all 79 MB per stream and step; only 7 of its clusters are co-resident, so 64 streams
-// ran as waves).  Every exchanged vector is 16 blocks of 16 channels x 8 streams; a CTA owns one block (clusters of 16) or
-// two (clusters of 8) and computes those rows of every stage for all 8 streams:
+// Tensor-core sampler for nets of width W = 256 or 512 (R = D = S = E = W, classes = 256, k = 2), one stream or many: a
+// thread-block cluster advances up to CL8_SB = 8 independent streams together, so the weights of a stage enter shared
+// memory ONCE per 8 streams and step (gen_kernel_cluster streams all 79 MB per stream and step; only 7 of its clusters are
+// co-resident, so 64 streams ran as waves).  Every exchanged vector is W / 16 blocks ("virtual ranks") of 16 channels x 8
+// streams; a CTA owns one block (W = 256, clusters of 16) or two (W = 256, clusters of 8; W = 512, clusters of 16) and
+// computes those rows of every stage for all 8 streams:
 //   * the dot products are mma.sync m16n8k16 (M = 16 rows of the stage, N = the 8 streams, K = 16 input channels = one
 //     block) with bf16 hi/lo operand pairs -- x = hi + lo up to 2^-17 relative, three MMAs per product (lo.hi, hi.lo, hi.hi
 //     on independent accumulators), fp32 accumulation: the scheme of the training kernels (tc_block.cu).  Weights are
@@ -1924,17 +1925,20 @@ __global__ void __launch_bounds__(GEN_NT + 32, 1) gen_kernel_cluster(const GenPa
 //   * exchange: a pusher warp reads a staged 512-byte block back and issues ONE st.async.v4 per destination CTA, crediting
 //     the bytes to an mbarrier there; consumers sleep on their own mbarrier; tools/dsmem_probe.cu compares this (H) with a bulk
 //     copy per destination (F) and per-lane stores (E);
-//   * weights: producer warp(s) keep a 128 KB ring of images full (bulk copies; cp.async for the second block of an 8-CTA
-//     cluster's CTA);
+//   * weights: producer warp(s) keep a ring of images full (bulk copies; cp.async for the second half of a CTA's image when
+//     it owns two blocks): 128 KB of whole stages at W = 256; at W = 512 a stage's image doubles with K and the vectors
+//     double too, so the ring is 2 x 32 KB and carries every stage in K-chunks (CL8 chunk constants below);
 //   * history: the {value, tag} fp32 ring of the other kernels (same layout: sessions, queue export and kernel switches keep
 //     working), written by the owning CTA, fetched one stage ahead into registers, validated by tag, split on arrival.
 // Streams never mix (N is the stream index of the MMA) and both cluster sizes add in the same order: a stream's indices and
 // logits do not depend on how many streams run beside it, bit for bit.
 constexpr int CL8_SB = 8;               // streams per cluster
-constexpr int CL8_W = 256;              // the width this kernel is specialised for
+constexpr int CL8_C = 256;              // classes of every net this kernel serves
 constexpr int CL8_BLK = 512;            // bytes of one (source CTA) block of an exchanged vector: 8 streams x 16 channels x (hi, lo)
-constexpr int CL8_VEC = CL * CL8_BLK;   // bytes of one exchanged vector in every CTA
-constexpr int CL8_IMG1 = 2 * 32 * 1024, CL8_IMG2 = 2 * 16 * 1024, CL8_IMGH = 16 * 1024;    // weight images per (layer, rank) / head stage
+constexpr int CL8_IMGH = 16 * 1024;     // one virtual rank's chunk of an end_conv_1 image: 16 k-steps of one m-tile
+// k-steps of one ring chunk of a layer stage (both m-tiles of a virtual rank): the whole K = 256 at W = 256, a quarter of
+// K = 512 at W = 512 (so that a CTA's chunk, 2 x 16 KB, fits a 32 KB slot)
+__host__ __device__ constexpr int cl8_ksc(int W) { return W == 256 ? 16 : 8; }
 // byte offset of the (hi pair | lo pair) unit of channels (c & ~1, c | 1) of stream s inside a block: per stream 64 bytes =
 // 4 x [unit t | unit t+4], the order in which lane (g = stream, t) of an m16n8k16 B fragment consumes them
 __device__ __forceinline__ int cl8_unit_off(int s, int c) {
@@ -1978,14 +1982,18 @@ __device__ __forceinline__ unsigned mapa_u32(unsigned laddr, unsigned dst) {
 
 // Weight images.  One (m-tile, k-step) = 1 KB: [hi: 32 lanes x 16 B][lo: 32 lanes x 16 B], lane's 16 bytes = the A fragment
 // registers a0..a3 of m16n8k16: a_j covers row g + 8*(j&1), k pair 2t + 8*(j>>1) (g = lane>>2, t = lane&3).
-//   layout [layer][kind][virtual rank 0-15][32 KB image = [m-tile][k-step 0-15][hi | lo]], kind 0 = stage 1, tap 0 (old;
-//   m-tile 0 = filter rows, 1 = gate rows; k-step = channel block), 1 = stage 1, tap 1 (current), 2 = stage 2 (m-tile 0 =
-//   residual rows, 1 = skip rows; k-step = z block); then [end_conv_1 | end_conv_2][virtual rank][16 KB: one m-tile].
-//   The images of consecutive virtual ranks are adjacent, so a CTA that owns VR of them fetches a stage with ONE copy.
+//   layout [layer][kind][chunk][virtual rank 0..W/16-1][image = [m-tile][k-step 0..KSC-1][hi | lo]], kind 0 = stage 1, tap
+//   0 (old; m-tile 0 = filter rows, 1 = gate rows; k-step = channel block), 1 = stage 1, tap 1 (current), 2 = stage 2
+//   (m-tile 0 = residual rows, 1 = skip rows; k-step = z block); chunk c holds k-steps c*KSC .. c*KSC+KSC-1 (KSC =
+//   cl8_ksc(W): one 32 KB chunk per virtual rank at W = 256, four of 16 KB at W = 512).  Then end_conv_1 as
+//   [chunk of 16 k-steps][virtual rank][16 KB: one m-tile] and end_conv_2 as [virtual rank 0-15][one m-tile, all W/16
+//   k-steps] (at W = 256 both are [virtual rank][16 KB]).  The images of consecutive virtual ranks are adjacent, so a CTA
+//   that owns VR of them fetches a chunk with ONE copy.
+template <int W>
 __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const float* e1w, const float* e2w, unsigned* img) {
-    const int W = CL8_W;
-    constexpr size_t IW = CL8_IMG2 / 4, HW = CL8_IMGH / 4;          // words per layer image / head image
-    const size_t per_layer = 3 * CL * IW, total = per_layer * n_layers + 2 * CL * HW;
+    constexpr int NVR = W / 16, KSC = cl8_ksc(W), NCH = NVR / KSC;
+    constexpr size_t IW = 2 * KSC * 256, HW = CL8_IMGH / 4;         // words per layer chunk image / end_conv_1 chunk image
+    const size_t per_layer = 3 * NCH * NVR * IW, total = per_layer * n_layers + (size_t)(NVR + CL8_C / 16) * NVR * 256;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const float* src;      // row-major weight matrix the word comes from
         int row, col, ld, stride = 1;
@@ -1993,18 +2001,24 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
         if (w < per_layer * n_layers) {
             const int l = (int)(w / per_layer);
             w -= (size_t)l * per_layer;
-            const int kind = (int)(w / (CL * IW));          // 0: stage 1, tap 0 (old)   1: stage 1, tap 1 (current)   2: stage 2
-            w -= (size_t)kind * CL * IW;
+            const int kind = (int)(w / (NCH * NVR * IW));   // 0: stage 1, tap 0 (old)   1: stage 1, tap 1 (current)   2: stage 2
+            w -= (size_t)kind * NCH * NVR * IW;
+            int c = 0;
+            if constexpr (NCH > 1) {
+                c = (int)(w / (NVR * IW));
+                w -= (size_t)c * NVR * IW;
+            }
             const int vrank = (int)(w / IW);
             w -= (size_t)vrank * IW;
             const GenLayer& L = layers[l];
-            const int j = (int)(w & 3), lane = (int)((w >> 2) & 31), ks = (int)((w >> 8) & 15), mt = (int)(w >> 12);
+            const int j = (int)(w & 3), lane = (int)((w >> 2) & 31), ks = c * KSC + (int)((w >> 8) & (KSC - 1)),
+                      mt = (int)(w / (KSC * 256));
             const int g = lane >> 2, t = lane & 3;
             row = vrank * 16 + g + 8 * (j & 1);
             const int kk = 2 * t + 8 * (j >> 1);
             if (kind < 2) { src = mt ? L.wg : L.wf; col = (ks * 16 + kk) * 2 + kind; ld = 2 * W; stride = 2; }
             else { src = mt ? L.ws : L.wr; col = ks * 16 + kk; ld = W; }
-        } else {
+        } else if (W == 256) {
             w -= per_layer * n_layers;
             const int which = (int)(w / (CL * HW));         // 0: end_conv_1   1: end_conv_2
             w -= (size_t)which * CL * HW;
@@ -2016,6 +2030,28 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
             col = ks * 16 + 2 * t + 8 * (j >> 1);
             ld = W;
             src = which ? e2w : e1w;
+        } else {
+            w -= per_layer * n_layers;
+            const bool e2 = w >= (size_t)NVR * NVR * 256;   // end_conv_1: NVR chunks of NVR x 16 KB; end_conv_2: 16 x NVR KB
+            int vrank, ks;
+            if (!e2) {
+                const int c = (int)(w / (NVR * HW));
+                w -= (size_t)c * NVR * HW;
+                vrank = (int)(w / HW);
+                w -= (size_t)vrank * HW;
+                ks = c * 16 + (int)(w >> 8);
+            } else {
+                w -= (size_t)NVR * NVR * 256;
+                vrank = (int)(w / (NVR * 256));
+                w -= (size_t)vrank * NVR * 256;
+                ks = (int)(w >> 8);
+            }
+            const int j = (int)(w & 3), lane = (int)((w >> 2) & 31);
+            const int g = lane >> 2, t = lane & 3;
+            row = vrank * 16 + g + 8 * (j & 1);
+            col = ks * 16 + 2 * t + 8 * (j >> 1);
+            ld = W;
+            src = e2 ? e2w : e1w;
         }
         const int half = (int)((i >> 7) & 1);                // every image is a multiple of 256 words: bit 7 of i is the hi/lo plane
         const float x0 = src[(size_t)row * ld + col], x1 = src[(size_t)row * ld + col + stride];
@@ -2026,29 +2062,39 @@ __global__ void cl8_pack_kernel(const GenLayer* layers, int n_layers, const floa
     }
 }
 
-// CS = CTAs per cluster (16 or 8).  The exchanged vectors always consist of 16 blocks ("virtual ranks" of 16 channels);
-// a CTA of a CS-cluster owns VR = 16 / CS consecutive virtual ranks and walks them one after the other in every stage.  Only
-// few clusters of 16 CTAs are co-resident (tools/cluster_occ.cu) but about twice as many clusters of 8: CS = 8 runs 64 streams
-// (8 clusters) in one wave on 64 SMs, at twice the per-CTA work -- the step is bound by the exchange latency, not by it.
+// W = the net's width (256 or 512).  CS = CTAs per cluster (16 or 8 at W = 256, 16 at W = 512).  The exchanged vectors
+// consist of NVR = W / 16 blocks ("virtual ranks" of 16 channels); a CTA of a CS-cluster owns VR = NVR / CS consecutive
+// virtual ranks and walks them one after the other in every stage.  Only few clusters of 16 CTAs are co-resident
+// (tools/cluster_occ.cu) but about twice as many clusters of 8: CS = 8 runs 64 streams (8 clusters) in one wave on 64 SMs,
+// at twice the per-CTA work -- the step is bound by the exchange latency, not by it.  At W = 512 VR = 2 with clusters of
+// 16 already; clusters of 8 (VR = 4) would need twice the accumulators and staging, and do not fit.  The logit vector has
+// 256 rows at both widths: NVRH = 16 virtual ranks, VRH = 16 / CS per CTA (1 at W = 512: the rows of CTA rank r are
+// classes 16r .. 16r+15).
 // COND: the filter / gate biases come from the condition table (a separate instantiation: the per-layer branch costs the
 // unconditioned single-stream kernel ~6 % of its time per sample).  FRAMES (with COND): the table is a local-conditioning
 // window, and each evaluation reads its frame's rows (a third instantiation, so the other two carry no trace of it).
 // PS: per-stream settings (p.ps set); the scalar path runs the PS = false instantiations, which read only the scalars.
-template <int CS, bool COND, bool FRAMES, bool PS>
-__global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
+template <int W, int CS, bool COND, bool FRAMES, bool PS>
+__global__ void __launch_bounds__(GEN_NT + 64 + (W / 16 / CS == 2 ? 32 : 0), 1) gen_kernel_cl8(const GenParams p) {
     extern __shared__ __align__(128) unsigned char smb[];
-    constexpr int W = CL8_W, SB = CL8_SB, NV = 16, BLK = CL8_BLK, VEC = CL8_VEC, VR = CL / CS, NVC = NV * VR;
-    // exchanged vectors first: same offsets in every CTA (mapa keeps the offset).  Each is 16 blocks of 512 bytes.
+    constexpr int C = CL8_C, SB = CL8_SB, NV = 16, BLK = CL8_BLK, NVR = W / NV, VEC = NVR * BLK, VR = NVR / CS, NVC = NV * VR;
+    constexpr int VRH = C / NV / CS;                    // virtual ranks of the logit vector per CTA
+    static_assert((W == 256 || W == 512) && VR * CS == NVR && (VR == 1 || VR == 2), "gen_kernel_cl8: unsupported geometry");
+    // ring chunks: a layer stage is NCH chunks of KSC k-steps (KQ per warp), end_conv_1 NCH1 chunks of 16 k-steps, and
+    // end_conv_2 one chunk of VRH virtual ranks x NVR k-steps
+    constexpr int KSC = cl8_ksc(W), NCH = NVR / KSC, KQ = KSC / 4, IMGC = 2 * KSC * 1024, NCH1 = NVR / 16;
+    // exchanged vectors first: same offsets in every CTA (mapa keeps the offset).  Each is NVR blocks of 512 bytes.
     unsigned char* Xcur = smb;                          // [2] layer input h (hi/lo split), by layer parity
     unsigned char* Xz = Xcur + 2 * VEC;                 // [2] gated activation z, by layer parity; Xz[1] doubles as sampling scratch
-    unsigned char* Xs = Xz + 2 * VEC;                   // relu(skip sum)           \  Xz[1], Xs, Xy are contiguous: 24 KB that no
+    unsigned char* Xs = Xz + 2 * VEC;                   // relu(skip sum)           \  Xz[1], Xs, Xy are contiguous: 3 vectors that no
     unsigned char* Xy = Xs + VEC;                       // end_conv_1 output        /  peer writes while this CTA samples
-    unsigned char* Xl = Xy + VEC;                       // logits, fp32: [virtual rank][stream][16]
+    unsigned char* Xl = Xy + VEC;                       // logits, fp32: [virtual rank 0-15][stream][16]
     unsigned char* Xold = Xl + VEC;                     // history taps of the coming stage 1 (local)
     unsigned char* stg = Xold + VEC;                    // [2][VR][BLK] this CTA's contribution of a stage, staged for the pusher
     float* part = reinterpret_cast<float*>(stg + 2 * VR * BLK);               // [2][VR][8 warps][32 lanes][4] partial C fragments
     float* hown = part + 2 * VR * 8 * 128;              // [2][VR][16][SB] fp32 layer input at the channels this CTA owns
-    constexpr int SLOTB = VR * CL8_IMG2, NSLOT = 4 / VR;         // weight ring: 4 x 32 KB (VR = 1) or 2 x 64 KB (VR = 2)
+    // weight ring: 4 x 32 KB (W = 256, VR = 1), 2 x 64 KB (W = 256, VR = 2) or 2 x 32 KB (W = 512)
+    constexpr int SLOTB = VR * IMGC, NSLOT = W == 256 ? 4 / VR : 2;
     constexpr int NTHR = GEN_NT + 64 + (VR == 2 ? 32 : 0);      // workers + producer + pusher (+ second producer for VR = 2)
     unsigned char* wbuf = reinterpret_cast<unsigned char*>(hown + 2 * NVC * SB);         // [NSLOT][SLOTB] weight image ring
     unsigned long long* fullb = reinterpret_cast<unsigned long long*>(wbuf + (size_t)NSLOT * SLOTB);
@@ -2057,8 +2103,8 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     GenLayer* lay_s = reinterpret_cast<GenLayer*>(xbar + 8);
     int* slot_s = reinterpret_cast<int*>(lay_s + p.n_layers);
     int* idx_s = slot_s + p.n_layers;                   // [SB] current class index per stream, [SB] abort flag
-    float* logit_s = reinterpret_cast<float*>(Xz + VEC);                      // [SB][W] sampling scratch (aliases Xz[1])
-    double* cdf = reinterpret_cast<double*>(Xs);                              // [SB][W]                   (aliases Xs, Xy)
+    float* logit_s = reinterpret_cast<float*>(Xz + VEC);                      // [SB][C] sampling scratch (aliases Xz[1])
+    double* cdf = reinterpret_cast<double*>(Xs);                              // [SB][C]  (aliases Xs; Xy too at W = 256)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int rank = (int)cluster_rank(), cl = blockIdx.x / CS, NS = p.NS, NL = p.n_layers;
@@ -2066,7 +2112,8 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     // live streams of this cluster: slots 0 .. n_live-1.  A stream's bytes in every exchanged block are contiguous (64 at
     // s * 64: cl8_unit_off, and the [stream][16] fp32 logits), so only the first 64 * n_live bytes of each block travel.
     const int n_live = min(SB, NS - cl * SB);
-    const unsigned XVEC = 64u * (unsigned)n_live * NV;  // bytes of one exchange round that land in each CTA
+    const unsigned XVEC = 64u * (unsigned)n_live * NVR; // bytes of one exchange round that land in each CTA
+    const unsigned XVECL = 64u * (unsigned)n_live * (C / NV);     // ... of the logit round (= XVEC at W = 256)
     const int o0 = v0 * NV;                             // first channel this CTA owns in every stage vector
 
     {
@@ -2088,16 +2135,33 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     // peers and may hold stale values or sampling scratch: harmless, since MMA columns (= streams) are independent, and
     // every reduction and store works per (row, stream) and is guarded by fs_on / hs_g < NS.
     if (tid == 0)
-        for (int i = 0; i < 7; ++i) mbar_expect_tx(xbar + i, XVEC);            // arm phase 0 of every exchange barrier
+        for (int i = 0; i < 7; ++i) mbar_expect_tx(xbar + i, (W != 256 && i == 6) ? XVECL : XVEC);     // arm phase 0 of every exchange barrier
     for (int l = tid; l < NL; l += GEN_NT) {
         const int len = lay_s[l].ring_len;
         slot_s[l] = (p.t0 + len - 1) % len;
     }
     cluster_sync_all();                                  // nobody may store into a peer before its barriers exist
     constexpr unsigned smask = (unsigned)NSLOT - 1u, sshift = (NSLOT == 4) ? 2u : 1u;
-    const size_t img_kind = (size_t)CL * CL8_IMG2;       // bytes of one (layer, kind): 16 virtual ranks
-    const unsigned char* img_mine = p.cl8_img + (size_t)v0 * CL8_IMG2;
-    const unsigned char* img_head = p.cl8_img + 3 * img_kind * NL + (size_t)v0 * CL8_IMGH;
+    const size_t img_kind = (size_t)NVR * IMGC;          // bytes of one (layer, kind, chunk): all virtual ranks
+    const unsigned char* img_mine = p.cl8_img + (size_t)v0 * IMGC;
+    const unsigned char* img_head = p.cl8_img + 3 * NCH * img_kind * NL + (size_t)v0 * CL8_IMGH;
+    // end_conv_2 (W = 512; at W = 256 it is end_conv_1's second chunk): this CTA's VRH virtual ranks x NVR k-steps
+    const unsigned char* img_e2 = p.cl8_img + 3 * NCH * img_kind * NL + (size_t)NVR * NVR * 1024 + (size_t)rank * VRH * NVR * 1024;
+    // the source and size of ring chunk st of an evaluation: the layer stages' chunks, then the head's
+    auto chunk_src = [&](int st, unsigned& bytes) {
+        const unsigned char* src;
+        if (st < 3 * NCH * NL) {
+            src = img_mine + (size_t)st * img_kind;
+            bytes = VR * IMGC;
+        } else if (W == 256 || st - 3 * NCH * NL < NCH1) {
+            src = img_head + (size_t)(st - 3 * NCH * NL) * NVR * CL8_IMGH;
+            bytes = VR * CL8_IMGH;
+        } else {
+            src = img_e2;
+            bytes = VRH * NVR * 1024;
+        }
+        return src;
+    };
 
     // push the staged blocks `sb` into blocks v0 .. v0+VR-1 of vector `vec` of every CTA of the cluster: the pusher warp
     // (warp 9) reads the live part of each 512-byte block back (16 bytes per lane, lanes 0 .. 4*n_live-1) and issues ONE
@@ -2114,10 +2178,12 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     for (int d = 0; d < CS; ++d) rdelta[d] = (warp == GEN_WARPS + 1) ? mapa_u32(sm_base, (unsigned)d) - sm_base : 0u;
     auto push = [&](int sb, unsigned char* vec, int bar_i) {
         if (lane >= 4 * n_live) return;
+        const bool lg = W != 256 && bar_i == 6;          // the logit vector: VRH blocks from rank * VRH
 #pragma unroll
         for (int vr = 0; vr < VR; ++vr) {
+            if (lg && vr >= VRH) break;
             const uint4 v = *reinterpret_cast<const uint4*>(stg + (sb * VR + vr) * BLK + lane * 16);
-            const unsigned la = smem_u32(vec + (v0 + vr) * BLK + lane * 16), lb = smem_u32(xbar + bar_i);
+            const unsigned la = smem_u32(vec + ((lg ? rank * VRH : v0) + vr) * BLK + lane * 16), lb = smem_u32(xbar + bar_i);
 #pragma unroll
             for (int d = 0; d < CS; ++d)
                 asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(
@@ -2160,17 +2226,11 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             unsigned q = 0;
             for (int ev = 0; ev < p.n_evals; ++ev) {
                 const bool wh = head_at(p, p.t0 + ev);
-                const int n_st = wh ? 3 * NL + 2 : 3 * NL;      // per layer: old taps, current input, stage 2; then the two head stages
+                // per layer: old taps, current input, stage 2 (NCH chunks each); then the head stages' chunks
+                const int n_st = wh ? 3 * NCH * NL + NCH1 + 1 : 3 * NCH * NL;
                 for (int st = 0; st < n_st; ++st, ++q) {
-                    const unsigned char* src;
                     unsigned bytes;
-                    if (st < 3 * NL) {
-                        src = img_mine + (size_t)st * img_kind;
-                        bytes = VR * CL8_IMG2;
-                    } else {
-                        src = img_head + (size_t)(st - 3 * NL) * CL * CL8_IMGH;
-                        bytes = VR * CL8_IMGH;
-                    }
+                    const unsigned char* src = chunk_src(st, bytes);
                     const int slot = (int)(q & smask);
                     if (q >= (unsigned)NSLOT) {
                         const unsigned par = ((q >> sshift) & 1u) ^ 1u;
@@ -2191,17 +2251,19 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         return;
     }
     // ---- second producer (VR = 2 only): one bulk copy at a time streams ~31 bytes/cycle into the 2-slot ring, which made
-    // the 192 KB of a layer the bottleneck; this warp fetches the second virtual rank's image of every stage as 16-byte
-    // cp.async copies (load/store path, ~27 bytes/cycle for one warp) in parallel with the bulk copy of the first.
+    // the 192 KB of a layer the bottleneck; this warp fetches the second half of every chunk (the second virtual rank's
+    // image; end_conv_2 at W = 512: the second half of its k-steps) as 16-byte cp.async copies (load/store path, ~27
+    // bytes/cycle for one warp) in parallel with the bulk copy of the first.
     if (VR == 2 && warp == GEN_WARPS + 2) {
         unsigned q = 0;
         for (int ev = 0; ev < p.n_evals; ++ev) {
             const bool wh = head_at(p, p.t0 + ev);
-            const int n_st = wh ? 3 * NL + 2 : 3 * NL;
+            const int n_st = wh ? 3 * NCH * NL + NCH1 + 1 : 3 * NCH * NL;
             for (int st = 0; st < n_st; ++st, ++q) {
-                const unsigned half = (st < 3 * NL) ? CL8_IMG2 : CL8_IMGH;
-                const unsigned char* src = (st < 3 * NL) ? img_mine + (size_t)st * img_kind + half
-                                                         : img_head + (size_t)(st - 3 * NL) * CL * CL8_IMGH + half;
+                unsigned half;
+                const unsigned char* src = chunk_src(st, half);
+                half /= 2;
+                src += half;
                 const int slot = (int)(q & smask);
                 if (q >= (unsigned)NSLOT) {
                     const unsigned par = ((q >> sshift) & 1u) ^ 1u;
@@ -2240,7 +2302,11 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     auto xwait = [&](int i) {
         mbar_wait_bounded(xbar + i, (xpar >> i) & 1u);
         xpar ^= 1u << i;
-        if (tid == 0) mbar_expect_tx(xbar + i, XVEC);
+        if constexpr (W == 256) {
+            if (tid == 0) mbar_expect_tx(xbar + i, XVEC);
+        } else {
+            if (tid == 0) mbar_expect_tx(xbar + i, i == 6 ? XVECL : XVEC);
+        }
     };
     // one k-step of this warp's m-tile: A fragments (hi, lo) from the stage image, B fragments of the 8 streams from a block
     const int mt = warp & 1, kq = warp >> 1;
@@ -2262,15 +2328,16 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         mma_bf16_16816(d.hl, ah, b.y, b.w);
         mma_bf16_16816(d.hh, ah, b.x, b.z);
     };
-    // this warp's four k-steps (4*kq .. 4*kq+3) of its m-tile of the 32 KB layer image of every virtual rank (images VR apart
-    // by CL8_IMG2) against blocks 4*kq.. of vector x.  The virtual ranks' chains are interleaved k-step by k-step: they are
+    // this warp's KQ k-steps (KQ*kq .. KQ*kq+KQ-1) of its m-tile of ring chunk c of every virtual rank (images VR apart by
+    // IMGC) against blocks c*KSC + KQ*kq.. of vector x.  The virtual ranks' chains are interleaved k-step by k-step: they are
     // independent, share the B fragments, and hide each other's MMA latency (nothing is stored until all are issued).
-    auto mma_quarter = [&](const unsigned char* wimg, const unsigned char* x, Acc3 (&d)[VR]) {
+    auto mma_quarter = [&](const unsigned char* wimg, const unsigned char* x, int c, Acc3 (&d)[VR]) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < KQ; ++i)
 #pragma unroll
             for (int vr = 0; vr < VR; ++vr)
-                mma_step(wimg + vr * CL8_IMG2 + ((size_t)(mt * 16 + 4 * kq + i) * 2) * 512 + lane * 16, x + (4 * kq + i) * BLK, d[vr]);
+                mma_step(wimg + vr * IMGC + ((size_t)(mt * KSC + KQ * kq + i) * 2) * 512 + lane * 16,
+                         x + (c * KSC + KQ * kq + i) * BLK, d[vr]);
     };
     // sum over the 4 K quarters of output (m-tile m, row r of the tile, stream s): fragment element (lane', j) of each partial
     auto part_sum = [&](const float* pb, int m, int r, int s) {
@@ -2279,7 +2346,8 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     };
     // history taps: thread -> (stream = warp, channels 2*lane + 64*j + {0,1}), fetched into registers one stage ahead
     const int hs_g = cl * SB + warp;                     // global stream whose taps this thread fetches (and which it samples)
-    Pair2 hq[4];
+    constexpr int NHQ = W / 64;
+    Pair2 hq[NHQ];
     const uint2* hsrc = nullptr;
     unsigned htag = 0;
     auto issue_old = [&](int ln, int te, int slot_te) {  // slot_te = ring slot of time te in layer ln
@@ -2290,12 +2358,12 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             hsrc = p.ringLL + Lp.ring_off + ((size_t)so * NS + hs_g) * W + 2 * lane;
             htag = (unsigned)(te - Lp.dil) + 1u;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) hq[j] = ld_pair2(hsrc + 64 * j);
+            for (int j = 0; j < NHQ; ++j) hq[j] = ld_pair2(hsrc + 64 * j);
         }
     };
     auto commit_old = [&]() {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < NHQ; ++j) {
             float a = 0.f, b = 0.f;
             if (hsrc != nullptr) {
                 if (hq[j].a.y != htag || hq[j].b.y != htag) hq[j] = poll2_spin(hsrc + 64 * j, htag, p.err, idx_s + SB);
@@ -2318,6 +2386,10 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
     const int fvr = (VR == 2) ? (tid >> 7) : 0, fc = (tid >> 3) & 15, fs = tid & 7;
     const bool fin_a = (VR == 2) || tid < NV * SB, fin_s = (VR == 2) || tid >= NV * SB;
     const int fch = o0 + fvr * NV + fc;                   // the channel (= row of the stage's weight matrix) this thread finishes
+    // the logit this thread finishes (end_conv_2 row): fch where the logit vector splits like the others (VRH = VR), else
+    // class rank*16 + fc in threads 0-127
+    const bool fin_l = (VRH == VR) ? fin_a : tid < NV * SB;
+    const int fcl = (VRH == VR) ? fch : rank * NV + fc, fvl = (VRH == VR) ? fvr : 0;
     const int fsg = cl * SB + fs;
     const bool fs_on = fsg < NS;
     unsigned pb_i = 0, sb_i = 0;                          // partial-sum / staging double-buffer indices
@@ -2350,13 +2422,13 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         // owners of a channel also enqueue it in the ring and keep the fp32 value for the residual add
         {
             int idx = idx_s[warp];
-            idx = idx < 0 ? 0 : (idx >= W ? W - 1 : idx);
+            idx = idx < 0 ? 0 : (idx >= C ? C - 1 : idx);
             const GenLayer& L0 = lay_s[0];
             uint2* ring0 = p.ringLL + L0.ring_off + ((size_t)slot_s[0] * NS + hs_g) * W;
 #pragma unroll
             for (int j = 0; j < W / 32; ++j) {
                 const int r = lane + 32 * j;
-                const float v = __ldg(p.start_w + (size_t)r * W + idx) + (p.start_b ? __ldg(p.start_b + r) : 0.f);
+                const float v = __ldg(p.start_w + (size_t)r * C + idx) + (p.start_b ? __ldg(p.start_b + r) : 0.f);
                 cl8_put(Xcur + (r >> 4) * BLK, warp, r & 15, v);
                 if (r >= o0 && r < o0 + NVC) {
                     hown[(r - o0) * SB + warp] = v;
@@ -2386,17 +2458,27 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
                 else if (ev + 1 < p.n_evals) issue_old(0, t + 1, (slot_s[0] + 1 == lay_s[0].ring_len) ? 0 : slot_s[0] + 1);
                 else hsrc = nullptr;
                 Acc3 d[VR];
-                const unsigned char* wimg = stage_weights();
-                TR8();         // 1: stage-1 weights (old tap) landed
 #pragma unroll
-                for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
-                mma_quarter(wimg, Xold, d);
-                release_slot();
-                wimg = stage_weights();
-                if (l > 0) xwait(l & 1);
-                TR8();         // 2: old-tap MMAs done, h arrived
-                mma_quarter(wimg, xc, d);
-                release_slot();
+                for (int c = 0; c < NCH; ++c) {
+                    const unsigned char* wimg = stage_weights();
+                    if (c == 0) {
+                        TR8();         // 1: stage-1 weights (old tap) landed
+#pragma unroll
+                        for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
+                    }
+                    mma_quarter(wimg, Xold, c, d);
+                    release_slot();
+                }
+#pragma unroll
+                for (int c = 0; c < NCH; ++c) {
+                    const unsigned char* wimg = stage_weights();
+                    if (c == 0) {
+                        if (l > 0) xwait(l & 1);
+                        TR8();         // 2: old-tap MMAs done, h arrived
+                    }
+                    mma_quarter(wimg, xc, c, d);
+                    release_slot();
+                }
 #pragma unroll
                 for (int vr = 0; vr < VR; ++vr) acc_store(d[vr], part_of(pb_i, vr) + ((kq * 2 + mt) * 32 + lane) * 4);
                 TR8();         // 3: MMAs done, partials stored
@@ -2419,15 +2501,20 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
                 commit_old();
                 TR8();         // 6: next history taps in place
                 const bool active = (mt == 0) ? more : want_head;
-                const unsigned char* wimg = stage_weights();
-                TR8();         // 7: stage-2 weights landed
-                xwait(2 + (l & 1));
-                TR8();         // 8: z arrived
                 Acc3 d[VR];
 #pragma unroll
-                for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
-                if (active) mma_quarter(wimg, zb, d);
-                release_slot();
+                for (int c = 0; c < NCH; ++c) {
+                    const unsigned char* wimg = stage_weights();
+                    if (c == 0) {
+                        TR8();         // 7: stage-2 weights landed
+                        xwait(2 + (l & 1));
+                        TR8();         // 8: z arrived
+#pragma unroll
+                        for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
+                    }
+                    if (active) mma_quarter(wimg, zb, c, d);
+                    release_slot();
+                }
 #pragma unroll
                 for (int vr = 0; vr < VR; ++vr) acc_store(d[vr], part_of(pb_i, vr) + ((kq * 2 + mt) * 32 + lane) * 4);
                 TR8();         // 9: MMAs done, partials stored
@@ -2457,26 +2544,37 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         if (tr_on) p.trace[2041] = clock64();             // layers done
         if (!want_head) continue;
 
-        // ================= head: relu(skip) -> end_conv_1 -> relu -> end_conv_2; one m-tile per virtual rank, 16 k-steps
-        // over the 8 warps (2 each)
+        // ================= head: relu(skip) -> end_conv_1 -> relu -> end_conv_2; one m-tile per virtual rank, the k-steps
+        // of each chunk spread over the 8 warps (end_conv_1: 2 of 16 each; end_conv_2: NVR / 8 of NVR)
         if (fin_s) cl8_put(stg_of(sb_i, fvr), fs, fc, fmaxf(skr, 0.f));
         CL8_STAGED_ARRIVE();
         sb_i ^= 1;
-        auto head_stage = [&](const unsigned char* x) {     // this warp's 2 k-steps of each virtual rank's m-tile -> part
-            const unsigned char* wimg = stage_weights();
+        // this warp's k-steps of each of the stage's nvr virtual ranks' m-tiles over its nch chunks of kpc k-steps -> part
+        auto head_stage = [&](const unsigned char* x, int nch, int nvr, int kpc) {
             Acc3 d[VR];
 #pragma unroll
-            for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
+            for (int c = 0; c < NCH1; ++c) {
+                if (c >= nch) break;
+                const unsigned char* wimg = stage_weights();
+                if (c == 0) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int vr = 0; vr < VR; ++vr) {
-                    const int ks = 2 * warp + i;
-                    mma_step(wimg + vr * CL8_IMGH + ((size_t)ks * 2) * 512 + lane * 16, x + ks * BLK, d[vr]);
+                    for (int vr = 0; vr < VR; ++vr) acc_zero(d[vr]);
                 }
-            release_slot();
 #pragma unroll
-            for (int vr = 0; vr < VR; ++vr) acc_store(d[vr], part_of(pb_i, vr) + (warp * 32 + lane) * 4);
+                for (int i = 0; i < NVR / 8; ++i) {
+                    if (i >= kpc / 8) break;
+#pragma unroll
+                    for (int vr = 0; vr < VR; ++vr) {
+                        if (vr >= nvr) break;
+                        const int ks = (kpc / 8) * warp + i;
+                        mma_step(wimg + vr * kpc * 1024 + ((size_t)ks * 2) * 512 + lane * 16, x + (c * kpc + ks) * BLK, d[vr]);
+                    }
+                }
+                release_slot();
+            }
+#pragma unroll
+            for (int vr = 0; vr < VR; ++vr)
+                if (vr < nvr) acc_store(d[vr], part_of(pb_i, vr) + (warp * 32 + lane) * 4);
         };
         auto head_sum = [&](const float* pb, int r, int s) {  // 8 partials, one per warp
             const float* q = pb + (((r & 7) * 4 + (s >> 1)) << 2) + ((r >> 3) << 1) + (s & 1);
@@ -2486,7 +2584,7 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             return v;
         };
         xwait(4);
-        head_stage(Xs);
+        head_stage(Xs, NCH1, VR, 16);
         WORKER_SYNC();
         if (fin_a) {
             const float y = fmaxf(head_sum(part_of(pb_i, fvr), fc, fs) + __ldg(p.e1b + fch), 0.f);
@@ -2496,17 +2594,17 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
         CL8_STAGED_ARRIVE();
         sb_i ^= 1;
         xwait(5);
-        head_stage(Xy);
+        head_stage(Xy, 1, VRH, NVR);
         WORKER_SYNC();
-        if (fin_a) {
-            const float dc = (float)fch - (float)W / 2.f;
-            const float v = (head_sum(part_of(pb_i, fvr), fc, fs) + __ldg(p.e2b + fch)) -
+        if (fin_l) {
+            const float dc = (float)fcl - (float)C / 2.f;
+            const float v = (head_sum(part_of(pb_i, fvl), fc, fs) + __ldg(p.e2b + fcl)) -
                             (dc * dc) * ((PS && fs_on) ? p.ps[fsg].regularize : p.regularize);
             if (fs_on && p.out_logits) {
                 const int samp = sample_of<PS ? PS_ON : PS_OFF>(p, fsg, t);
-                if (samp >= 0) p.out_logits[((size_t)fsg * p.n_samples + samp) * W + fch] = v;
+                if (samp >= 0) p.out_logits[((size_t)fsg * p.n_samples + samp) * C + fcl] = v;
             }
-            reinterpret_cast<float*>(stg_of(sb_i, fvr))[fs * NV + fc] = v;               // logits travel as fp32: [stream][16]
+            reinterpret_cast<float*>(stg_of(sb_i, fvl))[fs * NV + fc] = v;               // logits travel as fp32: [stream][16]
         }
         pb_i ^= 1;
         CL8_STAGED_ARRIVE();
@@ -2518,18 +2616,20 @@ __global__ void __launch_bounds__(GEN_NT + 64 + (CS == 8 ? 32 : 0), 1) gen_kerne
             const GenStream ss = stream_set<PS ? PS_ON : PS_OFF>(p, hs_g);
             const int samp = sample_of<PS ? PS_ON : PS_OFF>(p, hs_g, t);
             if (samp >= 0) {                              // no selection while the stream is inside its prompt
-                float* lg = logit_s + warp * W;
+                float* lg = logit_s + warp * C;
                 const float* xl = reinterpret_cast<const float*>(Xl);
-                for (int c = lane; c < W; c += 32) lg[c] = xl[(c >> 4) * (BLK / 4) + warp * NV + (c & 15)];
+                for (int c = lane; c < C; c += 32) lg[c] = xl[(c >> 4) * (BLK / 4) + warp * NV + (c & 15)];
                 __syncwarp();
-                const int choice = ss.trunc ? choose_truncated(lg, reinterpret_cast<unsigned*>(cdf + warp * W),
-                                                               reinterpret_cast<float*>(cdf + warp * W) + W, W, lane,
+                const int choice = ss.trunc ? choose_truncated(lg, reinterpret_cast<unsigned*>(cdf + warp * C),
+                                                               reinterpret_cast<float*>(cdf + warp * C) + C, C, lane,
                                                                ss.temperature, ss.top_k, ss.top_p,
                                                                p.uniforms + (size_t)hs_g * p.n_samples + samp)
-                                            : choose_sample(lg, cdf + warp * W, W, lane, ss.temperature,
+                                            : choose_sample(lg, cdf + warp * C, C, lane, ss.temperature,
                                                             p.uniforms ? p.uniforms + (size_t)hs_g * p.n_samples + samp : nullptr);
                 if (lane == 0) {
-                    idx_s[warp] = choice;
+                    // with forced samples the next evaluation's input is given, and the top of the loop stores it from
+                    // another thread that no barrier separates from this one: store the choice only where it is used
+                    if (p.forced == nullptr || ev + 1 == p.n_evals) idx_s[warp] = choice;
                     if (rank == 0) p.out_idx[(size_t)hs_g * p.n_samples + samp] = choice;
                 }
             }
@@ -2584,10 +2684,17 @@ __global__ void gen_prefill_kernel(const void* __restrict__ src, int pairs, int 
 struct ScratchLayout {
     size_t bar, cur_idx, layers, zbuf, skipbuf, y1buf, logitbuf, err, zLL, skipLL, y1LL, logitLL, ll_end, trace, cl8_img, cl8_bytes, total;
 };
-// the batched cluster kernel's shape: a k = 2 net whose five widths are all 256 (any number of streams)
+// the batched cluster kernel's shape: a k = 2 net of 256 classes whose other four widths are all 256 or all 512 (any
+// number of streams)
 static bool cl8_shape_ok(const wn_gen_shape& s) {
-    return s.n_streams >= 1 && s.k == 2 && s.n_layers >= 2 && s.R == CL8_W && s.D == CL8_W && s.S == CL8_W && s.E == CL8_W &&
-           s.classes == CL8_W;
+    return s.n_streams >= 1 && s.k == 2 && s.n_layers >= 2 && (s.R == 256 || s.R == 512) && s.D == s.R && s.S == s.R &&
+           s.E == s.R && s.classes == CL8_C;
+}
+// bytes of its weight images (cl8_pack_kernel): per layer 3 kinds x W/16 virtual ranks x 2 m-tiles x W/16 k-steps of 1 KB,
+// then end_conv_1 (W/16 x W/16 KB) and end_conv_2 (16 x W/16 KB): 1.5 MB per layer at W = 256, 6 MB at W = 512
+static size_t cl8_image_bytes(const wn_gen_shape& s) {
+    const size_t nvr = (size_t)s.R / 16;
+    return 1024 * (6 * nvr * nvr * (size_t)s.n_layers + nvr * nvr + 16 * nvr);
 }
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static ScratchLayout scratch_layout(const wn_gen_shape& s) {
@@ -2608,7 +2715,7 @@ static ScratchLayout scratch_layout(const wn_gen_shape& s) {
     o.ll_end = off;
     o.trace = off; off += 8 * 2048;
     o.cl8_img = off;
-    o.cl8_bytes = cl8_shape_ok(s) ? (size_t)CL * ((size_t)s.n_layers * (CL8_IMG1 + CL8_IMG2) + 2 * CL8_IMGH) : 0;
+    o.cl8_bytes = cl8_shape_ok(s) ? cl8_image_bytes(s) : 0;
     off = align_up(off + o.cl8_bytes, 256);
     o.total = off;
     return o;
@@ -2651,6 +2758,7 @@ struct wn_gen_handle {
     bool generic_ok, ll_ok;    // the grid-barrier / the generic flag-exchange kernel fit in shared memory for this stream count
     bool cl8_8_ok;             // ... and so does its 8-CTA-cluster instantiation
     int cl8_cs;                // its cluster size, 16 or 8 (wn_gen_create)
+    int cl8_w;                 // its width instantiation, 256 or 512 (the net's R)
     size_t smem_cl8, smem_cl8_8;
     int top_k;              // wn_gen_set_truncation (0, 1.0: off)
     double top_p;
@@ -2696,7 +2804,8 @@ extern "C" int wn_gen_workspace_bytes(const wn_gen_shape* s, size_t* ring_bytes,
 static cudaLaunchConfig_t cl8_config(const wn_gen_handle* h, int cs, cudaStream_t st, cudaLaunchAttribute* attr) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)((h->shape.n_streams + CL8_SB - 1) / CL8_SB * cs));
-    cfg.blockDim = dim3(GEN_NT + 64 + (cs == 8 ? 32 : 0));    // 8 worker warps, the weight producer warp(s), the pusher warp
+    // 8 worker warps, the weight producer warp(s) (two where a CTA owns two virtual ranks), the pusher warp
+    cfg.blockDim = dim3(GEN_NT + 64 + (h->cl8_w / 16 / cs == 2 ? 32 : 0));
     cfg.dynamicSmemBytes = cs == 16 ? h->smem_cl8 : h->smem_cl8_8;
     cfg.stream = st;
     attr->id = cudaLaunchAttributeClusterDimension;
@@ -2709,15 +2818,19 @@ static cudaLaunchConfig_t cl8_config(const wn_gen_handle* h, int cs, cudaStream_
 }
 
 // Cluster size of the batched cluster kernel: 16 CTAs (least work per CTA) while all clusters are co-resident, else 8
-// (15 clusters fit instead of 7).  WN_GEN_CL8_CS=16|8 forces one (8 only where it fits).
+// (15 clusters fit instead of 7).  WN_GEN_CL8_CS=16|8 forces one (8 only where it fits).  512-wide nets run clusters of 16.
 static int choose_cl8_cs(wn_gen_handle* h) {
+    if (h->cl8_w == 512) {
+        h->cl8_cs = 16;
+        return 0;
+    }
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cl8_config(h, 16, nullptr, &attr);
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<16, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<256, 16, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)cfg.dynamicSmemBytes));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<16, false, false, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<256, 16, false, false, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     int fit16 = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&fit16, gen_kernel_cl8<16, false, false, false>, &cfg));
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&fit16, gen_kernel_cl8<256, 16, false, false, false>, &cfg));
     const int need = (h->shape.n_streams + CL8_SB - 1) / CL8_SB;
     h->cl8_cs = (need <= fit16 || !h->cl8_8_ok) ? 16 : 8;
     if (const char* e = getenv("WN_GEN_CL8_CS")) {
@@ -2732,7 +2845,7 @@ static int pick_kernel(const wn_gen_handle* h) {
     const int m = h->mode;
     if (m == 3 || m == 4 || m == 6) return m;               // wn_gen_set_mode accepts these only where they apply
     if (m == 0) {
-        if (h->cl8_ok) return 6;                            // any number of streams of a 256-wide net
+        if (h->cl8_ok) return 6;                            // any number of streams of a 256- or 512-wide net
         if (h->cluster_ok && (h->shape.n_streams > 1 || !h->fast_ok)) return 4;
         // kernel 3 only where kernel 2 or 4 fits too: a net too deep for kernel 2's shared memory (on an H100 from ~2 240
         // layers of 256 channels with 512 end channels and classes) keeps kernel 1, which auto has always run there
@@ -2948,15 +3061,20 @@ extern "C" int wn_gen_create(const wn_gen_shape* s, const wn_gen_weights* w, flo
     }
     // ---- batched cluster kernel (8 streams per cluster, tensor cores)
     {
+        // gen_kernel_cl8's carve: 8 exchanged vectors of W/16 blocks, staging, partials, fp32 inputs, barriers, layer
+        // table, then the weight ring (4 x 32 KB at W = 256; 2 x 32 KB at W = 512, where the vectors take 128 KB)
+        const int W = s->R;
         auto smem_for = [&](int vr) {
-            const size_t fixed = (size_t)8 * CL8_VEC + (size_t)2 * vr * CL8_BLK + sizeof(float) * (size_t)(2 * vr * 8 * 128 + 2 * 16 * vr * CL8_SB) +
-                                 16 * 8 + sizeof(GenLayer) * (size_t)s->n_layers + sizeof(int) * (size_t)(s->n_layers + 2 * CL8_SB);
-            return align_up(fixed, 16) + 4 * (size_t)CL8_IMG2;
+            const size_t fixed = (size_t)8 * (W / 16) * CL8_BLK + (size_t)2 * vr * CL8_BLK +
+                                 sizeof(float) * (size_t)(2 * vr * 8 * 128 + 2 * 16 * vr * CL8_SB) + 16 * 8 +
+                                 sizeof(GenLayer) * (size_t)s->n_layers + sizeof(int) * (size_t)(s->n_layers + 2 * CL8_SB);
+            return align_up(fixed, 16) + (W == 256 ? 4 : 2) * (size_t)32 * 1024;
         };
-        h->smem_cl8 = smem_for(1);
+        h->cl8_w = W;
+        h->smem_cl8 = smem_for(W / 16 / 16);
         h->smem_cl8_8 = smem_for(2);
         h->cl8_ok = cl8_shape_ok(*s) && h->smem_cl8 <= (size_t)smem_optin && !getenv("WN_GEN_NOCL8");
-        h->cl8_8_ok = h->cl8_ok && h->smem_cl8_8 <= (size_t)smem_optin;
+        h->cl8_8_ok = h->cl8_ok && W == 256 && h->smem_cl8_8 <= (size_t)smem_optin;
         h->cl8_packed = false;
         p.cl8_img = reinterpret_cast<const unsigned char*>(h->scratch + h->lay.cl8_img);
     }
@@ -2997,8 +3115,11 @@ extern "C" int wn_gen_reset(wn_gen_handle* h, void* stream) {
         h->tables_uploaded = true;
     }
     if (h->cl8_ok && !h->cl8_packed) {               // weights are constant for the life of a handle: split them once
-        cl8_pack_kernel<<<1184, 256, 0, st>>>(h->base.layers, h->shape.n_layers, h->base.e1w, h->base.e2w,
-                                             reinterpret_cast<unsigned*>(h->scratch + h->lay.cl8_img));
+        unsigned* img = reinterpret_cast<unsigned*>(h->scratch + h->lay.cl8_img);
+        if (h->cl8_w == 512)
+            cl8_pack_kernel<512><<<1184, 256, 0, st>>>(h->base.layers, h->shape.n_layers, h->base.e1w, h->base.e2w, img);
+        else
+            cl8_pack_kernel<256><<<1184, 256, 0, st>>>(h->base.layers, h->shape.n_layers, h->base.e1w, h->base.e2w, img);
         WN_CUDA(cudaGetLastError());
         h->cl8_packed = true;
     }
@@ -3181,26 +3302,29 @@ static int launch_gen_cluster(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     return 0;
 }
 
-template <int CS, bool COND, bool FRAMES, bool PS>
+template <int W, int CS, bool COND, bool FRAMES, bool PS>
 static int launch_gen_cl8_cs(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cl8_config(h, CS, st, &attr);
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<W, CS, COND, FRAMES, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)cfg.dynamicSmemBytes));
-    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<CS, COND, FRAMES, PS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    WN_CUDA(cudaFuncSetAttribute(gen_kernel_cl8<W, CS, COND, FRAMES, PS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     int max_clusters = 0;
-    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<CS, COND, FRAMES, PS>, &cfg));
+    WN_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, gen_kernel_cl8<W, CS, COND, FRAMES, PS>, &cfg));
     WN_REQUIRE(max_clusters >= 1, WN_E_UNSUPP, "wn_gen_run: a %d-CTA cluster cannot be scheduled on this device", CS);
-    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<CS, COND, FRAMES, PS>, p));   // clusters are independent: more than fit run in waves
+    WN_CUDA(cudaLaunchKernelEx(&cfg, gen_kernel_cl8<W, CS, COND, FRAMES, PS>, p));   // clusters are independent: more than fit run in waves
     return 0;
+}
+template <bool COND, bool FRAMES, bool PS>
+static int launch_gen_cl8_w(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
+    if (h->cl8_w == 512) return launch_gen_cl8_cs<512, 16, COND, FRAMES, PS>(h, p, st);
+    return h->cl8_cs == 16 ? launch_gen_cl8_cs<256, 16, COND, FRAMES, PS>(h, p, st) : launch_gen_cl8_cs<256, 8, COND, FRAMES, PS>(h, p, st);
 }
 template <bool PS>
 static int launch_gen_cl8_cond(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
-    if (p.cond && p.cond_hop)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, true, PS>(h, p, st) : launch_gen_cl8_cs<8, true, true, PS>(h, p, st);
-    if (p.cond)
-        return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, true, false, PS>(h, p, st) : launch_gen_cl8_cs<8, true, false, PS>(h, p, st);
-    return h->cl8_cs == 16 ? launch_gen_cl8_cs<16, false, false, PS>(h, p, st) : launch_gen_cl8_cs<8, false, false, PS>(h, p, st);
+    if (p.cond && p.cond_hop) return launch_gen_cl8_w<true, true, PS>(h, p, st);
+    if (p.cond) return launch_gen_cl8_w<true, false, PS>(h, p, st);
+    return launch_gen_cl8_w<false, false, PS>(h, p, st);
 }
 static int launch_gen_cl8(wn_gen_handle* h, GenParams& p, cudaStream_t st) {
     return p.ps ? launch_gen_cl8_cond<true>(h, p, st) : launch_gen_cl8_cond<false>(h, p, st);
@@ -3519,7 +3643,7 @@ extern "C" int wn_gen_run(wn_gen_handle* h, const wn_gen_run_args* a, void* stre
         WN_CUDA(cudaMemsetAsync(p.bar, 0, sizeof(unsigned), st));
         int rc;
         switch (kid) {
-        case 6:                                              // several streams of a 256-wide net: 8 streams per cluster
+        case 6:                                              // 256- or 512-wide nets: 8 streams per cluster
             rc = launch_gen_cl8(h, p, st);
             break;
         case 4:

@@ -1046,7 +1046,7 @@ class _Runtime:
     def reset_sampler(self, s, stream):
         lib = native.lib()
         native.check(lib.wn_gen_reset(s["handle"], stream), "gen reset")
-        mode = getattr(self, "gen_mode", None)            # None: library default (wn_gen_set_mode 0: the tensor-core cluster kernel for 256-wide nets)
+        mode = getattr(self, "gen_mode", None)            # None: library default (wn_gen_set_mode 0: the tensor-core cluster kernel for 256- and 512-wide nets)
         if mode is not None:
             native.check(lib.wn_gen_set_mode(s["handle"], int(mode)), "gen mode")
 
@@ -2250,9 +2250,10 @@ class WaveNetModel(nn.Module):
         """``n_streams`` independent generate_fast runs batched in one kernel (the reference has a single stream,
         wavenet_model.py:179).  first_samples: (n_streams, n_given) ints.  Returns int64 indices
         (n_streams, num_samples) [and the per-step logits].  Run through the same sampler kernel, stream s equals a
-        single-stream run bit for bit (256-wide nets run the tensor-core cluster kernel for any number of streams; other
-        nets a latency kernel for one stream and one thread-block cluster per stream otherwise, which differ at rounding
-        level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream.
+        single-stream run bit for bit (256- and 512-wide nets of 256 classes run the tensor-core cluster kernel for any
+        number of streams; on a 512-wide net every handle holds its own 6 MB of pre-split weight images per layer, about
+        505 MB at cfg 5; other nets a latency kernel for one stream and one thread-block cluster per stream otherwise,
+        which differ at rounding level).  condition: a conditioned model's labels (n_streams,) or vectors (n_streams, G), one per stream.
         local_condition: a locally conditioned model's (n_streams, C, F) series, one per stream (see generate_fast).
         top_k, top_p: the truncated draw of generate_fast.
 
